@@ -2,7 +2,7 @@
 """bench.py - image-pairs/sec on synthetic pairs (BASELINE.json configs 2-5; default config 2 = 480x640).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config 2|3|4|5]
-                    [--engine f16x3|fp32|f16|tf32] [--lanes L] [--pairs-per-step P]
+                    [--engine f16x3|fp32|f16|tf32] [--lanes L] [--pairs-per-step P] [--dump-outputs DIR]
 
 One "step" = P independent pairs per GPU (default 32, `config.pairs_per_gpu_per_step`), each through the whole hot path
 (variant-A CoarseAlign.setPair -> getCoarse -> warp_grid -> PredFlowMask).  Config 2: nbScale 7, scaleR 2, nbIter 1000, one
@@ -14,7 +14,8 @@ through the public API from pinned HOST images (H2D of the inputs + D2H of the r
 engine `f16x3` is the fp32-grade tensor-core engine (fp16 hi / lo split operands, 3 MMAs per MAC); `parity` reports how far
 that engine is from the CPU oracle on pair 0 of the workload (computed outside the timed region from the file the
 cpu_baseline child wrote).  `--impl reference` times the CPU oracle (oracle/pair_oracle.py: the reference's own PyTorch-CPU
-algorithm, all host threads) on the same workload.
+algorithm, all host threads) on the same workload.  `--dump-outputs DIR` writes what the device-resident timed region computed
+in its last step as DIR/<name>.npy (float32 / float64), so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -40,7 +41,7 @@ METRIC = "image-pairs/sec at 480x640, nbIter=1k RANSAC"
 NA, NB, CFEAT = 13065, 1200, 1024
 PARITY_RAW_SEED = 1000            # the raw sample table both arms reduce modulo their match count for the parity pair
 DTYPES = {"fp32": "f32", "tf32": "tf32",
-          "f16x3": "f32-grade: fp16 hi/lo split operands and activations (22 significand bits), 3 tcgen05 MMAs per MAC, fp32 accumulate; fp16-split correlation; fp32/fp64 RANSAC",
+          "f16x3": "f32-grade: fp16 hi/lo split operands and activations (22 significand bits), 3 wgmma MMAs per MAC, fp32 accumulate; fp16-split correlation; fp32/fp64 RANSAC",
           "f16": "f16 (reduced precision fast mode: conv operands and activations fp16, fp32 accumulate; TF32 output convs of the heads; fp16-split correlation; fp32/fp64 RANSAC)",
           "f16-trunk": "f16 trunk + tf32 fine-flow nets (reduced precision)"}
 
@@ -50,14 +51,14 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained"), src="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s; not reached, only the yardstick
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=None, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """SM clock and throttle reasons during the timed region (B200_PROFILING.md's clocks line).  Sampled in-process through
-    NVML - the library nvidia-smi itself reads - every 100 ms: spawning `nvidia-smi -lms 100` next to the bench perturbed the
-    first timed region (every other 32-pair step took 143 instead of 123 ms while nvidia-smi was starting up on the 8-GPU
-    box); the subprocess form is kept as the fallback when pynvml is missing."""
+    """SM clock and throttle reasons during the timed region.  Sampled in-process through NVML - the library nvidia-smi itself
+    reads - every 100 ms: a `nvidia-smi -lms 100` process started next to the bench perturbs the first timed region while it
+    starts up; the subprocess form is kept as the fallback when pynvml is missing."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
     NAMES = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -129,47 +130,27 @@ class ClockSampler:
                 "samples": len(sm), "source": "nvidia-smi -lms 100"}
 
 
-def ncu_facts(precision, v2):
-    """What the committed `ncu --set full` capture of the correlation kernel says (profiles/*.json, one launch at config 2):
-    DRAM bytes read + written, duration and tensor-pipe activity of the dominant launch.  {} when there is no capture."""
-    try:
-        pf = {1: "r1_corr_ncu.json", 2: "r2_ncu_full_kernels.json" if v2 else "r1_corr_f16_ncu.json"}[int(precision)]
-        prof = json.load(open(os.path.join(ROOT, "profiles", pf)))
-        l = [l for l in prof["launches"] if "tc_kernel" in l["kernel"] or "tc_corr_pipe" in l["kernel"]][0]
-        dur = l["gpu__time_duration.sum"]
-        us = float(dur["value"]) * {"ns": 1e-3, "us": 1.0, "ms": 1e3, "nsecond": 1e-3, "usecond": 1.0, "msecond": 1e3}.get(dur["unit"], 1.0)
-        return {"file": "profiles/" + pf, "traffic": l["dram_traffic_bytes"], "kernel_us": us,
-                "tensor_pct": float(l["sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active"]["value"])}
-    except Exception:  # noqa: BLE001
-        return {}
-
-
 def roofline_record(prec, v2, corr_ms, ransac_ms, n_matches, pk, presplit=False):
     """The `roofline` object of the JSON line for the kernel BASELINE.json names (correlation + mutual NN, plus RANSAC as
     us/call): algorithmic flops / bytes of config 2 (SURVEY 8d) over the call's measured time, against the measured peaks.
-    Pure arithmetic (tests/test_abi_and_host.py runs it without a GPU)."""
+    `traffic` is the algorithmic byte count.  Pure arithmetic (tests/test_abi_and_host.py runs it without a GPU)."""
     flops = 2.0 * NA * NB * CFEAT
     abytes = 4.0 * CFEAT * (NA + NB) + 16.0 * n_matches
     tf = flops / (corr_ms * 1e-3) / 1e12
     tensor_peak = pk["bf16_tflops"]
-    ncu = ncu_facts(prec, v2)              # DRAM traffic etc. of the dominant launch, from the committed ncu --set full capture
-    kname = {0: "corr_argmax_kernel (fp32 SIMT)", 1: "tc_kernel<128,MODE_CORR> (3xTF32 tcgen05)",
-             2: ("tc_corr_pipe_kernel (persistent, two TMEM accumulator pairs; " if v2 else "tc_kernel<128,MODE_CORR,f16> (")
-                + "fp16 split tcgen05: hi*hi + (hi*lo + lo*hi) * 2^-11)"}[prec]
-    # tensor work actually issued per algorithmic MAC: 3 MMAs either way; kind::tf32 runs at half the bf16/f16 rate
+    kname = {0: "corr_argmax_kernel (fp32 SIMT)", 1: "wg_kernel<K_TF32X3,128,MODE_CORR> (3xTF32 wgmma)",
+             2: "wg_kernel<K_SPLIT,128,MODE_CORR> (fp16 split wgmma: hi*hi + (hi*lo + lo*hi) * 2^-11)"}[prec]
+    # tensor work actually issued per algorithmic MAC: 3 MMAs either way; TF32 MMAs run at half the bf16/f16 rate
     rate = {0: None, 1: tensor_peak / 2, 2: tensor_peak}[prec]
     call = ("rf_corr_mutual_nn_presplit = key memset + %s + column-driven compaction (operand planes written by rf_l2norm_split_nhwc)" if presplit
             else "rf_corr_mutual_nn = %s + split/compaction helpers")
     return {"kernel": call % kname,
-            "bound": "tensor", "achieved": tf, "peak": tensor_peak, "unit": "TFLOP/s", "frac": tf / tensor_peak, "traffic": ncu.get("traffic"),
+            "bound": "tensor", "achieved": tf, "peak": tensor_peak, "unit": "TFLOP/s", "frac": tf / tensor_peak, "traffic": abytes,
             "peak_source": pk["src"] + " bf16 dense GEMM (burst); fp32-grade scores need 3 tensor MMAs per algorithmic MAC (split operands), "
                            "so the executed tensor fraction is 3 x frac for the fp16 split (6 x for 3xTF32, whose MMAs run at half rate)",
             "executed_tensor_frac": (3 * tf) / rate if rate else None,
             "ms_per_launch": corr_ms, "algorithmic_gflop": flops / 1e9, "algorithmic_mb": abytes / 1e6,
             "hbm_gbs_achieved": abytes / (corr_ms * 1e-3) / 1e9, "hbm_frac": abytes / (corr_ms * 1e-3) / 1e9 / pk["hbm_gbs"],
-            # the dominant kernel alone, from the committed capture (the live number above times the whole 3-launch call)
-            "ncu_capture": ncu.get("file"), "kernel_us_ncu": ncu.get("kernel_us"), "tensor_pipe_active_pct_ncu": ncu.get("tensor_pct"),
-            "executed_tensor_frac_kernel_ncu": (3 * flops / (ncu["kernel_us"] * 1e-6) / 1e12 / rate) if (rate and ncu.get("kernel_us")) else None,
             "ransac_us_per_call": 1e3 * ransac_ms, "ransac_matches": n_matches,
             "corr_plus_ransac_gbs": (abytes + 61e3) / ((corr_ms + ransac_ms) * 1e-3) / 1e9}
 
@@ -201,7 +182,7 @@ def pair_size(config):
 
 
 def make_pairs(n, config=2):
-    import synthdata as synth                        # workload generator (repo root); nothing under oracle/ on the B200 arm
+    import synthdata as synth                        # workload generator (repo root); nothing under oracle/ on the GPU arm
     h, w = pair_size(config)
     return [synth.make_pair(i, h, w)[:2] for i in range(n)]
 
@@ -221,7 +202,7 @@ def states():
 def run_reference(args, rank, world):
     """The reference's own algorithm on the host cores (oracle/pair_oracle.py, torch-CPU fp32).  With --dump-parity FILE it
     also runs pair 0 of the workload once more with the shared raw sample table and writes everything a parity check needs
-    (index lists, score matrix, matches, H, inlier mask, flows) to FILE: the B200 arm reads that FILE, never the oracle."""
+    (index lists, score matrix, matches, H, inlier mask, flows) to FILE: the GPU arm reads that FILE, never the oracle."""
     if rank != 0:
         return
     import PIL.Image as Image
@@ -329,7 +310,42 @@ def parity_report(rf, torch, ref, coarse, net, pair, engine, label="pair 0"):
     return rec
 
 
-# ----------------------------------------------------------------------------- B200 arm
+DUMP_LIMIT = 64 << 20          # bytes written by --dump-outputs at most
+
+
+def last_step_outputs(outs, live_flow12):
+    """Host copies of the per-pair results of one step, as {name: float32 / float64 array}.  Every pair's host-side results
+    (homographies, matchability map, /8 flow and matchability, counts); the full-resolution flow12 only for the last
+    `live_flow12` pairs, whose device buffers the graphs have not refilled yet.  Pairs in step order until DUMP_LIMIT."""
+    import torch
+    arrays, total = {}, 0
+    for k, o in enumerate(outs):
+        for key in sorted(o):
+            v = o[key]
+            if key == "flow12" and k < len(outs) - live_flow12:
+                continue
+            vals = v if isinstance(v, list) else [v]
+            for j, x in enumerate(vals):
+                if isinstance(x, torch.Tensor):
+                    x = x.detach().cpu().numpy()
+                a = np.asarray(x)
+                if a.dtype.kind not in "fiub" or a.size == 0:
+                    continue
+                a = a.astype(np.float64 if a.dtype in (np.float64, np.int64) else np.float32)
+                if total + a.nbytes > DUMP_LIMIT:
+                    continue
+                arrays["pair%02d_%s%s" % (k, key, "" if len(vals) == 1 else "_%d" % j)] = a
+                total += a.nbytes
+    return arrays
+
+
+def write_outputs(d, arrays):
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), a)
+
+
+# ----------------------------------------------------------------------------- GPU arm
 def run_b200(args, rank, world, local):
     import PIL.Image as Image
     import torch
@@ -337,7 +353,7 @@ def run_b200(args, rank, world, local):
     import ransac_flow_b200 as rf
     from ransac_flow_b200 import shard
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 arm has no CPU fallback (use --impl reference for the CPU oracle)")
+        raise SystemExit("bench.py: no CUDA device; the GPU arm has no CPU fallback (use --impl reference for the CPU oracle)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     cfg = args.config
@@ -424,6 +440,11 @@ def run_b200(args, rank, world, local):
         if world > 1:
             dist.barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        # restart the RANSAC sample streams (torch's default generator; the lanes' own generators), so that what a region
+        # computes depends on the arguments only, not on how many pre-warm steps ran before it
+        torch.manual_seed(1000)
+        if multi is not None:
+            multi.seed(1000)
         l0 = rf._lib.launch_count() + replayed()
         e0.record()
         recs = []
@@ -452,14 +473,11 @@ def run_b200(args, rank, world, local):
             tmax = torch.tensor([ms], device=dev)
             dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
             ms = float(tmax.item())
-        return ms, launches, outs[-1], allr, gather_ms
+        return ms, launches, outs, allr, gather_ms
 
     # set-up, untimed and before the W warm-up steps of the contract: a couple of seconds of the real load (clocks, power state,
-    # allocator).  Observation (profiles/README.md): with device-resident inputs every other 32-pair step takes ~139 instead of
-    # ~123 ms (per-step host timestamps), whatever the pre-warm (2 s, 6 s, a discarded dry-run region) and however the clocks are
-    # sampled, while the pinned-host-input region of the same process is flat: the resident path copies each pair device-to-device
-    # into the graph's static input buffers on the lane's stream, the host path uses the copy engines.  `value` is therefore ~4 %
-    # conservative against `e2e`.
+    # allocator).  The resident path copies each pair device-to-device into the graph's static input buffers on the lane's stream,
+    # the host path uses the copy engines.
     # (the clock sampler starts first: nvidia-smi's own start-up perturbs the GPU for about a second)
     sampler = ClockSampler(local)
     if rank == 0:
@@ -471,8 +489,10 @@ def run_b200(args, rank, world, local):
             step(i_pre, False)
             i_pre += 1
         torch.cuda.synchronize()
-    ms_dev, launches, out, _, _ = timed(False, args.steps, args.warmup)
-    ms_e2e, _, out, allr, gather_ms = timed(True, args.steps, max(1, args.warmup // 2))
+    ms_dev, launches, outs, _, _ = timed(False, args.steps, args.warmup)
+    dumped = last_step_outputs(outs, lanes if multi is not None else 1) if args.dump_outputs else None     # before the next region reuses the buffers
+    ms_e2e, _, outs, allr, gather_ms = timed(True, args.steps, max(1, args.warmup // 2))
+    out = outs[-1]
     clocks = sampler.stop() if rank == 0 else None
     assert allr.shape[0] == args.steps * P * world
     if os.environ.get("RF_BENCH_REPEAT_RESIDENT") and rank == 0 and world == 1:      # experiment: order dependence of the two timed regions
@@ -593,7 +613,7 @@ def run_b200(args, rank, world, local):
     if rank == 0 and roofline is not None:
         # the whole pair against the chip: 655 GFLOP of convolutions + correlation per pair (SURVEY 8d), x3 MMAs on the split
         # engine; ~8.4 GB of algorithmic HBM traffic per pair at 4 B per activation element, every layer reading its inputs and writing
-        # its output once (the fused conv3 + down-sampling GEMMs of the split engine move 1.1 GB less: profiles/r2_split_floor_analysis.txt)
+        # its output once
         pps = P * args.steps / (ms_dev * 1e-3)                      # this GPU's pairs/s
         mma = 3.0 if args.engine == "f16x3" else 1.0
         gb = 8.4 if args.engine in ("f16x3", "fp32", "tf32") else 4.3
@@ -611,7 +631,7 @@ def run_b200(args, rank, world, local):
             "dtype": DTYPES[args.engine], "data": "synthetic",
             "config": {"workload": WORKLOADS[cfg], "engine": args.engine, "pairs_per_gpu_per_step": P, "pairs_in_flight": lanes,
                        "parallelism": "pairs sharded i %% %d" % world,
-                       "l2": "256 MiB buffer written between steps (L2 flush); activations per pair also exceed the 126 MB L2",
+                       "l2": "256 MiB buffer written between steps (L2 flush); activations per pair also exceed the 50 MB L2",
                        "preprocessing": "LANCZOS pyramid on the GPU (bit-exact PIL emulation)" if cfg != 5 else "coarse pyramid on the GPU; the two fine-level resizes with PIL on the host like the script",
                        "launch": ("one CUDA graph per pair" + (", %d independent pairs in flight on %d streams" % (lanes, lanes) if lanes > 1 else ""))
                                  + (" (the whole maxCoarse = 10 loop inside the graph: acceptance test and mask update on the device)" if cfg == 4 else "")
@@ -622,6 +642,8 @@ def run_b200(args, rank, world, local):
             "all_gather_ms": round(gather_ms, 3), "hypotheses_last_pair": nH_mean,
         }
         print(json.dumps(line))
+        if dumped is not None:
+            write_outputs(args.dump_outputs, dumped)
 
 
 def main():
@@ -632,7 +654,7 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", type=int, default=int(os.environ.get("RF_CONFIG", "2")), choices=[2, 3, 4, 5], help="BASELINE.json configs[N-1]")
     ap.add_argument("--engine", default=os.environ.get("RF_ENGINE", "f16x3"), choices=["f16x3", "fp32", "tf32", "f16", "f16-trunk"],
-                    help="f16x3 (default): fp32-grade tcgen05 engine, fp16 hi/lo split operands, 3 MMAs per MAC; fp32: exact-FMA SIMT engine; "
+                    help="f16x3 (default): fp32-grade wgmma engine, fp16 hi/lo split operands, 3 MMAs per MAC; fp32: exact-FMA SIMT engine; "
                          "f16 / tf32 / f16-trunk: reduced-precision fast modes (10-bit operands)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--lanes", type=int, default=int(os.environ.get("RF_LANES", "4")),
@@ -641,6 +663,8 @@ def main():
                     help="pairs per GPU and step (default 32 for configs 2 / 3, 8 for config 4, 4 for config 5)")
     ap.add_argument("--no-graph", dest="graph", action="store_false", help="launch the kernels of a pair one by one instead of replaying a CUDA graph")
     ap.add_argument("--dump-parity", default=None, help="(reference arm) write the oracle's outputs for pair 0 to this .npz")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the outputs of the last device-resident timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.pairs_per_step <= 0:
         args.pairs_per_step = {2: 32, 3: 32, 4: 8, 5: 4}[args.config]

@@ -1,5 +1,5 @@
 /*
- * ransacflow_b200 - C ABI of the B200 (sm_100a) implementation of RANSAC-Flow's
+ * ransacflow_b200 - C ABI of the H100 (sm_90a) implementation of RANSAC-Flow's
  * per-pair inference hot path.
  *
  * The reference (XiSHEN0220/RANSAC-Flow) is pure Python on PyTorch: it has no
@@ -52,13 +52,12 @@ uint64_t rf_launch_count(void);
  * utils/outil.py:32-45 mutualMatching, fused: the NA x NB score matrix is never
  * written.  featA [NA][C], featB [NB][C] (K-major rows = one feature vector).
  * Outputs: idx1/idx2 (int64, capacity >= min(NA,NB)) sorted by idx1, *count.
- * precision: 0 = exact fp32 FMA (SIMT); 1 = 3xTF32 on tcgen05 tensor cores (hi*hi + lo*hi + hi*lo, C % 32 == 0);
- * 2 = fp16 split on tcgen05 (x = hi + lo * 2^-11 in fp16, cross terms in a second TMEM accumulator, C % 64 == 0): the
+ * precision: 0 = exact fp32 FMA (SIMT); 1 = 3xTF32 on wgmma tensor cores (hi*hi + lo*hi + hi*lo, C % 32 == 0);
+ * 2 = fp16 split on wgmma (x = hi + lo * 2^-11 in fp16, cross terms in a second accumulator, C % 64 == 0): the
  * same 22 significand bits with half the MMAs per channel.
- * Precision 2 has two kernel sequences with identical outputs (environment RF_CORR_V2, read per call): the persistent
- * correlation kernel (one CTA per SM, two TMEM accumulator pairs, arg-max epilogue overlapped with the next tile's
- * MMAs) between a fused split / key-zeroing launch and a fused mutual-test + compaction launch (3 launches), or the
- * one-tile-per-CTA kernel with separate helpers (6 launches).  rf_corr_mutual_nn_launches() (host only) tells which
+ * Precision 2 has two launch sequences around the same correlation kernel, with identical outputs (environment
+ * RF_CORR_V2, read per call): a fused split / key-zeroing launch and a fused mutual-test + compaction launch
+ * (3 launches), or separate helpers (6 launches).  rf_corr_mutual_nn_launches() (host only) tells which
  * one a call with this precision would run now: it returns the number of launches. */
 size_t rf_corr_mutual_nn_workspace(int NA, int NB, int C, int precision);
 int rf_corr_mutual_nn_launches(int precision);
@@ -68,7 +67,7 @@ int rf_corr_mutual_nn(const float* featA, int NA, const float* featB, int NB, in
 
 /* The same with operands their producer already split (rf_l2norm_split_nhwc writes the normalised rows as fp16 hi / lo * 2^11
  * planes): no split pass.  A_hi / A_lo [NA][C], B_hi / B_lo [NB][C] fp16, C % 64 == 0.  Three graph nodes: memset of the
- * arg-max keys, the persistent fp16-split tcgen05 kernel (precision 2 of rf_corr_mutual_nn, identical arithmetic), the
+ * arg-max keys, the fp16-split wgmma kernel (precision 2 of rf_corr_mutual_nn, identical arithmetic), the
  * column-driven mutual test + compaction. */
 size_t rf_corr_mutual_nn_presplit_workspace(int NA, int NB);
 int rf_corr_mutual_nn_presplit(const void* A_hi, const void* A_lo, int NA, const void* B_hi, const void* B_lo, int NB, int C,
@@ -116,10 +115,10 @@ int rf_build_matches(const int64_t* idx1, const int64_t* idx2, const int* count_
  * model/model.py:27-56,59-125,167-322; torchvision ResNet-50 bottlenecks.
  * x: ragged NHWC [sum HW][Cin]; w: [R*S*Cin][Cout] (tap-major, Cout contiguous);
  * bias [Cout] (nullable); residual: packed like y (nullable).
- * engine: 0 = fp32 SIMT implicit GEMM everywhere; 1 = TF32 tcgen05 implicit GEMM for the layers it
+ * engine: 0 = fp32 SIMT implicit GEMM everywhere; 1 = TF32 wgmma implicit GEMM for the layers it
  * supports (stride 1, Cin % 32 == 0, 1x1 / 3x3; w_tc = same weights as [Cout][R*S*Cin]), the exact-fp32
  * SIMT kernel for the rest (3-channel stems, stride-2 convs);
- * 2 = fp16 tcgen05 implicit GEMM: x, residual, y and w_tc ([Cout][R*S*Cin]) hold IEEE fp16 elements behind the
+ * 2 = fp16 wgmma implicit GEMM: x, residual, y and w_tc ([Cout][R*S*Cin]) hold IEEE fp16 elements behind the
  * same pointers (10-bit mantissa like TF32, half the HBM bytes, twice the tensor rate), fp32 accumulation and fp32
  * bias, outputs saturated to +-65504; needs Cin % 64 == 0, Cout % 8 == 0, 1x1 / 3x3, stride 1 / 2 and fails otherwise
  * (no fallback).  Used for the ResNet-50 conv4 trunk. */
@@ -128,9 +127,9 @@ int rf_build_matches(const int64_t* idx1, const int64_t* idx2, const int* count_
 #define RF_ENGINE_F16 2
 #define RF_ENGINE_F16_OUT32 3   /* engine 2 operands, fp32 output rounded to TF32 after ReLU (3x3 / stride 1 / no residual):
                                    the layer that hands over from fp16 activations to a TF32 layer */
-/* 4 = fp32-GRADE tcgen05 implicit GEMM ("f16x3"): every activation / weight element is carried as two fp16 values,
+/* 4 = fp32-GRADE wgmma implicit GEMM ("f16x3"): every activation / weight element is carried as two fp16 values,
  * v = hi + lo * 2^-11 (hi = fp16(v), lo = fp16((v - hi) * 2^11): 22 significand bits), and every MAC is three kind::f16 MMAs
- * (hi*hi | hi*lo + lo*hi in a second TMEM accumulator).  x, residual and y are SPLIT tensors behind the same pointers:
+ * (hi*hi | hi*lo + lo*hi in a second accumulator).  x, residual and y are SPLIT tensors behind the same pointers:
  * [2][sum HW][C] fp16, plane 0 = hi, plane 1 = lo * 2^11 (4 bytes per element like fp32); w_tc = [2][Cout][R*S*Cin] fp16,
  * split the same way.  fp32 accumulation, bias, residual add and ReLU; needs Cin % 64 == 0, Cout % 8 == 0, 1x1 / 3x3,
  * stride 1 / 2 (no fallback).  This is the engine whose features reproduce the reference's fp32 arg-max (match set).

@@ -1,4 +1,4 @@
-"""ransac_flow_b200: B200-native (sm_100a) implementation of RANSAC-Flow's per-pair inference
+"""ransac_flow_b200: H100-native (sm_90a) implementation of RANSAC-Flow's per-pair inference
 hot path behind the reference's own Python API (SURVEY.md section 8).
 
 Modules mirror the reference's module names: ``outil`` (utils/outil.py), ``model``

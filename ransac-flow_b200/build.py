@@ -1,8 +1,8 @@
-"""Build libransacflow_b200.so in-tree with nvcc for sm_100a (and the oracle helpers).
+"""Build libransacflow_b200.so in-tree with nvcc for sm_90a (H100).
 
     python ransac-flow_b200/build.py [--force]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the object files under build/ are build products (git-ignored).
 """
 import hashlib
 import os
@@ -12,8 +12,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libransacflow_b200.so")
-SOURCES = ["api.cu", "ransac.cu", "gemm_simt.cu", "gemm_tc.cu", "gemm_split.cu", "elementwise.cu", "runner.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+SOURCES = ["api.cu", "ransac.cu", "gemm_simt.cu", "gemm_tc.cu", "elementwise.cu", "runner.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

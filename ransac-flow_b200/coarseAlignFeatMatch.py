@@ -120,6 +120,7 @@ def scale_list(nbScale, scaleR):
 
 class _CoarseAlignBase:
     resize_mode = "min"
+    sample_generator = None               # getCoarse_device's RANSAC samples: torch's default CUDA generator unless set
 
     def _setup(self, nbScale, nbIter, tolerance, transform, minSize, scaleR, imageNet, segNet, resnet_state_dict, verbose):
         if not torch.cuda.is_available():
@@ -345,7 +346,7 @@ class CoarseAlignA(_CoarseAlignBase):
             if samples is not None:
                 raw, mode = torch.as_tensor(samples, dtype=torch.int64).to(match1.device).contiguous(), ops.SAMPLES_MOD
             else:
-                raw, mode = ops.philox_words(self.nbIter, self.nbPoint, match1.device), ops.SAMPLES_PHILOX64
+                raw, mode = ops.philox_words(self.nbIter, self.nbPoint, match1.device, self.sample_generator), ops.SAMPLES_PHILOX64
             H, nb, mask, status = ops.ransac_homography(match1, match2, raw, self.tolerance, 100, cnt, mode)
             return H, nb, mask, status, cnt
 

@@ -1,4 +1,4 @@
-// Shared helpers for the ransacflow_b200 CUDA library (sm_100a only).
+// Shared helpers for the ransacflow_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -53,7 +53,7 @@ inline int num_sms() {
     const int dev = current_device();
     if (n[dev] == 0) {
         cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-        if (n[dev] <= 0) n[dev] = 148;
+        if (n[dev] <= 0) n[dev] = 132;
     }
     return n[dev];
 }

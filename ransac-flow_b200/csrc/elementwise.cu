@@ -152,7 +152,7 @@ template <> struct Vec16<__half> {
     }
 };
 // engine 4: split tensors, two fp16 planes `plane` elements apart (x = hi + lo * 2^-11); values are rebuilt exactly in fp32,
-// results are split again (gemm_split.cu)
+// results are split again (gemm_tc.cu)
 struct SplitH {};
 __device__ __forceinline__ void split_store8(__half* p, long long plane, const float (&v)[8]) {
     uint4 th, tl;

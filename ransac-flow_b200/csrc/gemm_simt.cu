@@ -10,7 +10,7 @@
 // 8 x TN accumulators per thread, K-slices staged through shared memory
 // (transposed on the store so fragment reads are 128-bit and conflict free),
 // global loads of slice k+1 in flight while slice k is multiplied.
-// The tcgen05 tensor-core engine (gemm_tc.cu) replaces these where TF32 is allowed.
+// The wgmma tensor-core engine (gemm_tc.cu) replaces these where TF32 is allowed.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -514,7 +514,7 @@ using namespace rf;
 // tensor-core engines live in gemm_tc.cu
 int rf_corr_argmax_tc(const float* featA, int NA, const float* featB, int NB, int C,
                       unsigned long long* rowbest, unsigned long long* colbest, void* ws, cudaStream_t st, int precision, bool v2,
-                      const void* const* presplit = nullptr, void* const* tail = nullptr);
+                      const void* const* presplit = nullptr);
 int rf_corr_v2_mode();
 size_t rf_corr_tc_workspace(int NA, int NB, int C);
 int rf_conv2d_tc(const ImgSet& set, const ConvParams& p, const void* w_tc, cudaStream_t st, bool f16, bool out32);
@@ -532,7 +532,7 @@ extern "C" size_t rf_corr_mutual_nn_workspace(int NA, int NB, int C, int precisi
 }
 
 extern "C" int rf_corr_mutual_nn_launches(int precision) {
-    if (precision == 2 && rf_corr_v2_mode() != 0) return 3;          // split+zero, persistent correlation, flag+compact
+    if (precision == 2 && rf_corr_v2_mode() != 0) return 3;          // split+zero, correlation, flag+compact
     return precision == 0 ? 4 : 6;                                   // memset, [split, split,] correlation, flag, compact
 }
 
@@ -545,7 +545,7 @@ extern "C" int rf_corr_mutual_nn(const float* featA, int NA, const float* featB,
     cudaStream_t st = as_stream(stream);
     unsigned long long* rowbest = reinterpret_cast<unsigned long long*>(ws);
     unsigned long long* colbest = rowbest + NA;
-    // precision 2 with RF_CORR_V2: persistent correlation kernel; its split launch zeroes the keys, and the mutual test
+    // precision 2 with RF_CORR_V2: one split launch that also zeroes the keys, and the mutual test
     // and the compaction are one kernel (3 launches instead of 6)
     const bool v2 = precision == 2 && NA > 0 && NB > 0 && rf_corr_v2_mode() != 0;
     if (!v2) RF_CUDA(cudaMemsetAsync(ws, 0, ((size_t)NA + NB) * sizeof(unsigned long long), st));
@@ -571,7 +571,7 @@ extern "C" int rf_corr_mutual_nn(const float* featA, int NA, const float* featB,
 }
 
 // utils/outil.py:32-45 with operands the producer already split (rf_l2norm_split_nhwc: hi = fp16(x), lo = fp16((x - hi) * 2^11)):
-// memset of the keys, the persistent fp16-split correlation kernel, the column-driven compaction.  ws: (NA + NB) keys.
+// memset of the keys, the fp16-split correlation kernel, the column-driven compaction.  ws: (NA + NB) keys.
 extern "C" size_t rf_corr_mutual_nn_presplit_workspace(int NA, int NB) { return keys_bytes(NA, NB) + 256; }
 
 extern "C" int rf_corr_mutual_nn_presplit(const void* A_hi, const void* A_lo, int NA, const void* B_hi, const void* B_lo, int NB, int C,
@@ -581,20 +581,12 @@ extern "C" int rf_corr_mutual_nn_presplit(const void* A_hi, const void* A_lo, in
     cudaStream_t st = as_stream(stream);
     unsigned long long* rowbest = reinterpret_cast<unsigned long long*>(ws);
     unsigned long long* colbest = rowbest + NA;
-    RF_CUDA(cudaMemsetAsync(ws, 0, ((size_t)NA + NB + 1) * sizeof(unsigned long long), st));       // keys + the tail's ticket counter
+    RF_CUDA(cudaMemsetAsync(ws, 0, ((size_t)NA + NB) * sizeof(unsigned long long), st));
     if (NA == 0 || NB == 0) {
         RF_CUDA(cudaMemsetAsync(count_out, 0, sizeof(int), st));
         return 0;
     }
     const void* planes[4] = {A_hi, A_lo, B_hi, B_lo};
-    // RF_CORR_TAIL=1: mutual test + compaction in the correlation kernel's last CTA (2 graph nodes instead of 3).  Measured
-    // SLOWER at config 2 (92.3 vs 86.5 us per call: 192 threads of one CTA do serially what the 1024-thread kernel does
-    // while nothing else is left to overlap with), so the separate column-driven kernel stays the default.
-    const char* e = getenv("RF_CORR_TAIL");
-    if ((e ? atoi(e) : 0) && NA <= 49152) {
-        void* tail[4] = {idx1_out, idx2_out, count_out, colbest + NB};
-        return rf_corr_argmax_tc(nullptr, NA, nullptr, NB, C, rowbest, colbest, nullptr, st, 2, true, planes, tail);
-    }
     int rc = rf_corr_argmax_tc(nullptr, NA, nullptr, NB, C, rowbest, colbest, nullptr, st, 2, true, planes);
     if (rc) return rc;
     return launch_mutual_compact(rowbest, colbest, NA, NB, (long long*)idx1_out, (long long*)idx2_out, count_out, st);
@@ -617,15 +609,15 @@ extern "C" int rf_conv2d_nhwc(const float* x, int nimg, const int* hw_host, int 
     p.round_out = ((engine == RF_ENGINE_TF32 || engine == RF_ENGINE_F16_OUT32) && relu) ? 1 : 0;
     cudaStream_t st = as_stream(stream);
     RF_REQUIRE(engine >= RF_ENGINE_FP32 && engine <= RF_ENGINE_SPLIT_OUT32, "rf_conv2d_nhwc: unknown engine");
-    // engine 2 = tcgen05 with fp16 activations and weights (x, residual, y, w_tc hold IEEE halves); no SIMT fallback.
+    // engine 2 = wgmma with fp16 activations and weights (x, residual, y, w_tc hold IEEE halves); no SIMT fallback.
     // engine 3 = the same with an fp32 (TF32-rounded after ReLU) output: the hand-over to a TF32 layer
     if (engine == RF_ENGINE_F16) return rf_conv2d_tc(set, p, w_tc, st, true, false);
     if (engine == RF_ENGINE_F16_OUT32) return rf_conv2d_tc(set, p, w_tc, st, true, true);
-    // engine 4 = tcgen05 with fp16 hi / lo split operands (fp32-grade, gemm_split.cu): x, residual, y are split tensors
+    // engine 4 = wgmma with fp16 hi / lo split operands (fp32-grade, gemm_tc.cu): x, residual, y are split tensors
     // ([2][P][C] fp16), w_tc = [2][Cout][K] fp16.  engine 5 = the same with an fp32 [P][Cout] output (no residual)
     if (engine == RF_ENGINE_SPLIT) return rf_conv2d_split(set, p, w_tc, st, false);
     if (engine == RF_ENGINE_SPLIT_OUT32) return rf_conv2d_split(set, p, w_tc, st, true);
-    // engine 1 = tcgen05 TF32 where the layer shape allows it (stride 1, Cin % 32 == 0); other layers
+    // engine 1 = wgmma TF32 where the layer shape allows it (stride 1, Cin % 32 == 0); other layers
     // (3-channel stems, stride-2 convs, 49-channel heads) run on the exact-fp32 SIMT engine below
     if (engine == 1 && w_tc != nullptr && rf_conv2d_tc_supported(p)) return rf_conv2d_tc(set, p, w_tc, st, false, false);
     RF_REQUIRE(((uintptr_t)x % 16) == 0 && ((uintptr_t)w % 16) == 0 && ((uintptr_t)y % 16) == 0, "rf_conv2d_nhwc: pointers must be 16-byte aligned");

@@ -1,20 +1,19 @@
-// tcgen05 / TMEM / TMA tensor-core engine (sm_100a).
+// Tensor-core engine (sm_90a): implicit-GEMM convolutions and the correlation with its row / column arg-max, on wgmma.
 //
-// One warp-specialised kernel, two epilogues:
-//   MODE_CONV : implicit-GEMM convolution (stride 1) over a ragged NHWC batch, TF32 operands,
-//               fp32 accumulation in TMEM, epilogue = folded-BN bias + residual + ReLU
-//               (model/model.py:27-56,59-125,167-322; torchvision ResNet-50 conv1..layer3);
-//   MODE_CORR : utils/outil.py:34-37 score = featA^T featB as 3xTF32 (hi*hi + lo*hi + hi*lo, fp32-grade
-//               accuracy so the arg-max agrees with an fp32 GEMM) with the row / column arg-max fused
-//               into the epilogue; the NA x NB matrix never leaves the SM.
-//
-// Data path per CTA (one 128-pixel x BN-channel output tile):
-//   warp 0  : TMA producer.  A tile = 3-D box (32 channels, tw, th) of the NHWC image at the tap's
-//             offset (out-of-bounds = zero padding for free), B tile = 2-D box (32 k, BN rows) of the
-//             K-major weight matrix; both land in 128B-swizzled shared memory, mbarrier complete_tx.
-//   warp 1  : allocates TMEM, issues tcgen05.mma.kind::tf32 (M=128, N=BN, K=8) x4 per stage from one
-//             thread, tcgen05.commit releases the stage / publishes the accumulator.
-//   warps 2-5: epilogue, tcgen05.ld 32 lanes x 32 columns at a time straight from TMEM.
+// One kernel template.  A CTA computes one output tile of 128 pixels (correlation: 128 rows of featA) x BN channels (columns of
+// featB) with 288 threads:
+//   warp 8        : TMA producer.  A = box (channels, tw, th[, 2 planes]) of the NHWC image at the tap's offset (out-of-bounds
+//                   zero fill is the zero padding, the traversal stride is the convolution stride), B = box of the K-major
+//                   weight matrix; both 128-byte swizzled, completion counted on the stage's mbarrier.
+//   warpgroups 0-1: tile rows 0..63 / 64..127.  wgmma.mma_async from the stage's descriptors into register accumulators; one
+//                   wgmma group stays in flight while the stage before it is handed back to the producer.  The epilogue
+//                   works on the registers: bias, residual, ReLU, conversion, store (convolution) or arg-max keys (correlation).
+// Operand kinds:
+//   K_TF32   : fp32 operands, TF32 MMAs (engine 1);
+//   K_F16    : fp16 operands (engines 2 and 3);
+//   K_SPLIT  : every operand as two fp16 planes, x = hi + lo * 2^-11 (22 significand bits, engines 4 / 5 and correlation
+//              precision 2): main += hi*hi, cross += lo*hi + hi*lo at 2^11 scale, result = main + cross * 2^-11;
+//   K_TF32X3 : fp32 operands split into TF32 hi + lo (correlation precision 1): lo*hi + hi*lo + hi*hi into one accumulator.
 #include <cuda.h>
 #include <cuda_fp16.h>
 
@@ -27,241 +26,97 @@
 
 namespace rf {
 
-struct alignas(64) TcParams {
-    CUtensorMap mapA[RF_MAX_IMGS];        // per image: (C, W, H) fp32, box (32, tw, th)
-    CUtensorMap mapY[RF_MAX_IMGS];        // per image: output (Cout, Wo, Ho), box (32, tw, th)   [TMA-store epilogue]
-    CUtensorMap mapR[RF_MAX_IMGS];        // per image: residual, same geometry                   [TMA-load in the epilogue]
-    CUtensorMap mapAlo;                   // MODE_CORR: low part of A
-    CUtensorMap mapB;                     // (K, Cout) fp32, box (32, BN)
-    CUtensorMap mapBlo;                   // MODE_CORR: low part of B
+constexpr int K_TF32 = 0, K_F16 = 1, K_SPLIT = 2, K_TF32X3 = 3;
+constexpr int MODE_CONV = 0, MODE_CORR = 1;
+constexpr int O_F32 = 0, O_F16 = 1, O_SPLIT = 2;     // convolution output (and residual) formats
+constexpr int WG_THREADS = 288;                       // two consumer warpgroups + the producer warp
+
+struct alignas(64) WgParams {
+    CUtensorMap mapA[RF_MAX_IMGS];        // per image: input (C, W, H[, 2]); correlation: A hi (C, NA, 1)
+    CUtensorMap mapA2[RF_MAX_IMGS];       // dual-input 1x1: the second input (Cin2, W2, H2, 2); correlation: [0] = A lo
+    CUtensorMap mapB;                     // weights (K, Cout[, 2]); correlation: B hi (C, NB)
+    CUtensorMap mapBlo;                   // correlation: B lo
     int nimg;
-    int tile_start[RF_MAX_IMGS + 1];      // prefix sums of tiles per image
+    int tile_start[RF_MAX_IMGS + 1];      // prefix sums of pixel tiles per image
     int tiles_x[RF_MAX_IMGS];
     int tw[RF_MAX_IMGS];                  // tile width (tile height = 128 / tw)
     int Ho[RF_MAX_IMGS], Wo[RF_MAX_IMGS];
     long long out_pix[RF_MAX_IMGS + 1];
-    int R, S, pad, stride, Cin, Cout, relu, round_out, tma_epi;
-    int stages;                           // fp16 tap-streaming kernel: ring depth chosen per layer on the host
-    int res_pf;                           // fp16 tap-streaming kernel: residual tile prefetched into its own staging at CTA start
-    int raster_n;                         // convolutions: channel tiles fastest in the grid (CTAs of one pixel tile run together)
+    int R, S, pad, stride, Cin, Cout, relu, round_out;
+    int kc1, stride2;                     // dual-input 1x1: K blocks [0, kc1) come from mapA, the rest from mapA2 (sampled with stride2)
+    long long plane;                      // split output / residual: elements from the hi to the lo plane
     const float* bias;
-    const float* residual;
-    float* y;
-    unsigned long long* rowbest;          // MODE_CORR
+    const void* residual;
+    void* y;
+    unsigned long long* rowbest;          // correlation
     unsigned long long* colbest;
-    // tc_corr_pipe_kernel, optional fused tail: the last CTA to finish runs the mutual test + order-preserving compaction
-    unsigned int* done_counter;           // zeroed by the caller with the keys
-    long long* tail_idx1;                 // nullptr: no tail
-    long long* tail_idx2;
-    int* tail_count;
     int NA, NB;
 };
+static_assert(sizeof(WgParams) <= 32764, "kernel parameter space (CUDA 12.1+ large kernel parameters)");
 
-
-constexpr int MODE_CONV = 0, MODE_CORR = 1;
-
-// Convolution epilogue shared by the tap-streaming and the halo kernels (warps 2..5 = 128 threads, thread m owns
-// accumulator row m = pixel m of the tile): + folded-BN bias, + residual, ReLU, TF32 rounding, store.
-// fp16 epilogue core (engine 2): thread m's accumulator row -> + bias, + residual, ReLU, saturate -> fp16 into the
-// 128-byte-swizzled staging boxes (64 channels x 128 pixels x 2 B = 16 KB each; the residual boxes were TMA-loaded into
-// the same place).  32 accumulator columns = 64 bytes = four 16-byte chunks of the pixel's 128-byte row.
-template <int BN>
-__device__ __forceinline__ void epi_rows_f16(const float* __restrict__ bias, int Cout, int relu, bool has_res, int n0, int m,
-                                             uint32_t trow, uint8_t* stg) {
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld32(trow + c * 32, v);
-        const int n = n0 + c * 32;
-        uint8_t* rowp = stg + (c >> 1) * TC_A_BYTES + m * 128;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int chunk = (c & 1) * 4 + j;
-            uint4* sp = reinterpret_cast<uint4*>(rowp + ((chunk ^ (m & 7)) << 4));
-            float o[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) o[e] = __uint_as_float(v[8 * j + e]);
-            if (bias && n + 8 * j < Cout) {
-                const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + n + 8 * j));
-                const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias + n + 8 * j + 4));
-                o[0] += b0.x; o[1] += b0.y; o[2] += b0.z; o[3] += b0.w; o[4] += b1.x; o[5] += b1.y; o[6] += b1.z; o[7] += b1.w;
-            }
-            if (has_res) {
-                const uint4 rr = *sp;
-                const __half2* h = reinterpret_cast<const __half2*>(&rr);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) { const float2 f = __half22float2(h[e]); o[2 * e] += f.x; o[2 * e + 1] += f.y; }
-            }
-            if (relu) {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) o[e] = fmaxf(o[e], 0.f);
-            }
-            uint4 out;
-            __half2* ho = reinterpret_cast<__half2*>(&out);
-#pragma unroll
-            for (int e = 0; e < 4; ++e)         // saturate instead of overflowing to inf
-                ho[e] = __floats2half2_rn(fminf(fmaxf(o[2 * e], -65504.f), 65504.f), fminf(fmaxf(o[2 * e + 1], -65504.f), 65504.f));
-            *sp = out;
-        }
-    }
-}
-
-template <int BN, bool F16 = false>
-__device__ __forceinline__ void conv_epilogue(const TcParams& p, int img, int ox0, int oy0, int tw, int n0, int m, uint32_t trow,
-                                              uint8_t* smem, uint64_t* res_full, int warp, int lane, bool res_issued = false) {
-    if constexpr (F16) {
-        // engine 2: always the bulk path (the host requires Cout % 8 == 0); boxes of 64 fp16 channels.  `smem` is the
-        // staging area: the idle pipeline stages, or the dedicated residual staging when the producer warp already
-        // issued the residual loads at CTA start (res_issued)
-        constexpr int NBOX = BN / 64;
-        uint8_t* stg = smem;
-        const bool has_res = p.residual != nullptr;
-        if (has_res) {
-            if (!res_issued && warp == 2 && lane == 0) {
-                mbar_expect_tx(res_full, NBOX * TC_A_BYTES);
-#pragma unroll
-                for (int b = 0; b < NBOX; ++b) tma_load_3d(stg + b * TC_A_BYTES, &p.mapR[img], res_full, n0 + b * 64, ox0, oy0);
-            }
-            mbar_wait(res_full, 0);
-        }
-        epi_rows_f16<BN>(p.bias, p.Cout, p.relu, has_res, n0, m, trow, stg);
-        fence_proxy_async();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (warp == 2 && lane == 0) {
-#pragma unroll
-            for (int b = 0; b < NBOX; ++b)
-                if (n0 + b * 64 < p.Cout) tma_store_3d(&p.mapY[img], stg + b * TC_A_BYTES, n0 + b * 64, ox0, oy0);
-            tma_store_commit_and_wait_read();
-        }
-        return;
-    }
-    if (p.tma_epi) {
-        // ---- bulk epilogue: residual tile in by TMA, result tile out by TMA; the pipeline stages are idle now and
-        // serve as staging: BN/32 boxes of (32 channels x tw x th) = 128 rows x 128 B, 128-byte swizzled ----
-        uint8_t* stg = smem;
-        const bool has_res = p.residual != nullptr;
-        if (has_res) {
-            if (warp == 2 && lane == 0) {
-                mbar_expect_tx(res_full, (BN / 32) * TC_A_BYTES);
-#pragma unroll
-                for (int c = 0; c < BN / 32; ++c) tma_load_3d(stg + c * TC_A_BYTES, &p.mapR[img], res_full, n0 + c * 32, ox0, oy0);
-            }
-            mbar_wait(res_full, 0);
-        }
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld32(trow + c * 32, v);
-            const int n = n0 + c * 32;
-            uint8_t* rowp = stg + c * TC_A_BYTES + m * 128;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float4* sp = reinterpret_cast<float4*>(rowp + ((j ^ (m & 7)) << 4));
-                float4 o = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                if (p.bias && n + 4 * j < p.Cout) { float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n + 4 * j)); o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w; }
-                if (has_res) { float4 rr = *sp; o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w; }
-                if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                if (p.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                *sp = o;
-            }
-        }
-        fence_proxy_async();                        // generic-proxy smem writes -> visible to the TMA (async proxy)
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (warp == 2 && lane == 0) {
-#pragma unroll
-            for (int c = 0; c < BN / 32; ++c)
-                if (n0 + c * 32 < p.Cout) tma_store_3d(&p.mapY[img], stg + c * TC_A_BYTES, n0 + c * 32, ox0, oy0);
-            tma_store_commit_and_wait_read();       // smem must stay valid until the bulk stores have read it
-        }
-    } else {
-        const int py = m / tw, px = m - py * tw;
-        const int oy = oy0 + py, ox = ox0 + px;
-        const bool valid = (oy < p.Ho[img]) && (ox < p.Wo[img]);
-        const long long pix = p.out_pix[img] + (long long)oy * p.Wo[img] + ox;
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld32(trow + c * 32, v);
-            const int n = n0 + c * 32;
-            if (valid && n < p.Cout) {
-                float* dst = p.y + pix * p.Cout + n;
-                const float* res = p.residual ? p.residual + pix * p.Cout + n : nullptr;
-                if (n + 32 <= p.Cout && (p.Cout & 3) == 0) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-                        if (p.bias) { float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n + j)); o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w; }
-                        if (res) { float4 rr = __ldg(reinterpret_cast<const float4*>(res + j)); o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w; }
-                        if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                        if (p.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                        *reinterpret_cast<float4*>(dst + j) = o;
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (n + j < p.Cout) {
-                            float o = __uint_as_float(v[j]);
-                            if (p.bias) o += __ldg(p.bias + n + j);
-                            if (res) o += __ldg(res + j);
-                            if (p.relu) o = fmaxf(o, 0.f);
-                            if (p.round_out) o = round_tf32(o);
-                            dst[j] = o;
-                        }
-                }
-            }
-        }
-    }
-}
-
-
-template <int BN, int MODE, bool DEEP = false>
-struct TcCfg {
-    static constexpr int NSPLIT = (MODE == MODE_CORR) ? 2 : 1;
-    static constexpr int B_BYTES = BN * 128;
-    static constexpr int STAGE_BYTES = NSPLIT * (TC_A_BYTES + B_BYTES);
-    // three CTAs per SM (so one tile's epilogue / prologue overlaps the others' main loops): <= 73 KB of stages each;
-    // the 3xTF32 correlation needs 64 KB per stage and keeps one CTA per SM with 3 stages
-    // measured in sequence (profiles/): co-resident CTAs matter more than ring depth (one tile's prologue /
-    // epilogue hides behind the others' main loops, and the loop itself is L2->SM bandwidth bound).  K-deep layers
-    // (3x3, wide 1x1): 2 CTAs x 3 stages; short-K layers (1x1 expansions with residual): 3 CTAs x 2 stages
-    static constexpr int BUDGET = (MODE == MODE_CORR) ? 200 * 1024 : (DEEP ? 100 * 1024 : 73 * 1024);
-    static constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
-    static constexpr int CTAS_PER_SM = (MODE == MODE_CORR) ? 1 : (DEEP ? 2 : 3);
-    static constexpr int TMEM_COLS = BN <= 32 ? 32 : BN <= 64 ? 64 : BN <= 128 ? 128 : 256;
+template <int KIND, int BN, int MODE>
+struct WgCfg {
+    static constexpr int NPL = (KIND == K_SPLIT || KIND == K_TF32X3) ? 2 : 1;     // operand planes
+    static constexpr int A_BYTES = NPL * TC_A_BYTES;
+    static constexpr int B_PLANE = BN * 128;
+    static constexpr int STAGE_BYTES = A_BYTES + NPL * B_PLANE;
+    // two CTAs per SM (one tile's epilogue overlaps the other's main loop) where the stages and the accumulators allow it
+    static constexpr bool ONE_CTA = MODE == MODE_CORR || NPL * BN >= 256;
+    static constexpr int BUDGET = ONE_CTA ? 200 * 1024 : 100 * 1024;
+    static constexpr int STAGES = BUDGET / STAGE_BYTES > 6 ? 6 : BUDGET / STAGE_BYTES;
+    static constexpr int CTAS_PER_SM = ONE_CTA ? 1 : 2;
     static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static_assert(STAGES >= 2 && SMEM_BYTES <= 227 * 1024, "shared memory");
 };
 
-template <int BN, int MODE, bool DEEP, bool F16 = false>
-__global__ void __launch_bounds__(TC_THREADS, TcCfg<BN, MODE, DEEP>::CTAS_PER_SM)
-tc_kernel(const __grid_constant__ TcParams p) {
-    using Cfg = TcCfg<BN, MODE, DEEP>;
-    constexpr int STAGES = Cfg::STAGES, NSPLIT = Cfg::NSPLIT;
-    constexpr int BK = tc_bk<F16>();              // channels per 128-byte K block
-    constexpr bool CORR16 = F16 && MODE == MODE_CORR;                 // correlation with fp16-split operands: two accumulators
-    constexpr int TMEM_COLS = CORR16 ? 2 * Cfg::TMEM_COLS : Cfg::TMEM_COLS;
-    static_assert(TMEM_COLS <= 512, "TMEM");
-    // fp16 convolutions: ring depth per layer (<= STAGES) and, for layers with a residual, a dedicated staging area
-    // behind the ring that the producer fills at CTA start (more bytes in flight per SM, one DRAM latency less per CTA)
-    const int NST = (F16 && MODE == MODE_CONV) ? p.stages : STAGES;
-    const bool res_pf = F16 && MODE == MODE_CONV && p.res_pf;
-    constexpr int RES_BYTES = (BN / 64) * TC_A_BYTES;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic keeps the shared address space (LDS / STS, not generic LD / ST)
-    uint8_t* res_stg = smem + NST * Cfg::STAGE_BYTES;
-    uint64_t* full = reinterpret_cast<uint64_t*>(res_stg + (res_pf ? RES_BYTES : 0));
-    uint64_t* empty = full + STAGES;
-    uint64_t* tmem_full = empty + STAGES;
-    uint64_t* res_full = tmem_full + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_full + 1);
+// fp32 pair -> fp16 pair, saturating at +-65504 instead of overflowing to inf
+__device__ __forceinline__ __half2 pack_sat(float a, float b) {
+    uint32_t r;
+    asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));     // first source -> upper half
+    return *reinterpret_cast<__half2*>(&r);
+}
+// (a, b) -> hi = fp16(x), lo = fp16((x - hi) * 2^11), saturating like the fp16 engine
+__device__ __forceinline__ void split2(float a, float b, __half2& hi, __half2& lo) {
+    hi = pack_sat(a, b);
+    const float2 f = __half22float2(hi);
+    lo = pack_sat((a - f.x) * 2048.f, (b - f.y) * 2048.f);
+}
 
+// One K block (128 bytes of every operand row) of this warpgroup's 64 rows.
+template <int KIND, int BN, int NACC>
+__device__ __forceinline__ void mma_block(float (&acc)[NACC][BN / 2], uint32_t sa, uint32_t sb) {
+    constexpr bool TF32 = KIND == K_TF32 || KIND == K_TF32X3;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint64_t ah = wg_desc(sa + 32 * k), bh = wg_desc(sb + 32 * k);
+        if constexpr (KIND == K_SPLIT || KIND == K_TF32X3) {
+            const uint64_t al = wg_desc(sa + TC_A_BYTES + 32 * k), bl = wg_desc(sb + BN * 128 + 32 * k);
+            float (&x)[BN / 2] = acc[NACC - 1];
+            wgmma<TF32, BN>(x, al, bh);
+            wgmma<TF32, BN>(x, ah, bl);
+            wgmma<TF32, BN>(acc[0], ah, bh);
+        } else {
+            wgmma<TF32, BN>(acc[0], ah, bh);
+        }
+    }
+}
+
+template <int KIND, int BN, int MODE, int OUT>
+__global__ void __launch_bounds__(WG_THREADS, WgCfg<KIND, BN, MODE>::CTAS_PER_SM)
+wg_kernel(const __grid_constant__ WgParams p) {
+    using Cfg = WgCfg<KIND, BN, MODE>;
+    constexpr int STAGES = Cfg::STAGES;
+    constexpr int BK = (KIND == K_TF32 || KIND == K_TF32X3) ? TC_BK : TC_BK_F16;
+    constexpr int NACC = KIND == K_SPLIT ? 2 : 1;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint64_t* empty = full + STAGES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    // ---- tile decode ----
-    // conv: blockIdx.x = pixel tile, blockIdx.y = channel tile.  corr: swapped, so that the CTAs sharing one 128-row
-    // slab of featA (1 MB of hi+lo) are co-resident and the slab is fetched from DRAM once
-    const bool nfast = (MODE == MODE_CORR) || p.raster_n;
-    const int mtile = nfast ? blockIdx.y : blockIdx.x;
-    const int ntile = nfast ? blockIdx.x : blockIdx.y;
+    // ---- tile decode.  Correlation: column tiles fastest, so that the CTAs sharing a 128-row slab of featA run together ----
+    const int mtile = MODE == MODE_CORR ? blockIdx.y : blockIdx.x;
+    const int ntile = MODE == MODE_CORR ? blockIdx.x : blockIdx.y;
     int img = 0;
 #pragma unroll
     for (int j = 1; j < RF_MAX_IMGS; ++j) img += (j < p.nimg && mtile >= p.tile_start[j]) ? 1 : 0;
@@ -270,1142 +125,353 @@ tc_kernel(const __grid_constant__ TcParams p) {
     const int tyi = tloc / p.tiles_x[img], txi = tloc - tyi * p.tiles_x[img];
     const int ox0 = txi * tw, oy0 = tyi * th;
     const int n0 = ntile * BN;
-    const int kc = p.Cin / BK;                    // K blocks (32 fp32 / 64 fp16 channels) per tap
+    const int kc = p.Cin / BK;
     const int KI = p.R * p.S * kc;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < NST; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tmem_full, 1);
-        mbar_init(res_full, 1);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }
         fence_barrier_init();
     }
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&p.mapA[img]);
-        tma_prefetch_desc(&p.mapB);
-        if (NSPLIT == 2) { tma_prefetch_desc(&p.mapAlo); tma_prefetch_desc(&p.mapBlo); }
-    }
-    if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         // =============================== TMA producer ===============================
         if (lane == 0) {
+            tma_prefetch_desc(&p.mapA[img]);
+            tma_prefetch_desc(&p.mapB);
             for (int it = 0; it < KI; ++it) {
-                const int st = it % NST, ph = (it / NST) & 1;
+                const int st = it % STAGES, ph = (it / STAGES) & 1;
                 mbar_wait(&empty[st], ph ^ 1);
-                uint8_t* sbase = smem + st * Cfg::STAGE_BYTES;
+                uint8_t* sa = smem + st * Cfg::STAGE_BYTES;
+                uint8_t* sb = sa + Cfg::A_BYTES;
                 mbar_expect_tx(&full[st], Cfg::STAGE_BYTES);
-                const int tap = it / kc, cc = it - tap * kc;
-                const int r = tap / p.S, s = tap - r * p.S;
-                const int c0 = cc * BK, x = ox0 * p.stride + s - p.pad, y = oy0 * p.stride + r - p.pad;
-                const int kcol = tap * p.Cin + c0;
-                tma_load_3d(sbase, &p.mapA[img], &full[st], c0, x, y);
-                tma_load_2d(sbase + NSPLIT * TC_A_BYTES, &p.mapB, &full[st], kcol, n0);
-                if (NSPLIT == 2) {
-                    tma_load_3d(sbase + TC_A_BYTES, &p.mapAlo, &full[st], c0, x, y);
-                    tma_load_2d(sbase + 2 * TC_A_BYTES + Cfg::B_BYTES, &p.mapBlo, &full[st], kcol, n0);
-                }
-                if (F16 && it == 0 && res_pf) {       // right behind the first operand tiles: the residual tile
-                    mbar_expect_tx(res_full, RES_BYTES);
-#pragma unroll
-                    for (int b = 0; b < BN / 64; ++b) tma_load_3d(res_stg + b * TC_A_BYTES, &p.mapR[img], res_full, n0 + b * 64, ox0, oy0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // =============================== MMA issuer ===============================
-        {   // whole warp, warp-uniform control flow; umma_* elect the issuing lane
-            constexpr uint32_t idesc = make_idesc<F16>(BN);
-            for (int it = 0; it < KI; ++it) {
-                const int st = it % NST, ph = (it / NST) & 1;
-                mbar_wait(&full[st], ph);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
-                const uint32_t sb = sa + NSPLIT * TC_A_BYTES;
-                const uint64_t da = make_desc_sw128(sa), db = make_desc_sw128(sb);
-                if (CORR16) {
-                    umma_f16split_x4(tmem_base, tmem_base + BN, da, make_desc_sw128(sa + TC_A_BYTES), db, make_desc_sw128(sb + Cfg::B_BYTES), idesc, it != 0 ? 1u : 0u);
-                } else if (NSPLIT == 2) {
-                    umma_3xtf32_x4(tmem_base, da, make_desc_sw128(sa + TC_A_BYTES), db, make_desc_sw128(sb + Cfg::B_BYTES), idesc, it != 0 ? 1u : 0u);
-                } else {
-                    umma_x4<F16>(tmem_base, da, db, idesc, it != 0 ? 1u : 0u);      // 4 x (UMMA_K = 8 tf32 / 16 fp16 = 32 bytes)
-                }
-                umma_commit(&empty[st]);            // stage free once these MMAs have read it
-            }
-            umma_commit(tmem_full);                 // accumulator complete
-        }
-    } else {
-        // =============================== epilogue (warps 2..5) ===============================
-        const int q = warp & 3;                     // TMEM lane quarter this warp may access
-        const int m = q * 32 + lane;                // accumulator row = pixel inside the tile
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-        const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16);
-        if (MODE == MODE_CONV) {
-            conv_epilogue<BN, F16>(p, img, ox0, oy0, tw, n0, m, trow, res_pf ? res_stg : smem, res_full, warp, lane, res_pf);
-        } else {
-            // utils/outil.py:36-37: row arg-max (thread-local over this tile's columns), column arg-max via an
-            // smem transpose of the score tile (the pipeline stages are idle by now)
-            float* sS = reinterpret_cast<float*>(smem);
-            constexpr int LD = BN + 1;
-            const int row = ox0 + m;                // corr "image" is 1 x NA: tile = 128 consecutive rows of featA
-            const bool rvalid = row < p.NA;
-            unsigned long long best = 0ull;
-#pragma unroll 1
-            for (int c = 0; c < BN / 32; ++c) {
-                uint32_t v[32];
-                tmem_ld32(trow + c * 32, v);
-                if (CORR16) {                       // + the cross terms, accumulated at 2^11 scale in the second accumulator
-                    uint32_t x[32];
-                    tmem_ld32(trow + BN + c * 32, x);
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(fmaf(__uint_as_float(x[j]), 0.00048828125f, __uint_as_float(v[j])));
-                }
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int col = n0 + c * 32 + j;
-                    const float s = __uint_as_float(v[j]);
-                    sS[m * LD + c * 32 + j] = s;
-                    if (col < p.NB) {
-                        unsigned long long k = pack_key(s, (uint32_t)col);
-                        best = k > best ? k : best;
-                    }
-                }
-            }
-            if (rvalid && best != 0ull) atomicMax(p.rowbest + row, best);
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            const int t = (warp - 2) * 32 + lane;
-            const int rmax = min(128, p.NA - ox0);
-            for (int cidx = t; cidx < BN; cidx += 128) {
-                const int col = n0 + cidx;
-                if (col >= p.NB) continue;
-                unsigned long long cb = 0ull;
-                for (int rr = 0; rr < rmax; ++rr) {
-                    unsigned long long k = pack_key(sS[rr * LD + cidx], (uint32_t)(ox0 + rr));
-                    cb = k > cb ? k : cb;
-                }
-                if (cb != 0ull) atomicMax(p.colbest + col, cb);
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
-}
-
-
-// ------------------------------------------------------------------------------------------------------------
-// 3x3 / stride-1 convolutions with HALO REUSE.  The tap-streaming kernel above fetches the A tile nine times per
-// 32-channel chunk (once per tap, shifted by one pixel) and is bound by L2->SM operand bandwidth.  Here the CTA
-// owns an 8 x 16 pixel tile, loads its (8+2) x (16+2) halo ONCE per chunk (180 rows x 128 B, one TMA box) and the
-// nine taps are nine UMMA descriptors into the same shared memory: tap (r, s) starts (r*10 + s) rows into the halo
-// and its sixteen 8-row core groups are 10 rows (1280 B) apart - the descriptor's stride-byte-offset.  Two rings:
-// A (halo chunks) and B (one K-major weight tile per tap).
-// ------------------------------------------------------------------------------------------------------------
-constexpr int HALO_TW = 8, HALO_TH = 16;
-constexpr int HALO_LD = HALO_TW + 2;                                   // halo row pitch in pixels
-constexpr int HALO_A_BYTES = HALO_LD * (HALO_TH + 2) * 128;            // 23040
-constexpr int HALO_A_SLOT = 23 * 1024;                                 // 1024-byte aligned slot
-
-template <int BN>
-struct HaloCfg {
-    static constexpr int B_BYTES = BN * 128;
-    static constexpr int NA = 2;
-    static constexpr int NB = (BN == 128) ? 3 : 4;
-    static constexpr int RING_BYTES = NA * HALO_A_SLOT + NB * B_BYTES;
-    static constexpr int STG_BYTES = BN * 512;
-    static constexpr int DATA_BYTES = RING_BYTES > STG_BYTES ? RING_BYTES : STG_BYTES;
-    static constexpr int SMEM_BYTES = DATA_BYTES + 1024 + 256;
-    static constexpr int TMEM_COLS = BN <= 64 ? 64 : 128;
-};
-
-__device__ __forceinline__ uint64_t make_desc_halo(uint32_t saddr, int mode) {
-    uint64_t d = 0;
-    d |= (uint64_t)(saddr >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)((HALO_LD * 128) >> 4) << 32;                       // 8-row core groups are one halo row pitch apart
-    d |= (uint64_t)1 << 46;
-    // The start address is NOT 1024-byte aligned and the groups are 1280 B apart.  Measured on B200 (round 1): the
-    // 128-byte swizzle of tcgen05.mma is a pure function of the shared-memory address bits (it matches what the TMA
-    // wrote for any row phase) and the descriptor's base-offset field must stay 0; setting it to (addr >> 7) & 7, as the
-    // PTX text suggests for unaligned starts, double-applies the phase and gives wrong results.
-    (void)mode;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-
-// OUT32 (with F16): fp16 operands, fp32 output through the fp32 epilogue (the layer feeding a TF32 / fp32 consumer)
-template <int BN, bool F16 = false, bool OUT32 = false>
-__global__ void __launch_bounds__(TC_THREADS, 2)
-tc_halo_kernel(const __grid_constant__ TcParams p, int desc_mode) {
-    using Cfg = HaloCfg<BN>;
-    constexpr int NA = Cfg::NA, NB = Cfg::NB;
-    constexpr int BK = tc_bk<F16>();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic keeps the shared address space (LDS / STS, not generic LD / ST)
-    uint8_t* sA = smem;
-    uint8_t* sB = smem + NA * HALO_A_SLOT;
-    uint64_t* fullA = reinterpret_cast<uint64_t*>(smem + Cfg::DATA_BYTES);
-    uint64_t* emptyA = fullA + NA;
-    uint64_t* fullB = emptyA + NA;
-    uint64_t* emptyB = fullB + NB;
-    uint64_t* tmem_full = emptyB + NB;
-    uint64_t* res_full = tmem_full + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_full + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    int img = 0;
-#pragma unroll
-    for (int j = 1; j < RF_MAX_IMGS; ++j) img += (j < p.nimg && (int)blockIdx.x >= p.tile_start[j]) ? 1 : 0;
-    const int tloc = blockIdx.x - p.tile_start[img];
-    const int tyi = tloc / p.tiles_x[img], txi = tloc - tyi * p.tiles_x[img];
-    const int ox0 = txi * HALO_TW, oy0 = tyi * HALO_TH;
-    const int n0 = blockIdx.y * BN;
-    const int kc = p.Cin / BK;
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NA; ++i) { mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], 1); }
-        for (int i = 0; i < NB; ++i) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 1); }
-        mbar_init(tmem_full, 1);
-        mbar_init(res_full, 1);
-        fence_barrier_init();
-    }
-    if (warp == 0 && lane == 0) { tma_prefetch_desc(&p.mapA[img]); tma_prefetch_desc(&p.mapB); }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int ib = 0;
-            for (int cc = 0; cc < kc; ++cc) {
-                const int sa = cc % NA, pha = (cc / NA) & 1;
-                mbar_wait(&emptyA[sa], pha ^ 1);
-                mbar_expect_tx(&fullA[sa], HALO_A_BYTES);
-                tma_load_3d(sA + sa * HALO_A_SLOT, &p.mapA[img], &fullA[sa], cc * BK, ox0 - 1, oy0 - 1);
-                for (int tap = 0; tap < 9; ++tap, ++ib) {
-                    const int sb = ib % NB, phb = (ib / NB) & 1;
-                    mbar_wait(&emptyB[sb], phb ^ 1);
-                    mbar_expect_tx(&fullB[sb], Cfg::B_BYTES);
-                    tma_load_2d(sB + sb * Cfg::B_BYTES, &p.mapB, &fullB[sb], tap * p.Cin + cc * BK, n0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        {   // whole warp, warp-uniform control flow; umma_* elect the issuing lane
-            constexpr uint32_t idesc = make_idesc<F16>(BN);
-            int ib = 0;
-            for (int cc = 0; cc < kc; ++cc) {
-                const int sa = cc % NA, pha = (cc / NA) & 1;
-                mbar_wait(&fullA[sa], pha);
-                tc_fence_after();
-                const uint32_t abase = smem_u32(sA + sa * HALO_A_SLOT);
-                for (int tap = 0; tap < 9; ++tap, ++ib) {
-                    const int sb = ib % NB, phb = (ib / NB) & 1;
-                    mbar_wait(&fullB[sb], phb);
-                    tc_fence_after();
-                    const int r = tap / 3, sx = tap - r * 3;
-                    const uint32_t aaddr = abase + (uint32_t)((r * HALO_LD + sx) * 128);
-                    const uint64_t db = make_desc_sw128(smem_u32(sB + sb * Cfg::B_BYTES));
-                    umma_x4<F16>(tmem_base, make_desc_halo(aaddr, desc_mode), db, idesc, (cc | tap) != 0 ? 1u : 0u);
-                    umma_commit(&emptyB[sb]);
-                }
-                umma_commit(&emptyA[sa]);
-            }
-            umma_commit(tmem_full);
-        }
-    } else {
-        const int q = warp & 3;
-        const int m = q * 32 + lane;
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-        conv_epilogue<BN, F16 && !OUT32>(p, img, ox0, oy0, HALO_TW, n0, m, tmem_base + ((uint32_t)(q * 32) << 16), smem, res_full, warp, lane);
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-}
-
-
-// ------------------------------------------------------------------------------------------------------------
-// PERSISTENT convolution kernel: one CTA per SM walks a static list of tiles.  Most layers of this workload have a
-// short K loop (1x1 convs: 2-32 steps; 3x3 on 64 channels: 2 halo chunks), so a one-tile-per-CTA kernel spends its
-// life in prologue / TMA round-trip / epilogue latency.  Here the three roles run decoupled across tiles:
-//   warp 0   : TMA producer - keeps the A ring (tap tiles, or halo chunks when HALO) and the B ring (weight tiles)
-//              full, running ahead into the next tile while the current one is multiplied;
-//   warp 1   : MMA issuer - two TMEM accumulators (2 x BN columns): tile i+1 accumulates while tile i drains;
-//   warps 2-5: epilogue - TMEM -> (+bias, +residual, ReLU, TF32 round) -> swizzled smem staging -> TMA store, two
-//              staging buffers so the residual tile of tile i+1 is prefetched while tile i is being stored.
-// ------------------------------------------------------------------------------------------------------------
-template <int BN, bool HALO>
-struct PCfg {
-    static constexpr int A_SLOT = HALO ? HALO_A_SLOT : TC_A_BYTES;
-    static constexpr int A_TX = HALO ? HALO_A_BYTES : TC_A_BYTES;
-    static constexpr int B_BYTES = BN * 128;
-    static constexpr int NA = HALO ? 2 : (BN == 128 ? 3 : 4);
-    static constexpr int NB = HALO ? (BN == 128 ? 3 : 6) : NA;
-    static constexpr int STG = BN * 512;
-    static constexpr int OFF_B = NA * A_SLOT;
-    static constexpr int OFF_STG = OFF_B + NB * B_BYTES;
-    static constexpr int DATA_BYTES = OFF_STG + 2 * STG;
-    static constexpr int SMEM_BYTES = DATA_BYTES + 1024 + 512;
-    static constexpr int TMEM_COLS = 2 * BN;
-    static constexpr int TB = HALO ? 9 : 1;                 // B tiles consumed per A slot
-};
-
-
-struct TileCoord { int img, ox0, oy0, tw, n0; };
-
-template <bool HALO>
-__device__ __forceinline__ TileCoord decode_tile(const TcParams& p, int t, int tiles_m, int BN) {
-    TileCoord c;
-    int nt = t / tiles_m, mt = t - nt * tiles_m;            // pixel tiles fastest: co-running CTAs share the weight tile
-    if (p.raster_n) {                                       // channel tiles fastest: co-running CTAs share the pixel tile
-        const int tiles_n = (p.Cout + BN - 1) / BN;
-        mt = t / tiles_n;
-        nt = t - mt * tiles_n;
-    }
-    int img = 0;
-#pragma unroll
-    for (int j = 1; j < RF_MAX_IMGS; ++j) img += (j < p.nimg && mt >= p.tile_start[j]) ? 1 : 0;
-    const int tloc = mt - p.tile_start[img];
-    c.img = img;
-    c.tw = HALO ? HALO_TW : p.tw[img];
-    const int th = 128 / c.tw;
-    const int tyi = tloc / p.tiles_x[img], txi = tloc - tyi * p.tiles_x[img];
-    c.ox0 = txi * c.tw;
-    c.oy0 = tyi * th;
-    c.n0 = nt * BN;
-    return c;
-}
-
-template <int BN, bool HALO>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tc_persist_kernel(const __grid_constant__ TcParams p, int tiles_m, int tiles_n) {
-    using Cfg = PCfg<BN, HALO>;
-    constexpr int NA = Cfg::NA, NB = Cfg::NB, TB = Cfg::TB;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic keeps the shared address space (LDS / STS, not generic LD / ST)
-    uint8_t* sA = smem;
-    uint8_t* sB = smem + Cfg::OFF_B;
-    uint8_t* sStg = smem + Cfg::OFF_STG;
-    uint64_t* fullA = reinterpret_cast<uint64_t*>(smem + Cfg::DATA_BYTES);
-    uint64_t* emptyA = fullA + NA;
-    uint64_t* fullB = emptyA + NA;
-    uint64_t* emptyB = fullB + NB;
-    uint64_t* tmem_full = emptyB + NB;          // [2]
-    uint64_t* tmem_empty = tmem_full + 2;       // [2]
-    uint64_t* res_full = tmem_empty + 2;        // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_full + 2);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total = tiles_m * tiles_n;
-    const int kc = p.Cin / TC_BK;
-    const int NAI = HALO ? kc : p.R * p.S * kc;             // A slots per tile
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NA; ++i) { mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], 1); }
-        for (int i = 0; i < NB; ++i) { mbar_init(&fullB[i], 1); mbar_init(&emptyB[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 128); mbar_init(&res_full[i], 1); }
-        fence_barrier_init();
-    }
-    if (warp == 0 && lane == 0) { tma_prefetch_desc(&p.mapA[0]); tma_prefetch_desc(&p.mapB); tma_prefetch_desc(&p.mapY[0]); }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // =============================== TMA producer ===============================
-        if (lane == 0) {
-            uint32_t ia_cnt = 0, ib_cnt = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x) {
-                const TileCoord c = decode_tile<HALO>(p, t, tiles_m, BN);
-                for (int ia = 0; ia < NAI; ++ia, ++ia_cnt) {
-                    const int sa = ia_cnt % NA;
-                    mbar_wait(&emptyA[sa], ((ia_cnt / NA) & 1) ^ 1);
-                    mbar_expect_tx(&fullA[sa], Cfg::A_TX);
-                    int tap = 0, cc = ia;
-                    if (HALO) {
-                        tma_load_3d(sA + sa * Cfg::A_SLOT, &p.mapA[c.img], &fullA[sa], ia * TC_BK, c.ox0 - 1, c.oy0 - 1);
-                    } else {
-                        tap = ia / kc;
-                        cc = ia - tap * kc;
-                        const int r = tap / p.S, sx = tap - r * p.S;
-                        tma_load_3d(sA + sa * Cfg::A_SLOT, &p.mapA[c.img], &fullA[sa], cc * TC_BK, c.ox0 * p.stride + sx - p.pad,
-                                    c.oy0 * p.stride + r - p.pad);
-                    }
-                    for (int jb = 0; jb < TB; ++jb, ++ib_cnt) {
-                        const int sb = ib_cnt % NB;
-                        mbar_wait(&emptyB[sb], ((ib_cnt / NB) & 1) ^ 1);
-                        mbar_expect_tx(&fullB[sb], Cfg::B_BYTES);
-                        const int btap = HALO ? jb : tap;
-                        tma_load_2d(sB + sb * Cfg::B_BYTES, &p.mapB, &fullB[sb], btap * p.Cin + cc * TC_BK, c.n0);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // =============================== MMA issuer ===============================
-        {   // whole warp, warp-uniform control flow; umma_* elect the issuing lane
-            constexpr uint32_t idesc = make_idesc_tf32(BN);
-            uint32_t ia_cnt = 0, ib_cnt = 0, ti = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x, ++ti) {
-                const uint32_t buf = ti & 1;
-                mbar_wait(&tmem_empty[buf], ((ti >> 1) & 1) ^ 1);       // the epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t tacc = tmem_base + buf * BN;
-                for (int ia = 0; ia < NAI; ++ia, ++ia_cnt) {
-                    const int sa = ia_cnt % NA;
-                    mbar_wait(&fullA[sa], (ia_cnt / NA) & 1);
-                    tc_fence_after();
-                    const uint32_t abase = smem_u32(sA + sa * Cfg::A_SLOT);
-                    for (int jb = 0; jb < TB; ++jb, ++ib_cnt) {
-                        const int sb = ib_cnt % NB;
-                        mbar_wait(&fullB[sb], (ib_cnt / NB) & 1);
-                        tc_fence_after();
-                        const uint64_t db = make_desc_sw128(smem_u32(sB + sb * Cfg::B_BYTES));
-                        uint32_t aaddr = abase;
-                        if (HALO) { const int r = jb / 3, sx = jb - r * 3; aaddr += (uint32_t)((r * HALO_LD + sx) * 128); }
-                        umma_tf32_x4(tacc, HALO ? make_desc_halo(aaddr, 2) : make_desc_sw128(aaddr), db, idesc, (ia | jb) != 0 ? 1u : 0u);
-                        umma_commit(&emptyB[sb]);
-                    }
-                    umma_commit(&emptyA[sa]);
-                }
-                umma_commit(&tmem_full[buf]);
-            }
-        }
-    } else {
-        // =============================== epilogue (warps 2..5) ===============================
-        const int q = warp & 3;
-        const int m = q * 32 + lane;
-        const bool leader = (warp == 2 && lane == 0);
-        const bool has_res = p.residual != nullptr;
-        if (leader && has_res && (int)blockIdx.x < total) {
-            const TileCoord c = decode_tile<HALO>(p, blockIdx.x, tiles_m, BN);
-            mbar_expect_tx(&res_full[0], (BN / 32) * TC_A_BYTES);
-#pragma unroll
-            for (int cb = 0; cb < BN / 32; ++cb) tma_load_3d(sStg + cb * TC_A_BYTES, &p.mapR[c.img], &res_full[0], c.n0 + cb * 32, c.ox0, c.oy0);
-        }
-        uint32_t ti = 0;
-        for (int t = blockIdx.x; t < total; t += gridDim.x, ++ti) {
-            const uint32_t buf = ti & 1;
-            const TileCoord c = decode_tile<HALO>(p, t, tiles_m, BN);
-            uint8_t* stg = sStg + buf * Cfg::STG;
-            asm volatile("bar.sync 1, 128;" ::: "memory");           // the leader's bookkeeping of the previous tile is done
-            mbar_wait(&tmem_full[buf], (ti >> 1) & 1);
-            tc_fence_after();
-            if (has_res) mbar_wait(&res_full[buf], (ti >> 1) & 1);
-            const uint32_t trow = tmem_base + buf * BN + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-            for (int cb = 0; cb < BN / 32; ++cb) {
-                uint32_t v[32];
-                tmem_ld32(trow + cb * 32, v);
-                const int n = c.n0 + cb * 32;
-                uint8_t* rowp = stg + cb * TC_A_BYTES + m * 128;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    float4* sp = reinterpret_cast<float4*>(rowp + ((j ^ (m & 7)) << 4));
-                    float4 o = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                    if (p.bias && n + 4 * j < p.Cout) { float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n + 4 * j)); o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w; }
-                    if (has_res) { float4 rr = *sp; o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w; }
-                    if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                    if (p.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                    *sp = o;
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&tmem_empty[buf]);                            // accumulator drained (128 arrivals)
-            fence_proxy_async();
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (leader) {
-#pragma unroll
-                for (int cb = 0; cb < BN / 32; ++cb)
-                    if (c.n0 + cb * 32 < p.Cout) tma_store_3d(&p.mapY[c.img], stg + cb * TC_A_BYTES, c.n0 + cb * 32, c.ox0, c.oy0);
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");      // the other staging buffer has been read out
-                const int tn = t + gridDim.x;
-                if (has_res && tn < total) {
-                    const TileCoord cn = decode_tile<HALO>(p, tn, tiles_m, BN);
-                    uint8_t* stn = sStg + (buf ^ 1) * Cfg::STG;
-                    mbar_expect_tx(&res_full[buf ^ 1], (BN / 32) * TC_A_BYTES);
-#pragma unroll
-                    for (int cb = 0; cb < BN / 32; ++cb) tma_load_3d(stn + cb * TC_A_BYTES, &p.mapR[cn.img], &res_full[buf ^ 1], cn.n0 + cb * 32, cn.ox0, cn.oy0);
-                }
-            }
-        }
-        if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-}
-
-
-// ------------------------------------------------------------------------------------------------------------
-// 3x3 / stride-1 / 64 -> 64 channel convolutions (ResNet-50 layer1 conv2, FeatureExtractor layer1): K is only two
-// 32-channel chunks, so a tile is ~1.2 us of MMA work and one-tile CTAs live mostly in launch / TMA / epilogue
-// latency.  All 18 weight tiles (9 taps x 2 chunks x 8 KB = 144 KB) fit in shared memory: this persistent kernel loads
-// them ONCE per CTA, then streams halo tiles (2 x 23 KB) through a two-slot ring while two TMEM accumulators let the
-// epilogue of tile i overlap the MMAs of tile i+1.  Per tile only the 46 KB halo crosses L2->SM.
-// ------------------------------------------------------------------------------------------------------------
-// fp16 (engine 2): 64 channels are ONE 128-byte K block, so the weights are 72 KB and the halo ring gets four slots
-template <bool F16>
-struct ResBCfg {
-    static constexpr int BN = 64, KC = F16 ? 1 : 2, NTAP = 9, NA = F16 ? 4 : 2;
-    static constexpr int B_TILE = BN * 128;                                 // 8 KB
-    static constexpr int B_BYTES = KC * NTAP * B_TILE;                      // 144 KB (72 KB fp16)
-    static constexpr int OFF_A = B_BYTES;
-    static constexpr int OFF_STG = OFF_A + NA * HALO_A_SLOT;
-    static constexpr int STG = F16 ? BN * 256 : BN * 512;                   // 32 KB (16 KB fp16)
-    static constexpr int DATA_BYTES = OFF_STG + STG;
-    static constexpr int SMEM_BYTES = DATA_BYTES + 1024 + 256;
-    static constexpr int TMEM_COLS = 128;                                   // two 64-column accumulators
-};
-
-template <bool F16 = false>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tc_resb_kernel(const __grid_constant__ TcParams p, int tiles_m) {
-    using Cfg = ResBCfg<F16>;
-    constexpr int BN = Cfg::BN, NA = Cfg::NA;
-    constexpr int BK = tc_bk<F16>();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic keeps the shared address space (LDS / STS, not generic LD / ST)
-    uint8_t* sB = smem;
-    uint8_t* sA = smem + Cfg::OFF_A;
-    uint8_t* sStg = smem + Cfg::OFF_STG;
-    uint64_t* fullA = reinterpret_cast<uint64_t*>(smem + Cfg::DATA_BYTES);
-    uint64_t* emptyA = fullA + NA;
-    uint64_t* fullB = emptyA + NA;              // [1]
-    uint64_t* tmem_full = fullB + 1;            // [2]
-    uint64_t* tmem_empty = tmem_full + 2;       // [2]
-    uint64_t* res_full = tmem_empty + 2;        // [1]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(res_full + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total = tiles_m;                  // Cout = 64: a single channel tile
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NA; ++i) { mbar_init(&fullA[i], 1); mbar_init(&emptyA[i], 1); }
-        mbar_init(fullB, 1);
-        for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 128); }
-        mbar_init(res_full, 1);
-        fence_barrier_init();
-    }
-    if (warp == 0 && lane == 0) { tma_prefetch_desc(&p.mapA[0]); tma_prefetch_desc(&p.mapB); tma_prefetch_desc(&p.mapY[0]); }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            // the whole weight set, once: tile (cc, tap) at sB + (cc * 9 + tap) * 8 KB
-            mbar_expect_tx(fullB, Cfg::B_BYTES);
-            for (int cc = 0; cc < Cfg::KC; ++cc)
-                for (int tap = 0; tap < Cfg::NTAP; ++tap)
-                    tma_load_2d(sB + (cc * Cfg::NTAP + tap) * Cfg::B_TILE, &p.mapB, fullB, tap * p.Cin + cc * BK, 0);
-            uint32_t ia = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x) {
-                const TileCoord c = decode_tile<true>(p, t, tiles_m, BN);
-                for (int cc = 0; cc < Cfg::KC; ++cc, ++ia) {
-                    const int sa = ia % NA;
-                    mbar_wait(&emptyA[sa], ((ia / NA) & 1) ^ 1);
-                    mbar_expect_tx(&fullA[sa], HALO_A_BYTES);
-                    tma_load_3d(sA + sa * HALO_A_SLOT, &p.mapA[c.img], &fullA[sa], cc * BK, c.ox0 - 1, c.oy0 - 1);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        {   // whole warp, warp-uniform control flow; umma_* elect the issuing lane
-            constexpr uint32_t idesc = make_idesc<F16>(BN);
-            mbar_wait(fullB, 0);
-            tc_fence_after();
-            uint32_t ia = 0, ti = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x, ++ti) {
-                const uint32_t buf = ti & 1;
-                mbar_wait(&tmem_empty[buf], ((ti >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t tacc = tmem_base + buf * BN;
-                for (int cc = 0; cc < Cfg::KC; ++cc, ++ia) {
-                    const int sa = ia % NA;
-                    mbar_wait(&fullA[sa], (ia / NA) & 1);
-                    tc_fence_after();
-                    const uint32_t abase = smem_u32(sA + sa * HALO_A_SLOT);
-#pragma unroll
-                    for (int tap = 0; tap < Cfg::NTAP; ++tap) {
-                        const int r = tap / 3, sx = tap - r * 3;
-                        const uint32_t aaddr = abase + (uint32_t)((r * HALO_LD + sx) * 128);
-                        const uint64_t db = make_desc_sw128(smem_u32(sB + (cc * Cfg::NTAP + tap) * Cfg::B_TILE));
-                        umma_x4<F16>(tacc, make_desc_halo(aaddr, 2), db, idesc, (cc | tap) != 0 ? 1u : 0u);
-                    }
-                    umma_commit(&emptyA[sa]);
-                }
-                umma_commit(&tmem_full[buf]);
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int m = q * 32 + lane;
-        const bool leader = (warp == 2 && lane == 0);
-        const bool has_res = p.residual != nullptr;
-        constexpr int NBOX = Cfg::STG / TC_A_BYTES;                 // staging boxes of 128 bytes per pixel: 2 (fp32) / 1 (fp16)
-        uint32_t ti = 0;
-        for (int t = blockIdx.x; t < total; t += gridDim.x, ++ti) {
-            const uint32_t buf = ti & 1;
-            const TileCoord c = decode_tile<true>(p, t, tiles_m, BN);
-            if (leader) {
-                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");          // staging buffer has been read out
-                if (has_res) {
-                    mbar_expect_tx(res_full, NBOX * TC_A_BYTES);
-#pragma unroll
-                    for (int cb = 0; cb < NBOX; ++cb) tma_load_3d(sStg + cb * TC_A_BYTES, &p.mapR[c.img], res_full, cb * BK, c.ox0, c.oy0);
-                }
-            }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            mbar_wait(&tmem_full[buf], (ti >> 1) & 1);
-            tc_fence_after();
-            if (has_res) mbar_wait(res_full, ti & 1);
-            const uint32_t trow = tmem_base + buf * BN + ((uint32_t)(q * 32) << 16);
-            if constexpr (F16) epi_rows_f16<BN>(p.bias, p.Cout, p.relu, has_res, 0, m, trow, sStg);
-#pragma unroll 1
-            for (int cb = 0; cb < (F16 ? 0 : BN / 32); ++cb) {
-                uint32_t v[32];
-                tmem_ld32(trow + cb * 32, v);
-                const int n = cb * 32;
-                uint8_t* rowp = sStg + cb * TC_A_BYTES + m * 128;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    float4* sp = reinterpret_cast<float4*>(rowp + ((j ^ (m & 7)) << 4));
-                    float4 o = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]), __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                    if (p.bias) { float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n + 4 * j)); o.x += b.x; o.y += b.y; o.z += b.z; o.w += b.w; }
-                    if (has_res) { float4 rr = *sp; o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w; }
-                    if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                    if (p.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                    *sp = o;
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&tmem_empty[buf]);
-            fence_proxy_async();
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            if (leader) {
-#pragma unroll
-                for (int cb = 0; cb < NBOX; ++cb) tma_store_3d(&p.mapY[c.img], sStg + cb * TC_A_BYTES, cb * BK, c.ox0, c.oy0);
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-        }
-        if (leader) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// PIPELINED persistent fp16 convolution (tap streaming: 1x1 of any stride, 3x3 / stride 2).  ncu on the one-tile-per-CTA
-// kernel (profiles/r1_f16_layers_ncu.json) shows every such layer latency bound - DRAM <= 55 %, L2 <= 32 %, tensor
-// pipe <= 28 %, a CTA lives ~10 us for ~1 us of work: operand load -> MMA -> residual load -> epilogue -> store drain
-// are serial inside a CTA and at most four CTAs fit an SM.  Here one CTA per SM software-pipelines tiles:
-//   warp 0     : TMA producer - residual tile of tile i (into staging buffer i & 1, as soon as the store of tile i-2
-//                has read it out) and the K blocks of tile i into an NS-deep ring; runs ahead across tiles;
-//   warp 1     : MMA issuer - accumulator i & 1 of two, so tile i+1 multiplies while tile i drains;
-//   warps 2-5  : epilogue group 0 (even tiles), warps 6-9: epilogue group 1 (odd tiles) - TMEM -> + bias, + residual,
-//                ReLU -> fp16 swizzled staging -> TMA store; two groups so that two epilogues overlap.
-// ------------------------------------------------------------------------------------------------------------
-template <int BN>
-struct PipeCfg {
-    static constexpr int B_BYTES = BN * 128;
-    static constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
-    static constexpr int NS = BN == 128 ? 4 : 6;
-    static constexpr int STG = (BN / 64) * TC_A_BYTES;                      // fp16 staging: BN / 64 boxes of 16 KB
-    static constexpr int OFF_STG = NS * STAGE_BYTES;
-    static constexpr int DATA_BYTES = OFF_STG + 2 * STG;
-    static constexpr int SMEM_BYTES = DATA_BYTES + 1024 + 512;
-    static constexpr int TMEM_COLS = 2 * BN;
-    static constexpr int THREADS = 320;
-};
-
-template <int BN>
-__global__ void __launch_bounds__(PipeCfg<BN>::THREADS, 1)
-tc_pipe_kernel(const __grid_constant__ TcParams p, int tiles_m, int tiles_n) {
-    using Cfg = PipeCfg<BN>;
-    constexpr int NS = Cfg::NS, NBOX = BN / 64, BK = TC_BK_F16;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic keeps the shared address space (LDS / STS, not generic LD / ST)
-    uint8_t* sStg = smem + Cfg::OFF_STG;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::DATA_BYTES);
-    uint64_t* empty = full + NS;
-    uint64_t* tmem_full = empty + NS;           // [2]
-    uint64_t* tmem_empty = tmem_full + 2;       // [2] 128 arrivals
-    uint64_t* res_full = tmem_empty + 2;        // [2]
-    uint64_t* stg_free = res_full + 2;          // [2] the group's leader: the TMA store has read the staging buffer
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(stg_free + 2);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total = tiles_m * tiles_n;
-    const int kc = p.Cin / BK;
-    const int KI = p.R * p.S * kc;
-    const bool has_res = p.residual != nullptr;
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NS; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 128); mbar_init(&res_full[i], 1); mbar_init(&stg_free[i], 1); }
-        fence_barrier_init();
-    }
-    if (warp == 0 && lane == 0) { tma_prefetch_desc(&p.mapA[0]); tma_prefetch_desc(&p.mapB); tma_prefetch_desc(&p.mapY[0]); }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // =============================== TMA producer ===============================
-        if (lane == 0) {
-            uint32_t cnt = 0, ti = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x, ++ti) {
-                const TileCoord c = decode_tile<false>(p, t, tiles_m, BN);
-                if (has_res) {
-                    const uint32_t g = ti & 1;
-                    mbar_wait(&stg_free[g], ((ti >> 1) & 1) ^ 1);        // tile ti-2's store has read this buffer (passes at once for ti < 2)
-                    mbar_expect_tx(&res_full[g], Cfg::STG);
-#pragma unroll
-                    for (int b = 0; b < NBOX; ++b)
-                        tma_load_3d(sStg + g * Cfg::STG + b * TC_A_BYTES, &p.mapR[c.img], &res_full[g], c.n0 + b * 64, c.ox0, c.oy0);
-                }
-                for (int it = 0; it < KI; ++it, ++cnt) {
-                    const int st = cnt % NS;
-                    mbar_wait(&empty[st], ((cnt / NS) & 1) ^ 1);
-                    uint8_t* sbase = smem + st * Cfg::STAGE_BYTES;
-                    mbar_expect_tx(&full[st], Cfg::STAGE_BYTES);
-                    const int tap = it / kc, cc = it - tap * kc;
-                    const int r = tap / p.S, sx = tap - r * p.S;
-                    tma_load_3d(sbase, &p.mapA[c.img], &full[st], cc * BK, c.ox0 * p.stride + sx - p.pad, c.oy0 * p.stride + r - p.pad);
-                    tma_load_2d(sbase + TC_A_BYTES, &p.mapB, &full[st], tap * p.Cin + cc * BK, c.n0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // =============================== MMA issuer (whole warp, warp-uniform) ===============================
-        constexpr uint32_t idesc = make_idesc_f16(BN);
-        uint32_t cnt = 0, ti = 0;
-        for (int t = blockIdx.x; t < total; t += gridDim.x, ++ti) {
-            const uint32_t buf = ti & 1;
-            mbar_wait(&tmem_empty[buf], ((ti >> 1) & 1) ^ 1);               // the epilogue has drained this accumulator
-            tc_fence_after();
-            const uint32_t tacc = tmem_base + buf * BN;
-            for (int it = 0; it < KI; ++it, ++cnt) {
-                const int st = cnt % NS;
-                mbar_wait(&full[st], (cnt / NS) & 1);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
-                umma_f16_x4(tacc, make_desc_sw128(sa), make_desc_sw128(sa + TC_A_BYTES), idesc, it != 0 ? 1u : 0u);
-                umma_commit(&empty[st]);
-            }
-            umma_commit(&tmem_full[buf]);
-        }
-    } else {
-        // =============================== epilogue groups ===============================
-        const uint32_t g = (uint32_t)(warp - 2) >> 2;                       // 0: warps 2-5, 1: warps 6-9
-        const int q = warp & 3;                                             // TMEM lane quarter this warp may access
-        const int m = q * 32 + lane;
-        const bool leader = ((warp - 2) & 3) == 0 && lane == 0;
-        uint8_t* stg = sStg + g * Cfg::STG;
-        uint32_t k = 0;                                                     // this group's tile counter
-        for (int t = blockIdx.x + (int)g * (int)gridDim.x; t < total; t += 2 * gridDim.x, ++k) {
-            const TileCoord c = decode_tile<false>(p, t, tiles_m, BN);
-            // the leader comes here only after the previous store has read the staging buffer
-            if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-            mbar_wait(&tmem_full[g], k & 1);
-            tc_fence_after();
-            if (has_res) mbar_wait(&res_full[g], k & 1);
-            const uint32_t trow = tmem_base + g * BN + ((uint32_t)(q * 32) << 16);
-            epi_rows_f16<BN>(p.bias, p.Cout, p.relu, has_res, c.n0, m, trow, stg);
-            tc_fence_before();
-            mbar_arrive(&tmem_empty[g]);                                    // accumulator drained (128 arrivals)
-            fence_proxy_async();
-            if (g == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
-            if (leader) {
-#pragma unroll
-                for (int b = 0; b < NBOX; ++b)
-                    if (c.n0 + b * 64 < p.Cout) tma_store_3d(&p.mapY[c.img], stg + b * TC_A_BYTES, c.n0 + b * 64, c.ox0, c.oy0);
-                tma_store_commit_and_wait_read();
-                if (has_res) mbar_arrive(&stg_free[g]);
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// PERSISTENT correlation + mutual-NN kernel (utils/outil.py:34-37, precision 2 = fp16 split).  ncu on the
-// one-tile-per-CTA kernel (profiles/r1_corr_f16_ncu.json): 17.8 us per 128 x 128 score tile for 6.3 us of MMAs - one
-// CTA per SM (192 KB of stages), so TMEM allocation, the first TMA round trip and the whole arg-max epilogue are
-// serial with the K loop.  Here one CTA per SM walks its tiles (N-tiles fastest: the CTAs sharing a featA slab run
-// together) with the three roles decoupled:
-//   warp 0    : TMA producer, 3-stage ring of (A hi, A lo, B hi, B lo) K blocks, runs ahead into the next tile;
-//   warp 1    : MMA issuer, TWO accumulator pairs (hi*hi | cross terms) x 128 columns = all 512 TMEM columns: tile
-//               i+1 multiplies while tile i drains;
-//   warps 2-5 : epilogue.  Row arg-max thread-local straight from TMEM; column arg-max 32 columns at a time through
-//               a 128 x 33 float transposition buffer of its own (the stages are busy), four row quarters combined
-//               through 1 KB of keys, one atomicMax per column and per row of the tile as before.
-// Same arithmetic per score as tc_kernel<128, MODE_CORR, false, true> (same MMAs in the same order, same fma of the
-// cross-term accumulator), same (score, smallest index) ordering => identical match lists.
-// ------------------------------------------------------------------------------------------------------------
-struct CorrPipeCfg {
-    static constexpr int BN = 128;
-    static constexpr int B_BYTES = BN * 128;
-    static constexpr int STAGE_BYTES = 2 * (TC_A_BYTES + B_BYTES);            // 64 KB
-    static constexpr int NS = 3;
-    static constexpr int LD = 33;                                             // transposition pitch: conflict-free both ways
-    static constexpr int OFF_T = NS * STAGE_BYTES;
-    static constexpr int T_BYTES = 128 * LD * 4;
-    static constexpr int OFF_P = OFF_T + T_BYTES;
-    static constexpr int P_BYTES = 4 * 32 * 8;
-    static constexpr int DATA_BYTES = OFF_P + P_BYTES;
-    static constexpr int SMEM_BYTES = DATA_BYTES + 1024 + 256;
-    static constexpr int TMEM_COLS = 512;
-};
-static_assert(CorrPipeCfg::SMEM_BYTES <= 227 * 1024, "shared memory");
-static_assert((CorrPipeCfg::OFF_P % 8) == 0 && (CorrPipeCfg::DATA_BYTES % 8) == 0, "alignment");
-
-
-__device__ __forceinline__ unsigned long long pack_ord(uint32_t ord, uint32_t idx) {
-    return ((unsigned long long)ord << 32) | (unsigned long long)(0xFFFFFFFFu - idx);
-}
-
-__global__ void __launch_bounds__(TC_THREADS, 1)
-tc_corr_pipe_kernel(const __grid_constant__ TcParams p, int tiles_m, int tiles_n) {
-    using Cfg = CorrPipeCfg;
-    constexpr int NS = Cfg::NS, BN = Cfg::BN, BK = TC_BK_F16, LD = Cfg::LD;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic keeps the shared address space (LDS / STS, not generic LD / ST)
-    float* sT = reinterpret_cast<float*>(smem + Cfg::OFF_T);
-    unsigned long long* sP = reinterpret_cast<unsigned long long*>(smem + Cfg::OFF_P);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::DATA_BYTES);
-    uint64_t* empty = full + NS;
-    uint64_t* tmem_full = empty + NS;           // [2]
-    uint64_t* tmem_empty = tmem_full + 2;       // [2] 128 arrivals
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int total = tiles_m * tiles_n;
-    const int KI = p.Cin / BK;
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < NS; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 128); }
-        fence_barrier_init();
-    }
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&p.mapA[0]); tma_prefetch_desc(&p.mapAlo); tma_prefetch_desc(&p.mapB); tma_prefetch_desc(&p.mapBlo);
-    }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // =============================== TMA producer ===============================
-        if (lane == 0) {
-            uint32_t cnt = 0;
-            for (int t = blockIdx.x; t < total; t += gridDim.x) {
-                const int mt = t / tiles_n, nt = t - mt * tiles_n;
-                const int row0 = mt * 128, n0 = nt * BN;
-                for (int it = 0; it < KI; ++it, ++cnt) {
-                    const int st = cnt % NS;
-                    mbar_wait(&empty[st], ((cnt / NS) & 1) ^ 1);
-                    uint8_t* sbase = smem + st * Cfg::STAGE_BYTES;
-                    mbar_expect_tx(&full[st], Cfg::STAGE_BYTES);
+                if constexpr (MODE == MODE_CORR) {
                     const int c0 = it * BK;
-                    tma_load_3d(sbase, &p.mapA[0], &full[st], c0, row0, 0);
-                    tma_load_2d(sbase + 2 * TC_A_BYTES, &p.mapB, &full[st], c0, n0);
-                    tma_load_3d(sbase + TC_A_BYTES, &p.mapAlo, &full[st], c0, row0, 0);
-                    tma_load_2d(sbase + 2 * TC_A_BYTES + Cfg::B_BYTES, &p.mapBlo, &full[st], c0, n0);
+                    tma_load_3d(sa, &p.mapA[0], &full[st], c0, ox0, 0);
+                    tma_load_3d(sa + TC_A_BYTES, &p.mapA2[0], &full[st], c0, ox0, 0);
+                    tma_load_2d(sb, &p.mapB, &full[st], c0, n0);
+                    tma_load_2d(sb + Cfg::B_PLANE, &p.mapBlo, &full[st], c0, n0);
+                } else {
+                    const int tap = it / kc, cc = it - tap * kc;
+                    const int r = tap / p.S, s = tap - r * p.S;
+                    const int c0 = cc * BK, x = ox0 * p.stride + s - p.pad, y = oy0 * p.stride + r - p.pad;
+                    const int kcol = tap * p.Cin + c0;
+                    if constexpr (KIND == K_SPLIT) {       // one 4-D box brings [hi tile | lo tile]
+                        if (cc < p.kc1) tma_load_4d(sa, &p.mapA[img], &full[st], c0, x, y, 0);
+                        else tma_load_4d(sa, &p.mapA2[img], &full[st], (cc - p.kc1) * BK, ox0 * p.stride2, oy0 * p.stride2, 0);
+                        tma_load_3d(sb, &p.mapB, &full[st], kcol, n0, 0);
+                    } else {
+                        tma_load_3d(sa, &p.mapA[img], &full[st], c0, x, y);
+                        tma_load_2d(sb, &p.mapB, &full[st], kcol, n0);
+                    }
                 }
             }
         }
-    } else if (warp == 1) {
-        // =============================== MMA issuer (whole warp, warp-uniform) ===============================
-        constexpr uint32_t idesc = make_idesc_f16(BN);
-        uint32_t cnt = 0, ti = 0;
-        for (int t = blockIdx.x; t < total; t += gridDim.x, ++ti) {
-            const uint32_t buf = ti & 1;
-            mbar_wait(&tmem_empty[buf], ((ti >> 1) & 1) ^ 1);               // the epilogue has drained this accumulator pair
-            tc_fence_after();
-            const uint32_t td = tmem_base + buf * (2 * BN), tx = td + BN;
-            for (int it = 0; it < KI; ++it, ++cnt) {
-                const int st = cnt % NS;
-                mbar_wait(&full[st], (cnt / NS) & 1);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
-                const uint32_t sb = sa + 2 * TC_A_BYTES;
-                if (p.stages == 3)      // RF_CORR_MMA3=1: three N = 128 instructions per K step (the first version; A/B timing)
-                    umma_f16split_x4(td, tx, make_desc_sw128(sa), make_desc_sw128(sa + TC_A_BYTES), make_desc_sw128(sb),
-                                     make_desc_sw128(sb + Cfg::B_BYTES), idesc, it != 0 ? 1u : 0u);
-                else                    // [B hi | B lo] are adjacent in the stage, [main | cross] in TMEM: one N = 256 instruction + A lo x B hi
-                    umma_f16split2_x4(td, BN, make_desc_sw128(sa), make_desc_sw128(sa + TC_A_BYTES), make_desc_sw128(sb),
-                                      make_idesc_f16(2 * BN), idesc, it != 0 ? 1u : 0u);
-                umma_commit(&empty[st]);
+        return;
+    }
+
+    // =============================== consumers: warpgroup g owns tile rows 64g .. 64g + 63 ===============================
+    const int g = warp >> 2;
+    float acc[NACC][BN / 2];
+#pragma unroll
+    for (int a = 0; a < NACC; ++a)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[a][i] = 0.f;
+    for (int it = 0; it < KI; ++it) {
+        const int st = it % STAGES, ph = (it / STAGES) & 1;
+        mbar_wait(&full[st], ph);
+        const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
+        wg_fence();
+        mma_block<KIND, BN, NACC>(acc, sa + g * (64 * 128), sa + Cfg::A_BYTES);
+        wg_commit();
+        wg_wait<1>();                             // the previous stage's MMAs are done: hand it back
+        if (it > 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+    }
+    wg_wait<0>();
+#pragma unroll
+    for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
+
+    // accumulator fragment: d[4j + 2h + e] = row 16 * (warp % 4) + lane / 4 + 8h, column 8j + 2 * (lane % 4) + e
+    const int rbase = 64 * g + 16 * (warp & 3) + (lane >> 2);
+    const int cbase = 2 * (lane & 3);
+    auto value = [&](int i) -> float {
+        if constexpr (KIND == K_SPLIT) return fmaf(acc[1][i], 0.00048828125f, acc[0][i]);
+        else return acc[0][i];
+    };
+
+    if constexpr (MODE == MODE_CONV) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int m = rbase + 8 * h;
+            const int py = m / tw, px = m - py * tw;
+            const int oy = oy0 + py, ox = ox0 + px;
+            if (oy >= p.Ho[img] || ox >= p.Wo[img]) continue;
+            const long long pix = p.out_pix[img] + (long long)oy * p.Wo[img] + ox;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int n = n0 + 8 * j + cbase;
+                if (n >= p.Cout) continue;
+                const bool two = n + 1 < p.Cout;
+                float v0 = value(4 * j + 2 * h), v1 = value(4 * j + 2 * h + 1);
+                if (p.bias) { v0 += __ldg(p.bias + n); if (two) v1 += __ldg(p.bias + n + 1); }
+                const long long o = pix * p.Cout + n;
+                if (p.residual) {
+                    if constexpr (OUT == O_F32) {
+                        const float* r = static_cast<const float*>(p.residual) + o;
+                        v0 += __ldg(r); if (two) v1 += __ldg(r + 1);
+                    } else if constexpr (OUT == O_F16) {
+                        const float2 r = __half22float2(*reinterpret_cast<const __half2*>(static_cast<const __half*>(p.residual) + o));
+                        v0 += r.x; v1 += r.y;
+                    } else {
+                        const __half* r = static_cast<const __half*>(p.residual) + o;
+                        const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(r));
+                        const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(r + p.plane));
+                        v0 += fmaf(rl.x, 0.00048828125f, rh.x); v1 += fmaf(rl.y, 0.00048828125f, rh.y);
+                    }
+                }
+                if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                if constexpr (OUT == O_F32) {
+                    if (p.round_out) { v0 = round_tf32(v0); v1 = round_tf32(v1); }
+                    float* y = static_cast<float*>(p.y) + o;
+                    if (two && (p.Cout & 1) == 0) *reinterpret_cast<float2*>(y) = make_float2(v0, v1);
+                    else { y[0] = v0; if (two) y[1] = v1; }
+                } else if constexpr (OUT == O_F16) {
+                    *reinterpret_cast<__half2*>(static_cast<__half*>(p.y) + o) = pack_sat(v0, v1);
+                } else {
+                    __half2 hi, lo;
+                    split2(v0, v1, hi, lo);
+                    __half* y = static_cast<__half*>(p.y) + o;
+                    *reinterpret_cast<__half2*>(y) = hi;
+                    *reinterpret_cast<__half2*>(y + p.plane) = lo;
+                }
             }
-            umma_commit(&tmem_full[buf]);
         }
     } else {
-        // =============================== epilogue (warps 2..5) ===============================
-        const int q = warp & 3;                     // TMEM lane quarter this warp may access
-        const int m = q * 32 + lane;                // accumulator row = featA row inside the tile
-        const int tid = (warp - 2) * 32 + lane;     // 0..127 for the column pass
-        const int cj = tid & 31, qq = tid >> 5;
-        uint32_t ti = 0;
-        for (int t = blockIdx.x; t < total; t += gridDim.x, ++ti) {
-            const uint32_t buf = ti & 1;
-            const int mt = t / tiles_n, nt = t - mt * tiles_n;
-            const int row0 = mt * 128, n0 = nt * BN;
-            const int rmax = min(128, p.NA - row0);
-            mbar_wait(&tmem_full[buf], (ti >> 1) & 1);
-            tc_fence_after();
-            const uint32_t trow = tmem_base + buf * (2 * BN) + ((uint32_t)(q * 32) << 16);
-            uint32_t rbo = 0u, rbi = 0u;            // row best: ordered score (0 = none yet), column
-#pragma unroll 1
-            for (int c = 0; c < BN / 32; ++c) {
-                uint32_t v[32], x[32];
-                tmem_ld32x2(trow + c * 32, v, trow + BN + c * 32, x);
-                if (c == BN / 32 - 1) {             // last TMEM read of this tile: hand the accumulators back
-                    tc_fence_before();
-                    mbar_arrive(&tmem_empty[buf]);
-                }
-                const int colbase = n0 + c * 32;
+        // utils/outil.py:36-37: per row the best (score, smallest column) key, per column the best (score, smallest row) key.
+        // Rows: the four lanes of a quad share a row.  Columns: the eight row groups of a warp by shuffles, then the eight
+        // warps through shared memory (the stages are idle: every TMA load has been consumed).
+        unsigned long long* sCol = reinterpret_cast<unsigned long long*>(smem);       // [8 warps][BN]
+        const int row0 = ox0 + rbase, row1 = row0 + 8;
+        const bool rv0 = row0 < p.NA, rv1 = row1 < p.NA;
+        unsigned long long rb0 = 0ull, rb1 = 0ull;
+        asm volatile("bar.sync 1, 256;" ::: "memory");          // both warpgroups are past their last wgmma reads
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float s = fmaf(__uint_as_float(x[j]), 0.00048828125f, __uint_as_float(v[j]));     // + cross terms * 2^-11
-                    sT[m * LD + j] = s;
-                    const uint32_t o = f2ord(s);
-                    if (colbase + j < p.NB && o > rbo) { rbo = o; rbi = (uint32_t)(colbase + j); }
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int c = 8 * j + cbase + e, col = n0 + c;
+                const bool cv = col < p.NB;
+                const float s0 = value(4 * j + e), s1 = value(4 * j + 2 + e);
+                unsigned long long ck = 0ull;
+                if (cv) {
+                    if (rv0) { const unsigned long long k = pack_key(s0, (uint32_t)col); rb0 = k > rb0 ? k : rb0; ck = pack_key(s0, (uint32_t)row0); }
+                    if (rv1) { const unsigned long long k = pack_key(s1, (uint32_t)col); rb1 = k > rb1 ? k : rb1;
+                               const unsigned long long k1 = pack_key(s1, (uint32_t)row1); ck = k1 > ck ? k1 : ck; }
                 }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                // column arg-max of this 128 x 32 block: thread (qq, cj) scans rows qq*32 .. +31 of column cj
-                uint32_t cbo = 0u, cbi = 0u;
-#pragma unroll 8
-                for (int rr = 0; rr < 32; ++rr) {
-                    const int r = qq * 32 + rr;
-                    const uint32_t o = f2ord(sT[r * LD + cj]);
-                    if (r < rmax && o > cbo) { cbo = o; cbi = (uint32_t)(row0 + r); }
+#pragma unroll
+                for (int off = 4; off < 32; off <<= 1) {
+                    const unsigned long long o = __shfl_xor_sync(0xffffffffu, ck, off);
+                    ck = o > ck ? o : ck;
                 }
-                sP[qq * 32 + cj] = cbo ? pack_ord(cbo, cbi) : 0ull;
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                if (tid < 32) {
-                    unsigned long long k0 = sP[tid], k1 = sP[32 + tid], k2 = sP[64 + tid], k3 = sP[96 + tid];
-                    k0 = k1 > k0 ? k1 : k0;
-                    k2 = k3 > k2 ? k3 : k2;
-                    k0 = k2 > k0 ? k2 : k0;
-                    if (colbase + tid < p.NB && k0 != 0ull) atomicMax(p.colbest + colbase + tid, k0);
-                }
+                if (lane < 4) sCol[warp * BN + c] = ck;
             }
-            if (m < rmax && rbo != 0u) atomicMax(p.rowbest + row0 + m, pack_ord(rbo, rbi));
+        }
+#pragma unroll
+        for (int off = 1; off < 4; off <<= 1) {
+            const unsigned long long o0 = __shfl_xor_sync(0xffffffffu, rb0, off), o1 = __shfl_xor_sync(0xffffffffu, rb1, off);
+            rb0 = o0 > rb0 ? o0 : rb0;
+            rb1 = o1 > rb1 ? o1 : rb1;
+        }
+        if ((lane & 3) == 0) {
+            if (rv0 && rb0 != 0ull) atomicMax(p.rowbest + row0, rb0);
+            if (rv1 && rb1 != 0ull) atomicMax(p.rowbest + row1, rb1);
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        for (int c = threadIdx.x; c < BN; c += 256) {
+            if (n0 + c >= p.NB) continue;
+            unsigned long long cb = 0ull;
+#pragma unroll
+            for (int w = 0; w < 8; ++w) { const unsigned long long k = sCol[w * BN + c]; cb = k > cb ? k : cb; }
+            if (cb != 0ull) atomicMax(p.colbest + n0 + c, cb);
         }
     }
-    tc_fence_before();
-    if (p.tail_idx1 != nullptr) __threadfence();                // this thread's arg-max atomics are performed before the ticket below
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-    if (p.tail_idx1 == nullptr) return;
-    // ---- fused tail: utils/outil.py:38-43 (mutual test, S*S > 0, nonzero() order) by the LAST CTA to finish, on the idle ring.
-    // Same algorithm as mutual_cols_compact_kernel (gemm_simt.cu), six warps instead of 32: identical index lists.
-    __shared__ unsigned int s_last;
-    __shared__ int s_cnt[TC_THREADS / 32];
-    if (threadIdx.x == 0) s_last = (atomicAdd(p.done_counter, 1u) == gridDim.x - 1) ? 1u : 0u;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
-    int* sRow = reinterpret_cast<int*>(smem);                   // 0 = unmatched row, j + 1 = matched with column j
-    const int tid = threadIdx.x, NA = p.NA, NB = p.NB;
-    constexpr int NW = TC_THREADS / 32;
-    for (int i = tid; i < NA; i += TC_THREADS) sRow[i] = 0;
-    __syncthreads();
-    for (int j = tid; j < NB; j += TC_THREADS) {
-        const unsigned long long ck = __ldcg(p.colbest + j);
-        if (ck == 0ull) continue;
-        const uint32_t i = key_index(ck);
-        if (i >= (uint32_t)NA) continue;
-        const unsigned long long rk = __ldcg(p.rowbest + i);
-        const float v = key_value(rk);
-        if (rk != 0ull && key_index(rk) == (uint32_t)j && (__fmul_rn(v, v) > 0.f)) sRow[i] = j + 1;
-    }
-    __syncthreads();
-    const int chunk = (((NA + 31) / 32) + NW - 1) / NW * 32;    // rows per warp, a multiple of 32
-    const int begin = warp * chunk;
-    int cnt = 0;
-    for (int b = 0; b < chunk; b += 32) {
-        const int i = begin + b + lane;
-        cnt += __popc(__ballot_sync(0xffffffffu, i < NA && sRow[i] != 0));
-    }
-    if (lane == 0) s_cnt[warp] = cnt;
-    __syncthreads();
-    int off = 0, total_m = 0;
-    for (int w = 0; w < NW; ++w) { const int v = s_cnt[w]; off += (w < warp) ? v : 0; total_m += v; }
-    for (int b = 0; b < chunk; b += 32) {
-        const int i = begin + b + lane;
-        const int f = (i < NA) ? sRow[i] : 0;
-        const uint32_t bal = __ballot_sync(0xffffffffu, f != 0);
-        if (f) {
-            const int o = off + __popc(bal & ((1u << lane) - 1u));
-            p.tail_idx1[o] = i;
-            p.tail_idx2[o] = (long long)(f - 1);
-        }
-        off += __popc(bal);
-    }
-    if (tid == 0) *p.tail_count = total_m;
 }
 
+
 // ------------------------------------------------------------------------------------------------------------
-// ResNet-50 stem, fused (engine 2): conv 7x7 / stride 2 / pad 3 on the 3-channel fp32 image + folded BN + ReLU ->
-// fp16 NHWC, without materialising the im2col matrix (350 MB written and read back per pair at 480x640 x 8 images).
-// One CTA = 16 x 8 output pixels x 64 channels:
-//   warps 0-3 : stage the 37 x 21 x 3 input window in shared memory (coalesced, zero padded), then each thread builds
-//               ITS pixel's 147-long (r, s, c) patch as fp16 directly in the 128-byte-swizzled K-major layout the
-//               UMMA descriptors expect (three K blocks of 64; 148..191 are zeros), fence.proxy.async, arrive;
-//   warp 4    : TMA-loads the 64 x 192 fp16 weights, issues 12 tcgen05.mma kind::f16 (M 128, N 64, K 16), commits;
-//   warps 0-3 : epilogue - TMEM -> + bias, ReLU -> fp16 swizzled staging (the A tile's first block) -> one TMA store.
+// ResNet-50 stem, fused: conv 7x7 / stride 2 / pad 3 on the 3-channel fp32 image + folded BN + ReLU -> fp16 (engine 2) or split
+// (engine 4) NHWC, without an im2col matrix in HBM.  One CTA = 16 x 8 output pixels x 64 channels, 256 threads:
+//   all threads : stage the 21 x 111 input window (split into (hi, lo) pairs once), then two threads per output pixel build its
+//                 147-long (r, s, c) patch as hi / lo planes in the 128-byte-swizzled K-major layout (3 K blocks of 64; 147..191
+//                 are zeros), fence.proxy.async;
+//   warpgroups  : 64 pixels each, wgmma over the three K blocks against the weights TMA-loaded at CTA start; register epilogue.
 // ------------------------------------------------------------------------------------------------------------
-constexpr int STEM_TW = 16, STEM_TH = 8, STEM_K = 7, STEM_C = 3, STEM_KK = 147, STEM_KB = 3;
-constexpr int STEM_IN_W = ((STEM_TW - 1) * 2 + STEM_K) * STEM_C;          // 111 floats per staged input row
-constexpr int STEM_IN_H = (STEM_TH - 1) * 2 + STEM_K;                     // 21 rows
-constexpr int STEM_IN_LD = 112;
-constexpr int STEM_B_TILE = 64 * 128;                                     // 8 KB per K block
-constexpr int STEM_OFF_B = STEM_KB * TC_A_BYTES;                          // 48 KB
-constexpr int STEM_OFF_IN = STEM_OFF_B + STEM_KB * STEM_B_TILE;           // 72 KB
-constexpr int STEM_OFF_BAR = STEM_OFF_IN + STEM_IN_H * STEM_IN_LD * 4;    // + 9408 B
-constexpr int STEM_SMEM = STEM_OFF_BAR + 64 + 1024;
-constexpr int STEM_THREADS = 160;
+constexpr int SS_TW = 16, SS_TH = 8, SS_K = 7, SS_C = 3, SS_KK = 147, SS_KB = 3;
+constexpr int SS_IN_W = ((SS_TW - 1) * 2 + SS_K) * SS_C;                  // 111 floats per staged input row
+constexpr int SS_IN_H = (SS_TH - 1) * 2 + SS_K;                           // 21 rows
+constexpr int SS_IN_LD = 112;
+constexpr int SS_THREADS = 256;
+constexpr int SS_B_PLANE = 64 * 128;                                      // one K block of 64 weight rows: 8 KB
+constexpr int SS_OFF_ALO = SS_KB * TC_A_BYTES;                            // 48 KB: lo planes of the patches
+constexpr int SS_OFF_B = 2 * SS_KB * TC_A_BYTES;                          // 96 KB
+constexpr int SS_OFF_IN = SS_OFF_B + SS_KB * 2 * SS_B_PLANE;              // 144 KB
+constexpr int SS_OFF_BAR = SS_OFF_IN + SS_IN_H * SS_IN_LD * 4;
+constexpr int SS_SMEM = SS_OFF_BAR + 64 + 1024;
+constexpr int SS_NLD = (SS_IN_H * SS_IN_W + SS_THREADS - 1) / SS_THREADS;  // window floats per thread
+static_assert(SS_SMEM <= 227 * 1024, "stem shared memory");
 
 struct alignas(64) StemParams {
-    CUtensorMap mapB;                     // weights fp16 [64][192], box (64, 64)
-    CUtensorMap mapY[RF_MAX_IMGS];        // output fp16 (64, Wo, Ho), box (64, 16, 8)
+    CUtensorMap mapB;                     // weights (192, 64[, 2]) fp16, box (64, 64[, 2])
     int nimg;
     int tile_start[RF_MAX_IMGS + 1];
     int tiles_x[RF_MAX_IMGS];
-    int H[RF_MAX_IMGS], W[RF_MAX_IMGS];
-    long long in_pix[RF_MAX_IMGS];
+    int H[RF_MAX_IMGS], W[RF_MAX_IMGS], Ho[RF_MAX_IMGS], Wo[RF_MAX_IMGS];
+    long long in_pix[RF_MAX_IMGS], out_pix[RF_MAX_IMGS];
+    long long plane;                      // split output: elements from the hi to the lo plane
     const float* x;
     const float* bias;
+    __half* y;
 };
 
-__global__ void __launch_bounds__(STEM_THREADS, 2)
-stem7_f16_kernel(const __grid_constant__ StemParams p) {
+// one staged window element: (hi, lo * 2^11) fp16 pair packed in 32 bits (hi in the low half)
+__device__ __forceinline__ uint32_t stem_pack_split(float v) {
+    __half2 hi, lo;
+    split2(v, 0.f, hi, lo);
+    return (*reinterpret_cast<uint32_t*>(&hi) & 0xFFFFu) | (*reinterpret_cast<uint32_t*>(&lo) << 16);
+}
+
+// half a patch: the 16-byte chunks 4 * HALF .. 4 * HALF + 3 of K block kb of pixel m, hi and lo planes
+template <int HALF, int kb>
+__device__ __forceinline__ void stem_build_half(const uint32_t* __restrict__ base, uint8_t* sA, int m) {
+#pragma unroll
+    for (int cc = 0; cc < 4; ++cc) {
+        const int c8 = HALF * 4 + cc;
+        uint4 oh, ol;
+        uint32_t* ph = reinterpret_cast<uint32_t*>(&oh);
+        uint32_t* pl = reinterpret_cast<uint32_t*>(&ol);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int k0 = kb * 64 + c8 * 8 + 2 * e, k1 = k0 + 1;
+            const uint32_t a = k0 < SS_KK ? base[(k0 / 21) * SS_IN_LD + (k0 % 21)] : 0u;
+            const uint32_t b = k1 < SS_KK ? base[(k1 / 21) * SS_IN_LD + (k1 % 21)] : 0u;
+            ph[e] = __byte_perm(a, b, 0x5410);          // (hi(a), hi(b))
+            pl[e] = __byte_perm(a, b, 0x7632);          // (lo(a), lo(b))
+        }
+        uint8_t* dst = sA + kb * TC_A_BYTES + m * 128 + ((c8 ^ (m & 7)) << 4);
+        *reinterpret_cast<uint4*>(dst) = oh;
+        *reinterpret_cast<uint4*>(dst + SS_OFF_ALO) = ol;
+    }
+}
+
+template <bool SPLIT>
+__global__ void __launch_bounds__(SS_THREADS, 1)
+stem7_kernel(const __grid_constant__ StemParams p) {
+    constexpr int NPL = SPLIT ? 2 : 1;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);      // pointer arithmetic keeps the shared address space (LDS / STS, not generic LD / ST)
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sA = smem;
-    uint8_t* sB = smem + STEM_OFF_B;
-    float* sIn = reinterpret_cast<float*>(smem + STEM_OFF_IN);
-    uint64_t* bar_b = reinterpret_cast<uint64_t*>(smem + STEM_OFF_BAR);
-    uint64_t* bar_a = bar_b + 1;
-    uint64_t* bar_mma = bar_a + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_mma + 1);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint8_t* sB = smem + SS_OFF_B;
+    uint32_t* sIn = reinterpret_cast<uint32_t*>(smem + SS_OFF_IN);
+    uint64_t* bar_b = reinterpret_cast<uint64_t*>(smem + SS_OFF_BAR);
+    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
 
     int img = 0;
 #pragma unroll
     for (int j = 1; j < RF_MAX_IMGS; ++j) img += (j < p.nimg && (int)blockIdx.x >= p.tile_start[j]) ? 1 : 0;
     const int tloc = blockIdx.x - p.tile_start[img];
     const int tyi = tloc / p.tiles_x[img], txi = tloc - tyi * p.tiles_x[img];
-    const int ox0 = txi * STEM_TW, oy0 = tyi * STEM_TH;
+    const int ox0 = txi * SS_TW, oy0 = tyi * SS_TH;
 
-    if (threadIdx.x == 0) {
+    if (t == 0) {
         mbar_init(bar_b, 1);
-        mbar_init(bar_a, 128);
-        mbar_init(bar_mma, 1);
         fence_barrier_init();
     }
-    if (warp == 4) {
-        if (lane == 0) { tma_prefetch_desc(&p.mapB); tma_prefetch_desc(&p.mapY[img]); }
-        tmem_alloc(tmem_slot, 64);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 4) {
-        if (lane == 0) {
-            mbar_expect_tx(bar_b, STEM_KB * STEM_B_TILE);
+    if (t == 0) {
+        mbar_expect_tx(bar_b, SS_KB * NPL * SS_B_PLANE);
 #pragma unroll
-            for (int kb = 0; kb < STEM_KB; ++kb) tma_load_2d(sB + kb * STEM_B_TILE, &p.mapB, bar_b, kb * 64, 0);
+        for (int kb = 0; kb < SS_KB; ++kb) {
+            if constexpr (SPLIT) tma_load_3d(sB + kb * 2 * SS_B_PLANE, &p.mapB, bar_b, kb * 64, 0, 0);
+            else tma_load_2d(sB + kb * SS_B_PLANE, &p.mapB, bar_b, kb * 64, 0);
         }
-        mbar_wait(bar_b, 0);
-        mbar_wait(bar_a, 0);
-        tc_fence_after();
-        constexpr uint32_t idesc = make_idesc_f16(64);
+    }
+    {   // the zero-padded input window, split once
+        const int H = p.H[img], WC = p.W[img] * SS_C;
+        const float* src = p.x + p.in_pix[img] * SS_C;
+        const int iy0 = oy0 * 2 - 3, col0 = (ox0 * 2 - 3) * SS_C;
 #pragma unroll
-        for (int kb = 0; kb < STEM_KB; ++kb)
-            umma_f16_x4(tmem_base, make_desc_sw128(smem_u32(sA + kb * TC_A_BYTES)), make_desc_sw128(smem_u32(sB + kb * STEM_B_TILE)), idesc, kb != 0 ? 1u : 0u);
-        umma_commit(bar_mma);
-    } else {
-        const int m = threadIdx.x;                              // 0..127: output pixel inside the tile = accumulator row
-        // ---- stage the input window: rows 2*oy0-3 .. +20, float columns (2*ox0-3)*3 .. +110 ----
-        const int H = p.H[img], WC = p.W[img] * STEM_C;
-        const float* src = p.x + p.in_pix[img] * STEM_C;
-        const int iy0 = oy0 * 2 - 3, col0 = (ox0 * 2 - 3) * STEM_C;
-        // all loads first (independent, one DRAM latency), then the shared-memory stores
-        constexpr int NLD = (STEM_IN_H * STEM_IN_W + 127) / 128;         // 19 per thread
-        float stage[NLD];
-#pragma unroll
-        for (int i = 0; i < NLD; ++i) {
-            const int idx = m + i * 128;
-            const int r = idx / STEM_IN_W, j = idx - r * STEM_IN_W;
+        for (int i = 0; i < SS_NLD; ++i) {
+            const int idx = t + i * SS_THREADS;
+            const int r = idx / SS_IN_W, j = idx - r * SS_IN_W;
             const int iy = iy0 + r, col = col0 + j;
-            stage[i] = (idx < STEM_IN_H * STEM_IN_W && iy >= 0 && iy < H && col >= 0 && col < WC) ? __ldg(src + (long long)iy * WC + col) : 0.f;
+            if (idx < SS_IN_H * SS_IN_W)
+                sIn[r * SS_IN_LD + j] = stem_pack_split((iy >= 0 && iy < H && col >= 0 && col < WC) ? __ldg(src + (long long)iy * WC + col) : 0.f);
         }
+    }
+    __syncthreads();
+    {   // this pixel's patch, (r, s, c) order: element k = r*21 + s*3 + c sits at sIn[2*py + r][6*px + (k % 21)]
+        const int m = t & 127, py = m >> 4, px = m & 15;
+        const uint32_t* base = sIn + (2 * py) * SS_IN_LD + 6 * px;
+        if (t < 128) { stem_build_half<0, 0>(base, sA, m); stem_build_half<0, 1>(base, sA, m); stem_build_half<0, 2>(base, sA, m); }
+        else { stem_build_half<1, 0>(base, sA, m); stem_build_half<1, 1>(base, sA, m); stem_build_half<1, 2>(base, sA, m); }
+    }
+    fence_proxy_async();            // generic-proxy writes -> visible to the tensor core (async proxy)
+    __syncthreads();
+    mbar_wait(bar_b, 0);
+
+    const int g = warp >> 2;
+    constexpr int NACC = SPLIT ? 2 : 1;
+    float acc[NACC][32];
 #pragma unroll
-        for (int i = 0; i < NLD; ++i) {
-            const int idx = m + i * 128;
-            const int r = idx / STEM_IN_W, j = idx - r * STEM_IN_W;
-            if (idx < STEM_IN_H * STEM_IN_W) sIn[r * STEM_IN_LD + j] = stage[i];
+    for (int a = 0; a < NACC; ++a)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[a][i] = 0.f;
+    wg_fence();
+#pragma unroll
+    for (int kb = 0; kb < SS_KB; ++kb) {
+        const uint32_t a = smem_u32(sA + kb * TC_A_BYTES + g * (64 * 128)), b = smem_u32(sB + kb * NPL * SS_B_PLANE);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t ah = wg_desc(a + 32 * k), bh = wg_desc(b + 32 * k);
+            if constexpr (SPLIT) {
+                wgmma<false, 64>(acc[1], wg_desc(a + SS_OFF_ALO + 32 * k), bh);
+                wgmma<false, 64>(acc[1], ah, wg_desc(b + SS_B_PLANE + 32 * k));
+            }
+            wgmma<false, 64>(acc[0], ah, bh);
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        // ---- this pixel's patch, (r, s, c) order: element k = r*21 + s*3 + c sits at sIn[2*py + r][6*px + (k % 21)] ----
-        const int py = m >> 4, px = m & 15;
-        const float* base = sIn + (2 * py) * STEM_IN_LD + 6 * px;
+    }
+    wg_commit();
+    wg_wait<0>();
 #pragma unroll
-        for (int kb = 0; kb < STEM_KB; ++kb) {
+    for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
+
+    const int rbase = 64 * g + 16 * (warp & 3) + (lane >> 2), cbase = 2 * (lane & 3);
 #pragma unroll
-            for (int c8 = 0; c8 < 8; ++c8) {
-                uint4 o;
-                __half2* ho = reinterpret_cast<__half2*>(&o);
+    for (int h = 0; h < 2; ++h) {
+        const int m = rbase + 8 * h;
+        const int oy = oy0 + (m >> 4), ox = ox0 + (m & 15);
+        if (oy >= p.Ho[img] || ox >= p.Wo[img]) continue;
+        __half* y = p.y + (p.out_pix[img] + (long long)oy * p.Wo[img] + ox) * 64;
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const int k0 = kb * 64 + c8 * 8 + 2 * e, k1 = k0 + 1;
-                    const float a = k0 < STEM_KK ? base[(k0 / 21) * STEM_IN_LD + (k0 % 21)] : 0.f;
-                    const float b = k1 < STEM_KK ? base[(k1 / 21) * STEM_IN_LD + (k1 % 21)] : 0.f;
-                    ho[e] = __floats2half2_rn(a, b);
-                }
-                *reinterpret_cast<uint4*>(sA + kb * TC_A_BYTES + m * 128 + ((c8 ^ (m & 7)) << 4)) = o;
+        for (int j = 0; j < 8; ++j) {
+            const int n = 8 * j + cbase, i = 4 * j + 2 * h;
+            float v0 = SPLIT ? fmaf(acc[NACC - 1][i], 0.00048828125f, acc[0][i]) : acc[0][i];
+            float v1 = SPLIT ? fmaf(acc[NACC - 1][i + 1], 0.00048828125f, acc[0][i + 1]) : acc[0][i + 1];
+            if (p.bias) { v0 += __ldg(p.bias + n); v1 += __ldg(p.bias + n + 1); }
+            v0 = fmaxf(v0, 0.f);
+            v1 = fmaxf(v1, 0.f);
+            if constexpr (SPLIT) {
+                __half2 hi, lo;
+                split2(v0, v1, hi, lo);
+                *reinterpret_cast<__half2*>(y + n) = hi;
+                *reinterpret_cast<__half2*>(y + p.plane + n) = lo;
+            } else {
+                *reinterpret_cast<__half2*>(y + n) = pack_sat(v0, v1);
             }
         }
-        fence_proxy_async();                                    // generic-proxy writes -> visible to the tensor core (async proxy)
-        mbar_arrive(bar_a);
-        // ---- epilogue ----
-        mbar_wait(bar_mma, 0);
-        tc_fence_after();
-        const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
-        epi_rows_f16<64>(p.bias, 64, 1, false, 0, m, trow, sA);
-        fence_proxy_async();
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (m == 0) {
-            tma_store_3d(&p.mapY[img], sA, 0, ox0, oy0);
-            tma_store_commit_and_wait_read();
-        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tmem_base, 64);
 }
+
 
 // hi = x with the 13 low mantissa bits cleared (exactly representable in TF32), lo = x - hi (exact in fp32)
 __global__ void split_tf32_kernel(const float4* __restrict__ x, float4* __restrict__ hi, float4* __restrict__ lo, long long n4) {
@@ -1437,8 +503,7 @@ __global__ void split_f16_kernel(const float4* __restrict__ x, uint2* __restrict
 }
 
 // Both feature matrices in ONE launch (fp16 split as above; hi/lo of A then hi/lo of B are consecutive in the workspace),
-// and the arg-max keys zeroed by the first threads: replaces a memset node and two split launches in front of the
-// persistent correlation kernel.
+// and the arg-max keys zeroed by the first threads: replaces a memset node and two split launches.
 __global__ void split_f16_all_kernel(const float4* __restrict__ A, const float4* __restrict__ B, uint2* __restrict__ Ahi, uint2* __restrict__ Alo,
                                      uint2* __restrict__ Bhi, uint2* __restrict__ Blo, long long na4, long long nb4,
                                      unsigned long long* __restrict__ keys, long long nkeys) {
@@ -1541,143 +606,113 @@ int pick_tw(int Ho, int Wo) {
     return best;
 }
 
-static int halo_mode() {
-    static int m = -1;
-    if (m < 0) {
-        const char* e = getenv("RF_TC_HALO");     // 0 = tap-streaming kernel, anything else = halo reuse (default)
-        m = (e && atoi(e) == 0) ? 0 : 2;
-    }
-    return m;
-}
-
-static int corr_tile_n() {
-    static int m = -1;
-    if (m < 0) {
-        const char* e = getenv("RF_CORR_BN");     // 128 (default) or 256; measured equal within 3 % (191 vs 185 us): the
-        m = e ? atoi(e) : 128;                    // kernel is shared-memory-bandwidth bound (A+B 8 KB per 64-cycle MMA), not L2 bound
-    }
-    return m;
-}
-
-static int persist_mode() {
-    static int m = -1;
-    if (m < 0) {
-        const char* e = getenv("RF_TC_PERSIST");
-        m = e ? atoi(e) : 0;
-    }
-    return m;
-}
-
-static int respf_mode() {
-    const char* e = getenv("RF_TC_RESPF");    // fp16 1x1 convs with a residual: prefetch the residual tile at CTA start.
-    return e ? atoi(e) : 0;                     // Measured (profiles/README.md): -2 % end to end - the extra staging costs a resident CTA
-}
-
-static int resb_mode() {
-    static int m = -1;
-    if (m < 0) {
-        const char* e = getenv("RF_TC_RESB");     // weights-resident persistent kernel for 64 -> 64 3x3 convs (default on);
-        m = e ? atoi(e) : 1;                      // a 3-slot / direct-store variant measured no faster (332 vs 320 us per pair)
-    }
-    return m;
-}
-
-template <bool F16>
-static int launch_resb(const TcParams& p, int tiles_m, cudaStream_t st) {
+template <int KIND, int BN, int MODE, int OUT>
+static int launch_wg(const WgParams& p, dim3 grid, cudaStream_t st) {
+    using Cfg = WgCfg<KIND, BN, MODE>;
     static bool attr[64] = {false};
     const int dev = current_device();
     if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(tc_resb_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, ResBCfg<F16>::SMEM_BYTES));
+        RF_CUDA(cudaFuncSetAttribute(wg_kernel<KIND, BN, MODE, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         attr[dev] = true;
     }
-    const int grid = tiles_m < num_sms() ? tiles_m : num_sms();
-    tc_resb_kernel<F16><<<grid, TC_THREADS, ResBCfg<F16>::SMEM_BYTES, st>>>(p, tiles_m);
+    wg_kernel<KIND, BN, MODE, OUT><<<grid, WG_THREADS, Cfg::SMEM_BYTES, st>>>(p);
     RF_LAUNCHED();
     return 0;
 }
 
-static int raster_mode() {
-    const char* e = getenv("RF_TC_RASTER");    // 1 (default): channel tiles fastest for the tap-streaming conv kernels - the CTAs
-    return e ? atoi(e) : 1;                     // of one pixel tile run together (A once from HBM, whole output rows); +2 % per pair
+template <int KIND, int OUT>
+static int launch_conv(const WgParams& p, int BN, int tiles, int nt, cudaStream_t st) {
+    return BN == 128 ? launch_wg<KIND, 128, MODE_CONV, OUT>(p, dim3(tiles, nt), st) : launch_wg<KIND, 64, MODE_CONV, OUT>(p, dim3(tiles, nt), st);
 }
 
-static int pipe_mode() {
-    const char* e = getenv("RF_TC_PIPE");    // pipelined persistent kernel for the fp16 tap-streaming convs: 0 never, 1 always,
-    return e ? atoi(e) : 2;                     // 2 (default) where it measured faster: >= 4 K blocks and >= 2 tiles per SM
+// dual: a second input (x2, its own per-image sizes hw2, Cin2 channels, sampled with stride2) whose channels continue the K axis
+// of a 1x1 convolution: y = act(W[:, :Cin] x + W[:, Cin:] x2[::stride2] + bias) - a bottleneck's conv3 and its down-sampling
+// branch in one GEMM (the branch's output never goes to HBM and comes back as a residual).
+struct SplitDual { const void* x2; const int* hw2; int Cin2, stride2; };
+
+// kind K_TF32: x / residual / y fp32, w [Cout][K] fp32.  K_F16: fp16 x / residual / w, y fp16 (out32: fp32).  K_SPLIT: x / residual /
+// y split tensors ([2][P][C] fp16, planes P * C elements apart), w [2][Cout][K] fp16 (out32: y fp32 [P][Cout], no residual).
+static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cudaStream_t st, int kind, bool out32, const SplitDual* dual) {
+    WgParams p;
+    memset(&p, 0, sizeof(p));
+    const bool split = kind == K_SPLIT;
+    const unsigned esz = kind == K_TF32 ? 4u : 2u;
+    const unsigned bk = kind == K_TF32 ? TC_BK : TC_BK_F16;
+    const int BN = cp.Cout > 64 ? 128 : 64;
+    const char* xb = reinterpret_cast<const char*>(cp.x);
+    const unsigned long long in_plane = (unsigned long long)set.in_pix[set.n] * cp.Cin * 2ull;
+    long long in2_pix[RF_MAX_IMGS + 1] = {0};
+    if (dual)
+        for (int i = 0; i < set.n; ++i) in2_pix[i + 1] = in2_pix[i] + (long long)dual->hw2[2 * i] * dual->hw2[2 * i + 1];
+    const unsigned long long in2_plane = dual ? (unsigned long long)in2_pix[set.n] * dual->Cin2 * 2ull : 0ull;
+    p.nimg = set.n;
+    int tiles = 0;
+    for (int i = 0; i < set.n; ++i) {
+        const int tw = pick_tw(set.Ho[i], set.Wo[i]), th = 128 / tw;
+        p.tw[i] = tw;
+        p.tiles_x[i] = (set.Wo[i] + tw - 1) / tw;
+        p.tile_start[i] = tiles;
+        tiles += p.tiles_x[i] * ((set.Ho[i] + th - 1) / th);
+        p.Ho[i] = set.Ho[i]; p.Wo[i] = set.Wo[i];
+        p.out_pix[i] = set.out_pix[i];
+        int rc = split ? get_map4(&p.mapA[i], xb + set.in_pix[i] * cp.Cin * 2, (unsigned long long)cp.Cin, (unsigned long long)set.W[i],
+                                  (unsigned long long)set.H[i], 2, in_plane, bk, (unsigned)tw, (unsigned)th, 2, (unsigned)cp.stride, 2)
+                       : get_map(&p.mapA[i], xb + set.in_pix[i] * cp.Cin * esz, (unsigned long long)cp.Cin, (unsigned long long)set.W[i],
+                                 (unsigned long long)set.H[i], bk, (unsigned)tw, (unsigned)th, (unsigned)cp.stride, esz);
+        if (!rc && dual)
+            rc = get_map4(&p.mapA2[i], static_cast<const char*>(dual->x2) + in2_pix[i] * dual->Cin2 * 2, (unsigned long long)dual->Cin2,
+                          (unsigned long long)dual->hw2[2 * i + 1], (unsigned long long)dual->hw2[2 * i], 2, in2_plane, bk, (unsigned)tw,
+                          (unsigned)th, 2, (unsigned)dual->stride2, 2);
+        if (rc) return rc;
+    }
+    RF_REQUIRE(tiles > 0, "rf_conv2d_nhwc: empty output");
+    for (int i = set.n; i <= RF_MAX_IMGS; ++i) p.tile_start[i] = tiles;
+    p.out_pix[set.n] = set.out_pix[set.n];
+    int rc = split ? get_map(&p.mapB, w, (unsigned long long)cp.K, (unsigned long long)cp.Cout, 2, bk, (unsigned)BN, 2, 1, 2)
+                   : get_map(&p.mapB, w, (unsigned long long)cp.K, (unsigned long long)cp.Cout, 0, bk, (unsigned)BN, 0, 1, esz);
+    if (rc) return rc;
+    p.R = cp.R; p.S = cp.S; p.pad = cp.pad; p.stride = cp.stride; p.Cin = cp.Cin; p.Cout = cp.Cout; p.relu = cp.relu; p.round_out = cp.round_out;
+    p.kc1 = cp.Cin / (int)bk;
+    p.stride2 = 1;
+    if (dual) { p.Cin = cp.Cin + dual->Cin2; p.stride2 = dual->stride2; }      // the kernel's K axis: both inputs
+    p.plane = (long long)set.out_pix[set.n] * cp.Cout;
+    p.bias = cp.bias; p.residual = cp.residual; p.y = cp.y;
+    const int nt = (cp.Cout + BN - 1) / BN;
+    if (kind == K_TF32) return launch_conv<K_TF32, O_F32>(p, BN, tiles, nt, st);
+    if (kind == K_F16) return out32 ? launch_conv<K_F16, O_F32>(p, BN, tiles, nt, st) : launch_conv<K_F16, O_F16>(p, BN, tiles, nt, st);
+    return out32 ? launch_conv<K_SPLIT, O_F32>(p, BN, tiles, nt, st) : launch_conv<K_SPLIT, O_SPLIT>(p, BN, tiles, nt, st);
 }
 
-template <int BN>
-static int launch_pipe(const TcParams& p, int tiles_m, int tiles_n, cudaStream_t st) {
-    using Cfg = PipeCfg<BN>;
+template <bool SPLIT>
+static int stem_impl(const float* x, int nimg, const int* hw_host, const void* w, const float* bias, void* y, void* stream) {
+    RF_REQUIRE(x != nullptr && w != nullptr && y != nullptr, "rf_stem7: null pointer");
+    RF_REQUIRE(((uintptr_t)y % 16) == 0 && ((uintptr_t)w % 16) == 0, "rf_stem7: pointers must be 16-byte aligned");
+    ImgSet set;
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, 7, 2, 3) == 0, "rf_stem7: bad image set");
+    StemParams p;
+    memset(&p, 0, sizeof(p));
+    p.nimg = nimg;
+    int tiles = 0;
+    for (int i = 0; i < nimg; ++i) {
+        p.tiles_x[i] = (set.Wo[i] + SS_TW - 1) / SS_TW;
+        p.tile_start[i] = tiles;
+        tiles += p.tiles_x[i] * ((set.Ho[i] + SS_TH - 1) / SS_TH);
+        p.H[i] = set.H[i]; p.W[i] = set.W[i]; p.Ho[i] = set.Ho[i]; p.Wo[i] = set.Wo[i];
+        p.in_pix[i] = set.in_pix[i];
+        p.out_pix[i] = set.out_pix[i];
+    }
+    for (int i = nimg; i <= RF_MAX_IMGS; ++i) p.tile_start[i] = tiles;
+    int rc = SPLIT ? get_map(&p.mapB, w, 192ull, 64ull, 2, 64, 64, 2, 1, 2) : get_map(&p.mapB, w, 192ull, 64ull, 0, 64, 64, 0, 1, 2);
+    if (rc) return rc;
+    p.plane = set.out_pix[nimg] * 64;
+    p.x = x; p.bias = bias; p.y = static_cast<__half*>(y);
     static bool attr[64] = {false};
     const int dev = current_device();
     if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(tc_pipe_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        RF_CUDA(cudaFuncSetAttribute(stem7_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SS_SMEM));
         attr[dev] = true;
     }
-    const int total = tiles_m * tiles_n;
-    const int grid = total < num_sms() ? total : num_sms();
-    tc_pipe_kernel<BN><<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(p, tiles_m, tiles_n);
-    RF_LAUNCHED();
-    return 0;
-}
-
-template <int BN, bool HALO>
-static int launch_persist(const TcParams& p, int tiles_m, int tiles_n, cudaStream_t st) {
-    using Cfg = PCfg<BN, HALO>;
-    static bool attr[64] = {false};
-    const int dev = current_device();
-    if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(tc_persist_kernel<BN, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-        attr[dev] = true;
-    }
-    const int total = tiles_m * tiles_n;
-    const int grid = total < num_sms() ? total : num_sms();
-    tc_persist_kernel<BN, HALO><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p, tiles_m, tiles_n);
-    RF_LAUNCHED();
-    return 0;
-}
-
-template <int BN, bool F16 = false, bool OUT32 = false>
-static int launch_halo(const TcParams& p, int tiles, int ntiles_n, int mode, cudaStream_t st) {
-    using Cfg = HaloCfg<BN>;
-    static bool attr[64] = {false};
-    const int dev = current_device();
-    if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(tc_halo_kernel<BN, F16, OUT32>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-        attr[dev] = true;
-    }
-    tc_halo_kernel<BN, F16, OUT32><<<dim3(tiles, ntiles_n), TC_THREADS, Cfg::SMEM_BYTES, st>>>(p, mode);
-    RF_LAUNCHED();
-    return 0;
-}
-
-template <int BN, int MODE, bool DEEP, bool F16 = false>
-static int launch_tc(const TcParams& p, int tiles, int ntiles_n, cudaStream_t st) {
-    using Cfg = TcCfg<BN, MODE, DEEP>;
-    static bool attr[64] = {false};
-    const int dev = current_device();
-    if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(tc_kernel<BN, MODE, DEEP, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     Cfg::SMEM_BYTES + (F16 ? (BN / 64) * TC_A_BYTES : 0)));
-        attr[dev] = true;
-    }
-    dim3 grid = (MODE == MODE_CORR || p.raster_n) ? dim3(ntiles_n, tiles) : dim3(tiles, ntiles_n);
-    if (F16 && MODE == MODE_CONV) {
-        // ring depth: never more stages than K blocks; with a prefetched residual two stages (+ its staging) keep two or
-        // three CTAs resident per SM
-        TcParams q = p;
-        const int KI = p.R * p.S * (p.Cin / TC_BK_F16);
-        q.res_pf = (p.residual != nullptr && respf_mode()) ? 1 : 0;
-        int stages = KI < Cfg::STAGES ? KI : Cfg::STAGES;
-        if (q.res_pf && stages > 2) stages = 2;
-        q.stages = stages;
-        const int smem = stages * Cfg::STAGE_BYTES + (q.res_pf ? (BN / 64) * TC_A_BYTES : 0) + 1024 + 256;
-        tc_kernel<BN, MODE, DEEP, F16><<<grid, TC_THREADS, smem, st>>>(q);
-        RF_LAUNCHED();
-        return 0;
-    }
-    tc_kernel<BN, MODE, DEEP, F16><<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(p);
+    stem7_kernel<SPLIT><<<tiles, SS_THREADS, SS_SMEM, as_stream(stream)>>>(p);
     RF_LAUNCHED();
     return 0;
 }
@@ -1693,6 +728,9 @@ bool rf_conv2d_tc_supported(const ConvParams& p) {
 bool rf_conv2d_f16_supported(const ConvParams& p) {
     return (p.stride == 1 || p.stride == 2) && (p.Cin % TC_BK_F16) == 0 && p.Cout >= 8 && (p.Cout % 8) == 0 && p.R == p.S && (p.R == 1 || p.R == 3);
 }
+bool rf_conv2d_split_supported(const ConvParams& p) {
+    return (p.stride == 1 || p.stride == 2) && (p.Cin % TC_BK_F16) == 0 && p.Cout >= 1 && p.R == p.S && (p.R == 1 || p.R == 3);
+}
 
 // f16 = false: x / residual / y fp32, w_tc fp32 [Cout][K] (TF32-rounded).  f16 = true: the same pointers hold IEEE fp16.
 // out32 (with f16): y is fp32 (3x3 / stride 1 layers only, no residual) - the hand-over from fp16 layers to a TF32 consumer.
@@ -1700,153 +738,75 @@ int rf_conv2d_tc(const ImgSet& set, const ConvParams& cp, const void* w_tc, cuda
     RF_REQUIRE(w_tc != nullptr, "rf_conv2d_nhwc: tensor-core engines need w_tc ([Cout][R*S*Cin])");
     RF_REQUIRE(f16 ? rf_conv2d_f16_supported(cp) : rf_conv2d_tc_supported(cp),
                "rf_conv2d_nhwc: tensor-core engines need stride 1 or 2, 1x1 or 3x3, Cin % 32 == 0 (fp16: Cin % 64 == 0, Cout % 8 == 0)");
-    TcParams p;
-    memset(&p, 0, sizeof(p));
-    const int BN = cp.Cout > 64 ? 128 : 64;
-    const unsigned esz = f16 ? 2u : 4u;
-    const unsigned bk = f16 ? TC_BK_F16 : TC_BK;
-    const unsigned esz_y = (f16 && !out32) ? 2u : 4u;                // output (and residual) element size
-    const unsigned bk_y = (f16 && !out32) ? TC_BK_F16 : TC_BK;
-    RF_REQUIRE(!out32 || (f16 && cp.R == 3 && cp.stride == 1 && cp.pad == 1 && cp.residual == nullptr && halo_mode() != 0),
+    RF_REQUIRE(!out32 || (f16 && cp.R == 3 && cp.stride == 1 && cp.pad == 1 && cp.residual == nullptr),
                "rf_conv2d_nhwc: engine 3 (fp16 operands, fp32 output) covers 3x3 / stride 1 / pad 1 layers without residual");
-    const char* xb = reinterpret_cast<const char*>(cp.x);
-    const char* rb = reinterpret_cast<const char*>(cp.residual);
-    char* yb = reinterpret_cast<char*>(cp.y);
-    p.nimg = set.n;
-    const int hmode = (cp.R == 3 && cp.stride == 1 && cp.pad == 1) ? halo_mode() : 0;
-    int tiles = 0;
-    for (int i = 0; i < set.n; ++i) {
-        int tw = hmode ? HALO_TW : pick_tw(set.Ho[i], set.Wo[i]), th = 128 / tw;
-        p.tw[i] = tw;
-        p.tiles_x[i] = (set.Wo[i] + tw - 1) / tw;
-        p.tile_start[i] = tiles;
-        tiles += p.tiles_x[i] * ((set.Ho[i] + th - 1) / th);
-        p.Ho[i] = set.Ho[i]; p.Wo[i] = set.Wo[i];
-        p.out_pix[i] = set.out_pix[i];
-        int rc = get_map(&p.mapA[i], xb + set.in_pix[i] * cp.Cin * esz, (unsigned long long)cp.Cin, (unsigned long long)set.W[i],
-                         (unsigned long long)set.H[i], bk, (unsigned)(hmode ? tw + 2 : tw), (unsigned)(hmode ? th + 2 : th), (unsigned)cp.stride, esz);
-        if (rc) return rc;
-    }
-    // bulk (TMA) epilogue whenever the output rows are 16-byte aligned (fp32: Cout % 4 == 0; fp16: Cout % 8 == 0, required)
-    p.tma_epi = (((cp.Cout * esz_y) & 15) == 0 && ((uintptr_t)cp.y % 16) == 0 && ((uintptr_t)cp.residual % 16) == 0) ? 1 : 0;
-    RF_REQUIRE(!f16 || out32 || p.tma_epi, "rf_conv2d_nhwc: engine 2 needs 16-byte aligned y / residual");
-    if (p.tma_epi) {
-        for (int i = 0; i < set.n; ++i) {
-            const unsigned tw = (unsigned)p.tw[i], th = 128u / tw;
-            int rc = get_map(&p.mapY[i], yb + set.out_pix[i] * cp.Cout * esz_y, (unsigned long long)cp.Cout, (unsigned long long)set.Wo[i],
-                             (unsigned long long)set.Ho[i], bk_y, tw, th, 1, esz_y);
-            if (!rc && cp.residual)
-                rc = get_map(&p.mapR[i], rb + set.out_pix[i] * cp.Cout * esz_y, (unsigned long long)cp.Cout, (unsigned long long)set.Wo[i],
-                             (unsigned long long)set.Ho[i], bk_y, tw, th, 1, esz_y);
-            if (rc) return rc;
-        }
-    }
-    for (int i = set.n; i <= RF_MAX_IMGS; ++i) p.tile_start[i] = tiles;
-    p.out_pix[set.n] = set.out_pix[set.n];
-    int rc = get_map(&p.mapB, w_tc, (unsigned long long)cp.K, (unsigned long long)cp.Cout, 0, bk, (unsigned)BN, 0, 1, esz);
-    if (rc) return rc;
-    p.R = cp.R; p.S = cp.S; p.pad = cp.pad; p.stride = cp.stride; p.Cin = cp.Cin; p.Cout = cp.Cout; p.relu = cp.relu; p.round_out = cp.round_out;
-    p.bias = cp.bias; p.residual = cp.residual; p.y = cp.y;
-    const int nt = (cp.Cout + BN - 1) / BN;
-    p.raster_n = (raster_mode() && tiles <= 65535) ? 1 : 0;
-    const bool deep = cp.K >= 512;                                   // >= 16 K-steps of 32 fp32 channels (8 of 64 fp16)
-    if (f16 && out32) return BN == 128 ? launch_halo<128, true, true>(p, tiles, nt, hmode, st) : launch_halo<64, true, true>(p, tiles, nt, hmode, st);
-    if (f16) {
-        if (hmode && resb_mode() && cp.Cin == 64 && cp.Cout == 64) return launch_resb<true>(p, tiles, st);
-        if (hmode) return BN == 128 ? launch_halo<128, true>(p, tiles, nt, hmode, st) : launch_halo<64, true>(p, tiles, nt, hmode, st);
-        const int pm = pipe_mode();
-        if (pm == 1 || (pm == 2 && cp.K >= 4 * TC_BK_F16 && (long long)tiles * nt >= 2ll * num_sms()))
-            return BN == 128 ? launch_pipe<128>(p, tiles, nt, st) : launch_pipe<64>(p, tiles, nt, st);
-        if (BN == 128) return deep ? launch_tc<128, MODE_CONV, true, true>(p, tiles, nt, st) : launch_tc<128, MODE_CONV, false, true>(p, tiles, nt, st);
-        return deep ? launch_tc<64, MODE_CONV, true, true>(p, tiles, nt, st) : launch_tc<64, MODE_CONV, false, true>(p, tiles, nt, st);
-    }
-    if (hmode && resb_mode() && p.tma_epi && cp.Cin == 64 && cp.Cout == 64) return launch_resb<false>(p, tiles, st);
-    if (persist_mode() && p.tma_epi) {
-        if (hmode) return BN == 128 ? launch_persist<128, true>(p, tiles, nt, st) : launch_persist<64, true>(p, tiles, nt, st);
-        return BN == 128 ? launch_persist<128, false>(p, tiles, nt, st) : launch_persist<64, false>(p, tiles, nt, st);
-    }
-    if (hmode) return BN == 128 ? launch_halo<128>(p, tiles, nt, hmode, st) : launch_halo<64>(p, tiles, nt, hmode, st);
-    if (BN == 128) return deep ? launch_tc<128, MODE_CONV, true>(p, tiles, nt, st) : launch_tc<128, MODE_CONV, false>(p, tiles, nt, st);
-    return deep ? launch_tc<64, MODE_CONV, true>(p, tiles, nt, st) : launch_tc<64, MODE_CONV, false>(p, tiles, nt, st);
+    RF_REQUIRE(!f16 || (((uintptr_t)cp.x % 16) == 0 && ((uintptr_t)cp.y % 16) == 0 && ((uintptr_t)cp.residual % 16) == 0),
+               "rf_conv2d_nhwc: engine 2 needs 16-byte aligned x / y / residual");
+    return conv_impl(set, cp, w_tc, st, f16 ? K_F16 : K_TF32, out32, nullptr);
 }
 
-// engine 2: fused ResNet-50 stem (see stem7_f16_kernel).  x fp32 [sum HW][3], w_f16 [64][192] ((r, s, c) order, zero
-// padded), bias fp32 [64], y fp16 [sum HoWo][64]
-int rf_stem7_f16_impl(const float* x, int nimg, const int* hw_host, const void* w_f16, const float* bias, void* y_f16, void* stream) {
-    RF_REQUIRE(x != nullptr && w_f16 != nullptr && y_f16 != nullptr, "rf_stem7: null pointer");
-    RF_REQUIRE(((uintptr_t)y_f16 % 16) == 0 && ((uintptr_t)w_f16 % 16) == 0, "rf_stem7: pointers must be 16-byte aligned");
+int rf_conv2d_split(const ImgSet& set, const ConvParams& cp, const void* w_split, cudaStream_t st, bool out32) {
+    RF_REQUIRE(w_split != nullptr, "rf_conv2d_nhwc: engine 4 needs the split weights ([2][Cout][R*S*Cin] fp16)");
+    RF_REQUIRE(rf_conv2d_split_supported(cp), "rf_conv2d_nhwc: engine 4 needs stride 1 or 2, 1x1 or 3x3, Cin % 64 == 0");
+    RF_REQUIRE(out32 || (cp.Cout % 8) == 0, "rf_conv2d_nhwc: engine 4 needs Cout % 8 == 0 for split outputs");
+    RF_REQUIRE(!out32 || cp.residual == nullptr, "rf_conv2d_nhwc: engine 4 fp32 outputs take no residual");
+    RF_REQUIRE(((uintptr_t)cp.x % 16) == 0 && ((uintptr_t)cp.y % 16) == 0 && ((uintptr_t)cp.residual % 16) == 0 && ((uintptr_t)w_split % 16) == 0,
+               "rf_conv2d_nhwc: engine 4 needs 16-byte aligned pointers");
+    return conv_impl(set, cp, w_split, st, K_SPLIT, out32, nullptr);
+}
+
+extern "C" int rf_conv1x1_dual_split(const void* x1, const void* x2, int nimg, const int* hw1_host, const int* hw2_host, int Cin1, int Cin2,
+                                     int stride2, const void* w_split, const float* bias, int Cout, int relu, void* y, void* stream) {
+    RF_REQUIRE(x1 != nullptr && x2 != nullptr && y != nullptr && hw1_host != nullptr && hw2_host != nullptr && w_split != nullptr,
+               "rf_conv1x1_dual_split: null pointer");
+    RF_REQUIRE(Cin1 >= 1 && Cin2 >= 1 && Cout >= 1, "rf_conv1x1_dual_split: bad channel counts");
+    RF_REQUIRE((Cin1 % TC_BK_F16) == 0 && (Cin2 % TC_BK_F16) == 0 && (Cout % 8) == 0 && (stride2 == 1 || stride2 == 2),
+               "rf_conv1x1_dual_split: Cin1 % 64 == 0, Cin2 % 64 == 0, Cout % 8 == 0, stride2 1 or 2");
+    RF_REQUIRE(((uintptr_t)x1 % 16) == 0 && ((uintptr_t)x2 % 16) == 0 && ((uintptr_t)y % 16) == 0 && ((uintptr_t)w_split % 16) == 0,
+               "rf_conv1x1_dual_split: pointers must be 16-byte aligned");
     ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, 7, 2, 3) == 0, "rf_stem7: bad image set");
-    StemParams p;
-    memset(&p, 0, sizeof(p));
-    p.nimg = nimg;
-    int tiles = 0;
-    for (int i = 0; i < nimg; ++i) {
-        p.tiles_x[i] = (set.Wo[i] + STEM_TW - 1) / STEM_TW;
-        p.tile_start[i] = tiles;
-        tiles += p.tiles_x[i] * ((set.Ho[i] + STEM_TH - 1) / STEM_TH);
-        p.H[i] = set.H[i]; p.W[i] = set.W[i];
-        p.in_pix[i] = set.in_pix[i];
-        int rc = get_map(&p.mapY[i], static_cast<char*>(y_f16) + set.out_pix[i] * 64 * 2, 64ull, (unsigned long long)set.Wo[i],
-                         (unsigned long long)set.Ho[i], 64, STEM_TW, STEM_TH, 1, 2);
-        if (rc) return rc;
-    }
-    for (int i = nimg; i <= RF_MAX_IMGS; ++i) p.tile_start[i] = tiles;
-    int rc = get_map(&p.mapB, w_f16, 192ull, 64ull, 0, 64, 64, 0, 1, 2);
-    if (rc) return rc;
-    p.x = x; p.bias = bias;
-    static bool attr[64] = {false};
-    const int dev = current_device();
-    if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(stem7_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, STEM_SMEM));
-        attr[dev] = true;
-    }
-    stem7_f16_kernel<<<tiles, STEM_THREADS, STEM_SMEM, as_stream(stream)>>>(p);
-    RF_LAUNCHED();
-    return 0;
+    RF_REQUIRE(make_imgset(set, nimg, hw1_host, 1, 1, 0) == 0, "rf_conv1x1_dual_split: bad image set");
+    for (int i = 0; i < nimg; ++i)
+        RF_REQUIRE((hw2_host[2 * i] - 1) / stride2 + 1 == set.Ho[i] && (hw2_host[2 * i + 1] - 1) / stride2 + 1 == set.Wo[i],
+                   "rf_conv1x1_dual_split: the second input, sampled with stride2, must have the first input's size");
+    ConvParams p;
+    p.x = static_cast<const float*>(x1); p.w = nullptr; p.bias = bias; p.residual = nullptr; p.y = static_cast<float*>(y);
+    p.Cin = Cin1; p.Cout = Cout; p.R = 1; p.S = 1; p.stride = 1; p.pad = 0; p.relu = relu;
+    p.round_out = 0;
+    p.Mtot = set.out_pix[nimg];
+    p.K = Cin1 + Cin2;
+    SplitDual dual{x2, hw2_host, Cin2, stride2};
+    return conv_impl(set, p, w_split, as_stream(stream), K_SPLIT, false, &dual);
+}
+
+// fused ResNet-50 stem.  x fp32 [sum HW][3], bias fp32 [64]; engine 2: w_f16 [64][192] ((r, s, c) order, zero padded), y fp16
+// [sum HoWo][64]; engine 4: w_split [2][64][192], y split [2][sum HoWo][64]
+int rf_stem7_f16_impl(const float* x, int nimg, const int* hw_host, const void* w_f16, const float* bias, void* y_f16, void* stream) {
+    return stem_impl<false>(x, nimg, hw_host, w_f16, bias, y_f16, stream);
+}
+int rf_stem7_split_impl(const float* x, int nimg, const int* hw_host, const void* w_split, const float* bias, void* y_split, void* stream) {
+    return stem_impl<true>(x, nimg, hw_host, w_split, bias, y_split, stream);
 }
 
 size_t rf_corr_tc_workspace(int NA, int NB, int C) { return 2ull * ((size_t)NA + NB) * C * sizeof(float) + 1024; }
 
-// RF_CORR_V2 (read per call): 1 (default) = precision 2 runs the persistent correlation kernel with the fused split /
-// key-zeroing launch in front and the fused flag + compaction kernel behind (3 launches); 0 = the one-tile-per-CTA
-// kernel with separate memset / split / split / flag / compact launches (6).  Identical outputs.
-constexpr int RF_CORR_V2_DEFAULT = 1;      // measured on B200: 178 -> 112 us per call at config 2 (profiles/README.md)
+// RF_CORR_V2 (read per call): 1 (default) = precision 2 splits both operands and zeroes the keys in one launch and runs the
+// mutual test + compaction as one kernel behind the correlation (3 launches); 0 = memset / split / split / correlation / flag /
+// compact (6).  Identical outputs.
 int rf_corr_v2_mode() {
     const char* e = getenv("RF_CORR_V2");
-    return e ? atoi(e) : RF_CORR_V2_DEFAULT;
+    return e ? atoi(e) : 1;
 }
 
-static int launch_corr_pipe(const TcParams& p, int tiles_m, int tiles_n, cudaStream_t st) {
-    using Cfg = CorrPipeCfg;
-    static bool attr[64] = {false};
-    const int dev = current_device();
-    if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(tc_corr_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-        attr[dev] = true;
-    }
-    const long long total = (long long)tiles_m * tiles_n;
-    const int grid = total < num_sms() ? (int)total : num_sms();
-    static int mma3 = -1;
-    if (mma3 < 0) { const char* e = getenv("RF_CORR_MMA3"); mma3 = (e && atoi(e) != 0) ? 1 : 0; }
-    TcParams q = p;
-    q.stages = mma3 ? 3 : 0;              // this kernel's ring depth is fixed; the field selects the MMA sequence
-    tc_corr_pipe_kernel<<<grid, TC_THREADS, Cfg::SMEM_BYTES, st>>>(q, tiles_m, tiles_n);
-    RF_LAUNCHED();
-    return 0;
-}
-
-// v2 (precision 2 only): the caller has NOT zeroed rowbest / colbest (contiguous, NA + NB keys): the split launch does it
+// v2 (precision 2 only): the caller has NOT zeroed rowbest / colbest (contiguous, NA + NB keys): the split launch does it.
 // presplit (precision 2, v2 only; nullable): {A hi, A lo, B hi, B lo} fp16 planes written by the producer of the features
 // (rf_l2norm_split_nhwc): no split launch; the caller has zeroed the keys.
-// tail (nullable; v2 only): {idx1, idx2, count, done_counter} - the persistent kernel's last CTA also runs the mutual test and
-// the compaction (NA <= 49152: the row table lives in the idle operand ring); done_counter is zeroed by the caller.
 int rf_corr_argmax_tc(const float* featA, int NA, const float* featB, int NB, int C,
                       unsigned long long* rowbest, unsigned long long* colbest, void* ws, cudaStream_t st, int precision, bool v2,
-                      const void* const* presplit, void* const* tail) {
+                      const void* const* presplit) {
     const bool f16 = precision == 2;
-    RF_REQUIRE(presplit == nullptr || (v2 && f16), "rf_corr_mutual_nn: pre-split operands go with the persistent fp16-split kernel");
-    RF_REQUIRE(!v2 || f16, "rf_corr_mutual_nn: the persistent correlation kernel is the fp16-split one (precision 2)");
+    RF_REQUIRE(presplit == nullptr || (v2 && f16), "rf_corr_mutual_nn: pre-split operands go with the fp16-split kernel sequence");
+    RF_REQUIRE(!v2 || f16, "rf_corr_mutual_nn: the fused kernel sequence is the fp16-split one (precision 2)");
     RF_REQUIRE((C % (f16 ? TC_BK_F16 : TC_BK)) == 0, "rf_corr_mutual_nn: precision 1 needs C % 32 == 0, precision 2 C % 64 == 0");
     uintptr_t base = (reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255;
     const size_t esz = f16 ? 2 : 4;
@@ -1878,34 +838,24 @@ int rf_corr_argmax_tc(const float* featA, int NA, const float* featB, int NB, in
         split_tf32_kernel<<<(unsigned)((nb4 + 255) / 256), 256, 0, st>>>((const float4*)featB, (float4*)Bhi, (float4*)Blo, nb4);
         RF_LAUNCHED();
     }
-    // optional 256-wide score tiles (RF_CORR_BN=256, 3xTF32 only): the featA slab (hi + lo) is fetched once per 256 columns
-    const bool wide = !f16 && NB > 128 && corr_tile_n() == 256;
-    const int BN = wide ? 256 : 128;
+    constexpr int BN = 128;
     const unsigned bk = f16 ? TC_BK_F16 : TC_BK, es = (unsigned)esz;
-    TcParams p;
+    WgParams p;
     memset(&p, 0, sizeof(p));
     p.nimg = 1;
     p.tw[0] = 128;
     p.tiles_x[0] = (NA + 127) / 128;
-    p.tile_start[0] = 0;
     for (int i = 1; i <= RF_MAX_IMGS; ++i) p.tile_start[i] = p.tiles_x[0];
     p.Ho[0] = 1; p.Wo[0] = NA;
     int rc = get_map(&p.mapA[0], Ahi, (unsigned long long)C, (unsigned long long)NA, 1, bk, 128, 1, 1, es);
-    if (!rc) rc = get_map(&p.mapAlo, Alo, (unsigned long long)C, (unsigned long long)NA, 1, bk, 128, 1, 1, es);
+    if (!rc) rc = get_map(&p.mapA2[0], Alo, (unsigned long long)C, (unsigned long long)NA, 1, bk, 128, 1, 1, es);
     if (!rc) rc = get_map(&p.mapB, Bhi, (unsigned long long)C, (unsigned long long)NB, 0, bk, BN, 0, 1, es);
     if (!rc) rc = get_map(&p.mapBlo, Blo, (unsigned long long)C, (unsigned long long)NB, 0, bk, BN, 0, 1, es);
     if (rc) return rc;
     p.R = 1; p.S = 1; p.pad = 0; p.stride = 1; p.Cin = C; p.Cout = NB;
     p.rowbest = rowbest; p.colbest = colbest; p.NA = NA; p.NB = NB;
-    if (tail != nullptr) {
-        RF_REQUIRE(v2 && (size_t)NA * sizeof(int) <= (size_t)CorrPipeCfg::OFF_T, "rf_corr_mutual_nn: fused compaction needs the persistent kernel and NA <= 49152");
-        p.tail_idx1 = static_cast<long long*>(tail[0]);
-        p.tail_idx2 = static_cast<long long*>(tail[1]);
-        p.tail_count = static_cast<int*>(tail[2]);
-        p.done_counter = static_cast<unsigned int*>(tail[3]);
-    }
-    if (v2) return launch_corr_pipe(p, p.tiles_x[0], (NB + 127) / 128, st);
-    if (f16) return launch_tc<128, MODE_CORR, false, true>(p, p.tiles_x[0], (NB + 127) / 128, st);
-    if (wide) return launch_tc<256, MODE_CORR, false>(p, p.tiles_x[0], (NB + 255) / 256, st);
-    return launch_tc<128, MODE_CORR, false>(p, p.tiles_x[0], (NB + 127) / 128, st);
+    const dim3 grid((NB + BN - 1) / BN, p.tiles_x[0]);
+    RF_REQUIRE(grid.y <= 65535u, "rf_corr_mutual_nn: NA > 8388480");
+    if (f16) return launch_wg<K_SPLIT, BN, MODE_CORR, 0>(p, grid, st);
+    return launch_wg<K_TF32X3, BN, MODE_CORR, 0>(p, grid, st);
 }

@@ -1,4 +1,4 @@
-// Batched RANSAC homography as one persistent kernel (sm_100a).
+// Batched RANSAC homography as one persistent kernel (sm_90a).
 //
 // Replaces utils/outil.py:117-164 (RANSAC), :102-113 (ScoreRANSAC), :68-87
 // (Homography: 4-point DLT through numpy/LAPACK SVD) and :97-100 (Prediction).

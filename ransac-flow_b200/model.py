@@ -18,9 +18,9 @@ _engine = ops.ENGINE_FP32
 
 
 def set_engine(engine):
-    """'fp32' (exact FMA, SIMT), 'f16x3' (tcgen05 tensor cores with fp16 hi / lo split operands and activations: fp32-GRADE,
-    22 significand bits, three MMAs per MAC - the engine that reproduces the reference's fp32 match set), 'tf32' (tcgen05,
-    fp32 activations, 10-bit operands), 'f16' (tcgen05 with fp16 activations: the fast, reduced-precision mode; the 49- /
+    """'fp32' (exact FMA, SIMT), 'f16x3' (wgmma tensor cores with fp16 hi / lo split operands and activations: fp32-GRADE,
+    22 significand bits, three MMAs per MAC - the engine that reproduces the reference's fp32 match set), 'tf32' (wgmma,
+    fp32 activations, 10-bit operands), 'f16' (wgmma with fp16 activations: the fast, reduced-precision mode; the 49- /
     1-channel head outputs stay TF32 / fp32) or 'f16-trunk' (fp16 trunk only, fine-flow networks on 'tf32')."""
     global _engine, _fine_f16
     _fine_f16 = engine != "f16-trunk"

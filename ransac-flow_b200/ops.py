@@ -14,9 +14,9 @@ from . import _lib
 from ._lib import check, lib, need_cuda, ptr, stream
 
 ENGINE_FP32 = 0      # exact fp32 FMA (SIMT)
-ENGINE_TF32 = 1      # tcgen05 tensor cores, TF32 operands, fp32 accumulate
-ENGINE_F16 = 2       # tcgen05 tensor cores, fp16 activations + weights in HBM, fp32 accumulate (ResNet-50 trunk)
-ENGINE_SPLIT = 4     # tcgen05 tensor cores, fp16 hi / lo split activations + weights (22 significand bits, 3 MMAs per MAC): fp32-grade
+ENGINE_TF32 = 1      # wgmma tensor cores, TF32 operands, fp32 accumulate
+ENGINE_F16 = 2       # wgmma tensor cores, fp16 activations + weights in HBM, fp32 accumulate (ResNet-50 trunk)
+ENGINE_SPLIT = 4     # wgmma tensor cores, fp16 hi / lo split activations + weights (22 significand bits, 3 MMAs per MAC): fp32-grade
 
 
 def to_split(x):
@@ -246,13 +246,14 @@ def corr_mutual_nn(featA, featB, precision=0):
 SAMPLES_INDEX, SAMPLES_MOD, SAMPLES_PHILOX64 = 0, 1, 2
 
 
-def philox_words(nbIter, nbPoint, device):
+def philox_words(nbIter, nbPoint, device, generator=None):
     """(nbIter, nbPoint) full-range 64-bit words from torch's CUDA generator: element i is (x << 32) | y of the curand4 call
     whose x torch.randint(M, (nbIter, nbPoint), device='cuda') reduces modulo M from the same generator state (and the
     generator advances by the same offset).  With ``SAMPLES_PHILOX64`` the RANSAC kernel therefore sees the reference's
-    seeded sample stream (utils/outil.py:120) with M read on the device; the draw is graph-capturable."""
+    seeded sample stream (utils/outil.py:120) with M read on the device; the draw is graph-capturable.  ``generator``: a CUDA
+    generator of its own instead of torch's default one."""
     assert nbIter * nbPoint <= 256 * 1024, "beyond this size ATen maps several elements to one Philox subsequence"
-    return torch.empty((nbIter, nbPoint), dtype=torch.int64, device=device).random_(-2 ** 63, None)
+    return torch.empty((nbIter, nbPoint), dtype=torch.int64, device=device).random_(-2 ** 63, None, generator=generator)
 
 
 def corr_mutual_nn_presplit(A_hi, A_lo, B_hi, B_lo):

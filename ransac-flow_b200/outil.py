@@ -1,4 +1,4 @@
-"""Drop-in for the reference's ``outil`` module (utils/outil.py) on the B200 library.
+"""Drop-in for the reference's ``outil`` module (utils/outil.py) on the H100 library.
 
 Same function names, argument meaning, return types and error behaviour for the
 hot-path functions; the arithmetic runs in the library's CUDA kernels.
@@ -15,7 +15,7 @@ from ._lib import RFError
 
 RF_RANSAC_OK, RF_RANSAC_NONE, RF_RANSAC_NO_MODEL, RF_RANSAC_TOO_FEW = 0, 1, 2, 3
 
-# precision of the dense correlation: 0 = exact fp32 FMA, 1 = 3xTF32 on tcgen05, 2 = fp16 split on tcgen05
+# precision of the dense correlation: 0 = exact fp32 FMA, 1 = 3xTF32 on wgmma, 2 = fp16 split on wgmma
 corr_precision = 0
 
 

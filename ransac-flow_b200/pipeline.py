@@ -44,7 +44,7 @@ def PredFlowMask_device(IsTensor, featt, flowCoarse, size, network, with_match21
     """PredFlowMask without the device->host copies: returns CUDA tensors
     (flow12 (1,H,W,2), match (1,1,H,W), flowDown8 (1,2,h8,w8), matchDown8 (2,1,h8,w8) = [match12, match21]).
     ``featt = None`` with ``ItTensor``: the target's fine features are computed HERE, in one two-image batch with the warped
-    source's (twice the tiles per FeatureExtractor launch: 8.1 waves on 148 SMs instead of 2 x 4.05, half the launches);
+    source's (twice the tiles per FeatureExtractor launch, half the launches);
     ``feat_box`` (a dict) receives them for the next hypotheses."""
     with torch.no_grad():
         IsSample = ops.grid_sample(IsTensor, flowCoarse, align_corners)
@@ -68,7 +68,7 @@ def PredFlowMask_device(IsTensor, featt, flowCoarse, size, network, with_match21
             corr12 = ops.corr_neigh(ft, fs, k, ld, tc)
             corr21 = ops.corr_neigh(fs, ft, k, ld, tc)
             both = Ragged(torch.cat([corr12.data, corr21.data], dim=0), corr12.hw + corr21.hw)
-        # the two heads are independent: the flow head (one image: 152 tiles in its widest layer, i.e. one full wave + 4 tiles on 148
+        # the two heads are independent: the flow head (one image: 152 tiles in its widest layer, more than one wave on 132
         # SMs) runs on the side stream and fills the tails of the matchability head's kernels (two images) and vice versa
         main, side = torch.cuda.current_stream(), _side_stream()
         if _HEADS_TWO_STREAMS and side != main:
@@ -190,6 +190,15 @@ class GraphedAligner:
         self.graphs = {}                # insertion-ordered: least recently used first
         self.max_graphs = max_graphs    # datasets with many image sizes (HPatches, MegaDepth, YFCC): LRU-bounded graph memory
         self.replayed_kernels = 0       # library kernels executed through graph replays (they bypass rf_launch_count)
+        self.generator = None           # RANSAC sample stream: torch's default CUDA generator (the reference's stream)
+
+    def use_generator(self, generator):
+        """Draw this aligner's RANSAC samples from ``generator`` (a CUDA torch.Generator of its own) instead of torch's default
+        generator.  A replay copies its generator's seed and offset into device memory that the graph reads; graphs replayed
+        concurrently on several streams must therefore not share a generator.  Call before the first graph is captured."""
+        assert not self.graphs, "use_generator: graphs already captured with another generator"
+        self.generator = generator
+        self.coarse.sample_generator = generator
 
     def _device(self, s_in, t_in):
         """The device work of one pair, queued on the current stream: (packed results, flow12 | None, (H, W), flowDown8 shape)."""
@@ -233,6 +242,8 @@ class GraphedAligner:
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
+        if self.generator is not None:
+            g.register_generator_state(self.generator)
         n0 = _lib.launch_count()
         with torch.cuda.graph(g):
             packed, flow12, size, f8shape = self._device(s_in, t_in)
@@ -381,14 +392,23 @@ class ConcurrentAligner:
     pinned result buffer and stream) replayed side by side: pairs are independent (SURVEY 8e), and a single pair leaves
     SMs idle in its small layers (the /16 grids of the trunk's late layers, the 60 x 80 heads, RANSAC), which the other
     lanes' kernels fill.  ``make_models()`` must return a fresh ``(coarseModel, network)`` per lane (layer programs cache
-    their activation buffers per module, so lanes cannot share modules).  Results are per pair and identical to what a
-    single GraphedAligner returns for it."""
+    their activation buffers per module, so lanes cannot share modules).  Every lane draws its RANSAC samples from a CUDA
+    generator of its own (``seed``): what a pair returns depends on the seed and on the pair's position in the sequence
+    given to the aligner, never on how the lanes' replays interleave in time."""
 
-    def __init__(self, make_models, lanes=2, with_match21=False, make_aligner=None):
+    def __init__(self, make_models, lanes=2, with_match21=False, make_aligner=None, seed=0):
         """``make_aligner(coarseModel, network)`` (optional): the per-lane aligner, e.g. a ``GraphedMultiAligner``."""
         mk = make_aligner or (lambda c, n: GraphedAligner(c, n, with_match21=with_match21))
         self.lanes = [mk(*make_models()) for _ in range(lanes)]
         self.streams = [torch.cuda.Stream() for _ in range(lanes)]
+        for a in self.lanes:
+            a.use_generator(torch.Generator(device=torch.device("cuda", torch.cuda.current_device())))
+        self.seed(seed)
+
+    def seed(self, s):
+        """Restart the lanes' sample streams: lane k's generator is seeded with s + k."""
+        for k, a in enumerate(self.lanes):
+            a.generator.manual_seed(s + k)
 
     @property
     def replayed_kernels(self):

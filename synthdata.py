@@ -3,7 +3,7 @@
 Workload generator, not part of the oracle and not part of the product (no reference arithmetic in here): image pairs as in
 SURVEY.md section 8(d), random network weights with the reference's state_dict
 key names (SURVEY.md section 8b), synthetic match sets for kernel-level RANSAC
-cases.  Everything is generated on the CPU generators so both arms (B200 path
+cases.  Everything is generated on the CPU generators so both arms (GPU path
 and CPU oracle) see identical bytes on any machine.
 """
 import math

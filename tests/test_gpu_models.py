@@ -73,7 +73,7 @@ def test_resnet50_conv4_vs_torchvision(rf):
 
 @pytest.mark.parametrize("engine", ["tf32", "f16"])
 def test_fine_networks_on_tensor_core_engines(rf, engine):
-    """FeatureExtractor and the two heads through the nn.Module API on the tcgen05 engines.  'f16': fp16 activations
+    """FeatureExtractor and the two heads through the nn.Module API on the wgmma engines.  'f16': fp16 activations
     (stem patches of 64 halves, fp16 pool+blur / blur, kind::f16 convs; conv3 of the heads hands fp32 to the TF32 conv4).
     10-bit operands either way: outputs close to the fp32 golden values, flow error far below 1e-3."""
     g = golden("feature_extractor")
@@ -104,7 +104,7 @@ def test_fine_networks_on_tensor_core_engines(rf, engine):
 
 def test_resnet50_conv4_f16_engine(rf):
     """Engine 'f16': the trunk with fp16 activations (stem im2col -> 192-half rows, fp16 max-pool, every bottleneck on
-    tcgen05 kind::f16).  10-bit operands like TF32: close to the fp32 golden output, and ragged == alone."""
+    wgmma fp16).  10-bit operands like TF32: close to the fp32 golden output, and ragged == alone."""
     g = golden("resnet50_conv4")
     from ransac_flow_b200.coarseAlignFeatMatch import ResNet50Conv4
     net = ResNet50Conv4(synth.resnet50_conv4_state(int(g["seed"])))

@@ -104,10 +104,9 @@ def test_pred_flow_mask_vs_reference(rf, tag, m21):
 def test_pred_flow_mask_tensor_core_engines_vs_reference(rf, eng, tag, m21):
     """The fine-flow stage of the tensor-core engines ('f16' is bench.py's default) against the UNMODIFIED reference's
     golden PredFlowMask output for a fixed coarse homography: what the reference saves (flowDown8 / matchDown8) and the
-    full-resolution flow on the pixels that sample the coarse grid away from its border stay within north_star's 1e-3
-    (measured on B200: tf32 1.6e-4 / 1.5e-4 / 1.6e-4, f16 2.4e-4 / 2.0e-4 / 2.2e-4).  Within a pixel of the border
-    grid_sample's zero padding makes the flow discontinuous in the sampling position, which amplifies 10-bit-operand
-    differences (tf32 1.4e-3, f16 1.05e-3 there): bounded by 3e-3."""
+    full-resolution flow on the pixels that sample the coarse grid away from its border stay within north_star's 1e-3.
+    Within a pixel of the border grid_sample's zero padding makes the flow discontinuous in the sampling position, which
+    amplifies 10-bit-operand differences: bounded by 3e-3."""
     g = golden("pred_flow_mask_" + tag)
     rf.model.set_engine(eng)
     try:

@@ -1,8 +1,8 @@
-"""The split engine's kernel selections pinned against each other.  The library reads RF_SPLIT_* once per process, so every variant
-runs tests/split_variant_probe.py in its own process on the same seeded inputs.  Tile shapes, epilogue warp counts and staging
-depth do not change any output element's arithmetic: BIT-identical.  The MMA sequence (three N-wide instructions per K step vs
-[B hi | B lo] as one 2N-wide instruction + A lo x B hi) changes the order in which the two cross terms are accumulated, and the
-fused down-sampling branch accumulates in one fp32 chain what the plain topology rounds to 22 bits twice: fp32-grade tolerance."""
+"""The split engine under the kernel-selection switches of earlier builds (RF_SPLIT_*, RF_CORR_MMA3; the wgmma engine has one
+kernel for all of them) and the fused / plain down-sampling topology (RF_FUSE_DOWNSAMPLE).  Every variant runs
+tests/split_variant_probe.py in its own process on the same seeded inputs.  The selection switches must not change any output
+element: BIT-identical.  The fused down-sampling branch accumulates in one fp32 chain what the plain topology rounds to 22 bits
+twice: fp32-grade tolerance."""
 import os
 import subprocess
 import sys

@@ -1,4 +1,4 @@
-"""tcgen05 engine: TF32 implicit-GEMM convolution and 3xTF32 correlation vs fp32 references."""
+"""wgmma engine: TF32 implicit-GEMM convolution and 3xTF32 correlation vs fp32 references."""
 import numpy as np
 import pytest
 import torch
@@ -52,7 +52,7 @@ F16_TOL = 2e-3           # fp16 output rounding (2^-11 relative) + fp32 accumula
     (512, 128, 1, [(60, 80)]), (192, 64, 1, [(37, 53)]), (64, 48, 3, [(12, 20)]), (128, 8, 3, [(6, 8)]), (512, 2048, 1, [(9, 5)])])
 @pytest.mark.parametrize("relu,res,stride", [(True, True, 1), (False, False, 1), (True, False, 2)])
 def test_conv2d_f16(rf, cin, cout, k, sizes, relu, res, stride):
-    """Engine 2: fp16 activations and weights through tcgen05 kind::f16, fp32 accumulation, fp16 output.  The
+    """Engine 2: fp16 activations and weights through wgmma fp16, fp32 accumulation, fp16 output.  The
     reference is an fp32 convolution of the same fp16-rounded operands."""
     g = torch.Generator().manual_seed(cin + cout * 3 + k)
     xs = [torch.randn(1, cin, h, w, generator=g).half() for h, w in sizes]
@@ -83,9 +83,9 @@ def test_conv2d_f16(rf, cin, cout, k, sizes, relu, res, stride):
     (512, 1024, 1, 2, False, [(60, 80), (30, 44)]), (128, 128, 3, 2, False, [(64, 96), (37, 41)]),
     (256, 1024, 1, 1, True, [(30, 40), (60, 80), (15, 20)]), (128, 512, 1, 1, True, [(9, 7)])])
 def test_conv2d_f16_kernel_variants(rf, monkeypatch, env, cin, cout, k, stride, res, sizes):
-    """The same fp16 convolutions through every tap-streaming kernel variant (the switches are read per call): the
-    pipelined persistent kernel (two epilogue groups, producer-issued residual prefetch), pixel-tile-fastest raster,
-    and the residual-prefetching one-tile kernel.  All must agree with the fp32 reference."""
+    """The fp16 convolutions of the ResNet-50 shapes (1x1 expansions with residual, strided 1x1 / 3x3, ragged batches) under
+    the kernel-selection switches earlier builds read (the wgmma engine has one kernel for all of them): all must agree
+    with the fp32 reference."""
     for kk, v in env.items():
         monkeypatch.setenv(kk, v)
     g = torch.Generator().manual_seed(cin + cout + k + stride)
@@ -130,7 +130,7 @@ def test_tf32_engine_falls_back_to_fp32_kernels_for_unsupported_shapes(rf):
                                            (1024, 300, 1200, 5), (32, 500, 260, 6)])
 @pytest.mark.parametrize("precision", [1, 2])
 def test_corr_3xtf32_matches_fp32_argmax(rf, C, NA, NB, seed, precision):
-    """precision 1 = 3xTF32, 2 = fp16 split (hi + lo * 2^-11, two TMEM accumulators): both carry 22 significand bits."""
+    """precision 1 = 3xTF32, 2 = fp16 split (hi + lo * 2^-11, two accumulators): both carry 22 significand bits."""
     if precision == 2 and C % 64:
         pytest.skip("fp16 split needs C % 64 == 0")
     rs = np.random.RandomState(seed)
@@ -176,10 +176,10 @@ def test_corr_kitti_shape_both_engines_agree(rf):
 @pytest.mark.parametrize("C,NA,NB,seed", [(1024, 13065, 1200, 0), (1024, 2107, 300, 1), (64, 129, 127, 2), (256, 1, 1, 4),
                                            (1024, 300, 1200, 5), (128, 5000, 130, 6), (64, 128, 128, 7), (192, 40000, 257, 8)])
 def test_corr_persistent_kernel_identical_to_one_tile_kernel(rf, monkeypatch, C, NA, NB, seed):
-    """Precision 2 has two kernel sequences (RF_CORR_V2, read per call): the persistent correlation kernel (two TMEM
-    accumulator pairs, arg-max epilogue overlapped with the next tile's MMAs, fused split / zeroing and fused mutual test +
-    compaction) must return exactly the pairs of the one-tile-per-CTA kernel - same MMAs, same (score, smallest index)
-    order - and both agree with the fp32 oracle up to arg-max ties below fp32 accumulation noise."""
+    """Precision 2 has two launch sequences (RF_CORR_V2, read per call): fused split / key zeroing and fused mutual test +
+    compaction (3 launches) must return exactly the pairs of memset / split / split / correlation / flag / compact (6) -
+    same MMAs, same (score, smallest index) order - and both agree with the fp32 oracle up to arg-max ties below fp32
+    accumulation noise."""
     rs = np.random.RandomState(seed)
     A = np.abs(rs.randn(C, NA)).astype(np.float32)
     B = np.abs(rs.randn(C, NB)).astype(np.float32)
@@ -208,9 +208,9 @@ def test_corr_persistent_kernel_identical_to_one_tile_kernel(rf, monkeypatch, C,
 @pytest.mark.parametrize("C,NA,NB,seed", [(1024, 13065, 1200, 0), (1024, 2107, 300, 1), (64, 129, 127, 2), (256, 1, 1, 4), (1024, 300, 1200, 5),
                                            (1024, 25747, 8250, 7)])
 def test_corr_presplit_operands_and_column_compaction_identical(rf, monkeypatch, C, NA, NB, seed):
-    """rf_corr_mutual_nn_presplit (operand planes written by rf_l2norm_split_nhwc, key memset, persistent kernel whose last CTA
-    runs the mutual test + compaction) == rf_corr_mutual_nn at precision 2 (split launch + separate compaction): identical
-    index lists, also with the separate column-driven / row-driven compaction kernels (RF_CORR_TAIL, RF_COMPACT_COLS)."""
+    """rf_corr_mutual_nn_presplit (operand planes written by rf_l2norm_split_nhwc, key memset, correlation kernel, mutual
+    test + compaction) == rf_corr_mutual_nn at precision 2 (split launch + separate compaction): identical index lists, with
+    the column-driven and the row-driven compaction kernels (RF_COMPACT_COLS)."""
     g = torch.Generator().manual_seed(seed)
     raw = torch.cat([torch.randn(NA + NB, C, generator=g).abs()]).cuda()
     raw[NA:NA + min(NA, NB) // 2] = raw[torch.randperm(NA, generator=g)[:min(NA, NB) // 2].cuda()] + 0.05 * raw[NA:NA + min(NA, NB) // 2]
