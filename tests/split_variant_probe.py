@@ -1,5 +1,6 @@
-"""Helper of tests/test_gpu_split_variants.py (not a test module): runs a fixed set of split-engine layers under whatever
-RF_SPLIT_* / RF_FUSE_* / RF_CORR_* switches the environment holds (the library reads them once per process) and saves the outputs.
+"""Helper of tests/test_gpu_split_variants.py (not a test module): runs a fixed set of split-engine layers, the split trunk and
+a correlation under whatever RF_FUSE_DOWNSAMPLE the environment holds (read when the trunk's split program is built) and saves
+the outputs.
 Usage: python tests/split_variant_probe.py OUT.npz"""
 import os
 import sys

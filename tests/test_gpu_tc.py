@@ -1,109 +1,59 @@
-"""wgmma engine: TF32 implicit-GEMM convolution and 3xTF32 correlation vs fp32 references."""
+"""wgmma engine: TF32 and fp16 implicit-GEMM convolutions against fp64 references of the operands the kernels consume
+(tests/wgmma_ref.py), element by element, and the 3xTF32 / fp16-split correlation against fp32 references."""
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+import wgmma_ref as R
 from oracle import outil_oracle as OO
 from test_gpu_matching import check_same
 from test_gpu_ops import ragged
 
 pytestmark = pytest.mark.gpu
-TF32_TOL = 4e-3          # two TF32-truncated operands (2^-10 each), fp32 accumulation
+TW_SWEEP_S1, TW_SWEEP_S2, ring_cases, _inputs = R.TW_SWEEP_S1, R.TW_SWEEP_S2, R.ring_cases, R.conv_inputs
 
-
-@pytest.mark.parametrize("cin,cout,k,sizes", [
+TF32_CASES = [
     (64, 49, 3, [(6, 8)]), (128, 1, 3, [(6, 8), (6, 8)]), (64, 512, 3, [(60, 80)]),
     (64, 64, 3, [(24, 32), (9, 7)]), (64, 64, 1, [(16, 16)]), (64, 256, 1, [(13, 17), (6, 5), (1, 1)]),
     (128, 128, 3, [(16, 16), (16, 16)]), (256, 64, 1, [(30, 40)]), (1024, 256, 1, [(15, 20), (30, 40)]),
     (256, 256, 3, [(15, 20), (33, 25)]), (256, 1024, 1, [(20, 15), (40, 30)]), (512, 128, 1, [(60, 80)]),
-    (64, 48, 3, [(12, 20)]), (128, 16, 3, [(6, 8)]), (32, 32, 3, [(128, 3), (3, 128)])])
+    (64, 48, 3, [(12, 20)]), (128, 16, 3, [(6, 8)]), (32, 32, 3, [(128, 3), (3, 128)]),
+    # partial N tiles of BN = 64 / 128, odd Cout (scalar stores)
+    (64, 72, 3, [(9, 13)]), (64, 136, 1, [(11, 7)]), (32, 200, 3, [(6, 5), (1, 1)]), (64, 65, 3, [(7, 9)]), (32, 97, 1, [(12, 10)]),
+    (64, 129, 3, [(5, 6)]),
+    (32, 72, 3, TW_SWEEP_S1), (64, 136, 3, TW_SWEEP_S2)] + ring_cases("tf32")
+
+
+@pytest.mark.parametrize("cin,cout,k,sizes", TF32_CASES)
 @pytest.mark.parametrize("relu,res,stride", [(True, True, 1), (False, False, 1), (True, False, 2)])
 def test_conv2d_tf32(rf, cin, cout, k, sizes, relu, res, stride):
-    g = torch.Generator().manual_seed(cin + cout * 3 + k)
-    xs = [torch.randn(1, cin, h, w, generator=g) for h, w in sizes]
-    w = torch.randn(cout, cin, k, k, generator=g) / np.sqrt(cin * k * k)
-    bias = torch.randn(cout, generator=g)
-    refs = [F.conv2d(x, w, bias, stride=stride, padding=k // 2) for x in xs]
-    rs = [torch.randn(r.shape, generator=g) for r in refs] if res else None
-    if res:
-        refs = [a + b for a, b in zip(refs, rs)]
-    if relu:
-        refs = [F.relu(r) for r in refs]
-    wp = w.permute(2, 3, 1, 0).reshape(k * k * cin, cout).contiguous().cuda()
-    wtc = w.permute(0, 2, 3, 1).reshape(cout, k * k * cin).contiguous().cuda()
-    y = rf.ops.conv2d(ragged(rf, xs), wp, bias.cuda(), cout, k, stride, k // 2, relu, ragged(rf, rs) if res else None,
-                      rf.ops.ENGINE_TF32, wtc)
-    torch.cuda.synchronize()
-    for i, r in enumerate(refs):
-        got = y.image(i).cpu()
-        assert tuple(got.shape) == tuple(r.shape)
-        err = (got - r).abs().max().item()
-        assert err <= TF32_TOL * max(1.0, r.abs().max().item()), (err, r.abs().max().item())
+    """Engine 1: the reference convolves the TF32-truncated operands in fp64.  With ReLU the output is TF32-rounded."""
+    xs, w, bias, rs = _inputs(cin + cout * 3 + k, cin, cout, k, sizes, res, stride)
+    R.check_conv(rf, 1, xs, w, bias, rs, stride, relu, "tf32 %dx%d %d->%d stride %d" % (k, k, cin, cout, stride))
 
 
-F16_TOL = 2e-3           # fp16 output rounding (2^-11 relative) + fp32 accumulation order
-
-
-@pytest.mark.parametrize("cin,cout,k,sizes", [
+F16_CASES = [
     (64, 64, 3, [(24, 32), (9, 7)]), (64, 64, 3, [(120, 160), (60, 80), (33, 47)]), (64, 64, 1, [(16, 16)]),
     (64, 256, 1, [(13, 17), (6, 5), (1, 1)]), (128, 128, 3, [(16, 16), (16, 16)]), (256, 64, 1, [(30, 40)]),
     (1024, 256, 1, [(15, 20), (30, 40)]), (256, 256, 3, [(15, 20), (33, 25)]), (256, 1024, 1, [(20, 15), (40, 30)]),
-    (512, 128, 1, [(60, 80)]), (192, 64, 1, [(37, 53)]), (64, 48, 3, [(12, 20)]), (128, 8, 3, [(6, 8)]), (512, 2048, 1, [(9, 5)])])
+    (512, 128, 1, [(60, 80)]), (192, 64, 1, [(37, 53)]), (64, 48, 3, [(12, 20)]), (128, 8, 3, [(6, 8)]), (512, 2048, 1, [(9, 5)]),
+    # the ResNet-50 shapes: 1x1 expansions, strided 1x1 / 3x3, ragged batches
+    (64, 256, 1, [(120, 160), (60, 80), (33, 47)]), (256, 64, 1, [(120, 160), (31, 17)]), (512, 1024, 1, [(60, 80), (30, 44)]),
+    (128, 128, 3, [(64, 96), (37, 41)]), (256, 1024, 1, [(30, 40), (60, 80), (15, 20)]), (128, 512, 1, [(9, 7)]),
+    # partial N tiles of BN = 128
+    (64, 72, 3, [(9, 13)]), (64, 136, 1, [(11, 7)]), (128, 200, 3, [(6, 5), (1, 1)]),
+    (64, 72, 3, TW_SWEEP_S1), (64, 136, 3, TW_SWEEP_S2)] + ring_cases("f16")
+
+
+@pytest.mark.parametrize("cin,cout,k,sizes", F16_CASES)
 @pytest.mark.parametrize("relu,res,stride", [(True, True, 1), (False, False, 1), (True, False, 2)])
 def test_conv2d_f16(rf, cin, cout, k, sizes, relu, res, stride):
-    """Engine 2: fp16 activations and weights through wgmma fp16, fp32 accumulation, fp16 output.  The
-    reference is an fp32 convolution of the same fp16-rounded operands."""
-    g = torch.Generator().manual_seed(cin + cout * 3 + k)
-    xs = [torch.randn(1, cin, h, w, generator=g).half() for h, w in sizes]
-    w = (torch.randn(cout, cin, k, k, generator=g) / np.sqrt(cin * k * k)).half()
-    bias = torch.randn(cout, generator=g)
-    refs = [F.conv2d(x.float(), w.float(), bias, stride=stride, padding=k // 2) for x in xs]
-    rs = [torch.randn(r.shape, generator=g).half() for r in refs] if res else None
-    if res:
-        refs = [a + b.float() for a, b in zip(refs, rs)]
-    if relu:
-        refs = [F.relu(r) for r in refs]
-    wtc = w.permute(0, 2, 3, 1).reshape(cout, k * k * cin).contiguous().cuda()
-    y = rf.ops.conv2d(ragged(rf, xs), None, bias.cuda(), cout, k, stride, k // 2, relu, ragged(rf, rs) if res else None,
-                      rf.ops.ENGINE_F16, wtc)
-    torch.cuda.synchronize()
-    assert y.data.dtype == torch.float16
-    for i, r in enumerate(refs):
-        got = y.image(i).float().cpu()
-        assert tuple(got.shape) == tuple(r.shape)
-        err = (got - r).abs().max().item()
-        assert err <= F16_TOL * max(1.0, r.abs().max().item()), (err, r.abs().max().item())
-
-
-@pytest.mark.parametrize("env", [{"RF_TC_PIPE": "1"}, {"RF_TC_PIPE": "0", "RF_TC_RASTER": "0"}, {"RF_TC_PIPE": "0", "RF_TC_RESPF": "1"},
-                                 {"RF_TC_PIPE": "1", "RF_TC_RASTER": "0"}])
-@pytest.mark.parametrize("cin,cout,k,stride,res,sizes", [
-    (64, 256, 1, 1, True, [(120, 160), (60, 80), (33, 47)]), (256, 64, 1, 1, False, [(120, 160), (31, 17)]),
-    (512, 1024, 1, 2, False, [(60, 80), (30, 44)]), (128, 128, 3, 2, False, [(64, 96), (37, 41)]),
-    (256, 1024, 1, 1, True, [(30, 40), (60, 80), (15, 20)]), (128, 512, 1, 1, True, [(9, 7)])])
-def test_conv2d_f16_kernel_variants(rf, monkeypatch, env, cin, cout, k, stride, res, sizes):
-    """The fp16 convolutions of the ResNet-50 shapes (1x1 expansions with residual, strided 1x1 / 3x3, ragged batches) under
-    the kernel-selection switches earlier builds read (the wgmma engine has one kernel for all of them): all must agree
-    with the fp32 reference."""
-    for kk, v in env.items():
-        monkeypatch.setenv(kk, v)
-    g = torch.Generator().manual_seed(cin + cout + k + stride)
-    xs = [torch.randn(1, cin, h, w, generator=g).half() for h, w in sizes]
-    w = (torch.randn(cout, cin, k, k, generator=g) / np.sqrt(cin * k * k)).half()
-    bias = torch.randn(cout, generator=g)
-    refs = [F.conv2d(x.float(), w.float(), bias, stride=stride, padding=k // 2) for x in xs]
-    rs = [torch.randn(r.shape, generator=g).half() for r in refs] if res else None
-    if res:
-        refs = [a + b.float() for a, b in zip(refs, rs)]
-    refs = [F.relu(r) for r in refs]
-    wtc = w.permute(0, 2, 3, 1).reshape(cout, k * k * cin).contiguous().cuda()
-    y = rf.ops.conv2d(ragged(rf, xs), None, bias.cuda(), cout, k, stride, k // 2, True, ragged(rf, rs) if res else None,
-                      rf.ops.ENGINE_F16, wtc)
-    torch.cuda.synchronize()
-    for i, r in enumerate(refs):
-        err = (y.image(i).float().cpu() - r).abs().max().item()
-        assert err <= F16_TOL * max(1.0, r.abs().max().item()), (env, err, r.abs().max().item())
+    """Engine 2: fp16 activations, weights and residual through wgmma fp16, fp32 accumulation, fp16 output.  The reference
+    convolves the same fp16 values in fp64."""
+    xs, w, bias, rs = _inputs(cin + cout * 3 + k, cin, cout, k, sizes, res, stride)
+    _, y = R.check_conv(rf, 2, xs, w, bias, rs, stride, relu, "f16 %dx%d %d->%d stride %d" % (k, k, cin, cout, stride))
+    assert y.dtype == torch.float16
 
 
 def test_f16_engine_saturates_and_rejects_unsupported_shapes(rf):
