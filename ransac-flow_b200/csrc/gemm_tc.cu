@@ -1,13 +1,18 @@
 // Tensor-core engine (sm_90a): implicit-GEMM convolutions and the correlation with its row / column arg-max, on wgmma.
 //
-// One kernel template.  A CTA computes one output tile of 128 pixels (correlation: 128 rows of featA) x BN channels (columns of
-// featB) with 288 threads:
+// One kernel template.  An output tile is 128 pixels (correlation: 128 rows of featA) x BN channels (columns of featB); a CTA
+// has 288 threads:
 //   warp 8        : TMA producer.  A = box (channels, tw, th[, 2 planes]) of the NHWC image at the tap's offset (out-of-bounds
 //                   zero fill is the zero padding, the traversal stride is the convolution stride), B = box of the K-major
 //                   weight matrix; both 128-byte swizzled, completion counted on the stage's mbarrier.
 //   warpgroups 0-1: tile rows 0..63 / 64..127.  wgmma.mma_async from the stage's descriptors into register accumulators; one
 //                   wgmma group stays in flight while the stage before it is handed back to the producer.  The epilogue
 //                   works on the registers: bias, residual, ReLU, conversion, store (convolution) or arg-max keys (correlation).
+// Convolutions are persistent: tile t (pixel tiles fastest) runs on CTA t mod gridDim.x, and the ring runs on across tile
+// boundaries, so one tile's epilogue overlaps the loads of the next.  fp16 and split outputs take one more ring stage per tile
+// (the epilogue slot): the producer TMA-loads the residual tile into it, the consumers add it and write the result back in
+// place, one thread TMA-stores the slot and hands it back once the store has read it.  fp32 outputs (rows of 49 or 1 floats
+// are not 16-byte multiples) keep register stores.  The correlation runs one tile per CTA.
 // Operand kinds:
 //   K_TF32   : fp32 operands, TF32 MMAs (engine 1);
 //   K_F16    : fp16 operands (engines 2 and 3);
@@ -34,9 +39,12 @@ constexpr int WG_THREADS = 288;                       // two consumer warpgroups
 struct alignas(64) WgParams {
     CUtensorMap mapA[RF_MAX_IMGS];        // per image: input (C, W, H[, 2]); correlation: A hi (C, NA, 1)
     CUtensorMap mapA2[RF_MAX_IMGS];       // dual-input 1x1: the second input (Cin2, W2, H2, 2); correlation: [0] = A lo
+    CUtensorMap mapY[RF_MAX_IMGS];        // fp16 / split output per image: (Cout, Wo, Ho[, 2]), box (64, tw, th[, 2])
+    CUtensorMap mapR[RF_MAX_IMGS];        // its residual, same geometry
     CUtensorMap mapB;                     // weights (K, Cout[, 2]); correlation: B hi (C, NB)
     CUtensorMap mapBlo;                   // correlation: B lo
     int nimg;
+    int tiles, ntiles;                    // convolution: pixel tiles of the batch, and times the N tiles
     int tile_start[RF_MAX_IMGS + 1];      // prefix sums of pixel tiles per image
     int tiles_x[RF_MAX_IMGS];
     int tw[RF_MAX_IMGS];                  // tile width (tile height = 128 / tw)
@@ -108,25 +116,42 @@ wg_kernel(const __grid_constant__ WgParams p) {
     constexpr int STAGES = Cfg::STAGES;
     constexpr int BK = (KIND == K_TF32 || KIND == K_TF32X3) ? TC_BK : TC_BK_F16;
     constexpr int NACC = KIND == K_SPLIT ? 2 : 1;
+    // fp16 / split convolution outputs: epilogue slot + TMA store.  One 64-channel box of the output tile is 128 pixel rows of
+    // 128 bytes per plane, swizzled like the operand tiles; the BN / 64 boxes of a tile fit one stage in every instance.
+    constexpr bool SLOT = MODE == MODE_CONV && OUT != O_F32;
+    constexpr int BOX_BYTES = (OUT == O_SPLIT ? 2 : 1) * 128 * 128;
+    static_assert(!SLOT || (BN / 64) * BOX_BYTES <= Cfg::STAGE_BYTES, "the output tile fits one stage");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
     uint64_t* empty = full + STAGES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    // ---- tile decode.  Correlation: column tiles fastest, so that the CTAs sharing a 128-row slab of featA run together ----
-    const int mtile = MODE == MODE_CORR ? blockIdx.y : blockIdx.x;
-    const int ntile = MODE == MODE_CORR ? blockIdx.x : blockIdx.y;
-    int img = 0;
-#pragma unroll
-    for (int j = 1; j < RF_MAX_IMGS; ++j) img += (j < p.nimg && mtile >= p.tile_start[j]) ? 1 : 0;
-    const int tloc = mtile - p.tile_start[img];
-    const int tw = p.tw[img], th = 128 / tw;
-    const int tyi = tloc / p.tiles_x[img], txi = tloc - tyi * p.tiles_x[img];
-    const int ox0 = txi * tw, oy0 = tyi * th;
-    const int n0 = ntile * BN;
     const int kc = p.Cin / BK;
     const int KI = p.R * p.S * kc;
+
+    // ---- tiles.  Convolution: tile t -> pixel tile t % tiles, N tile t / tiles, on CTA t mod gridDim.x.  Correlation: one tile
+    // per CTA, column tiles fastest, so that the CTAs sharing a 128-row slab of featA run together ----
+    const int t_first = MODE == MODE_CORR ? 0 : (int)blockIdx.x;
+    const int t_step = MODE == MODE_CORR ? 1 : (int)gridDim.x;
+    const int t_end = MODE == MODE_CORR ? 1 : p.ntiles;
+    struct Tile { int img, tw, ox0, oy0, n0; };
+    auto decode = [&](int t) {
+        const int mtile = MODE == MODE_CORR ? (int)blockIdx.y : t % p.tiles;
+        const int ntile = MODE == MODE_CORR ? (int)blockIdx.x : t / p.tiles;
+        Tile T;
+        T.img = 0;
+#pragma unroll
+        for (int j = 1; j < RF_MAX_IMGS; ++j) T.img += (j < p.nimg && mtile >= p.tile_start[j]) ? 1 : 0;
+        const int tloc = mtile - p.tile_start[T.img];
+        T.tw = p.tw[T.img];
+        const int tyi = tloc / p.tiles_x[T.img], txi = tloc - tyi * p.tiles_x[T.img];
+        T.ox0 = txi * T.tw;
+        T.oy0 = tyi * (128 / T.tw);
+        T.n0 = ntile * BN;
+        return T;
+    };
+    // 64-channel boxes of the tile that hold output channels (BN = 128 with Cout - n0 <= 64: the second box is all outside)
+    auto boxes = [&](const Tile& T) { return BN == 64 || T.n0 + 64 >= p.Cout ? 1 : 2; };
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }
@@ -137,33 +162,61 @@ wg_kernel(const __grid_constant__ WgParams p) {
     if (warp == 8) {
         // =============================== TMA producer ===============================
         if (lane == 0) {
-            tma_prefetch_desc(&p.mapA[img]);
             tma_prefetch_desc(&p.mapB);
-            for (int it = 0; it < KI; ++it) {
-                const int st = it % STAGES, ph = (it / STAGES) & 1;
-                mbar_wait(&empty[st], ph ^ 1);
-                uint8_t* sa = smem + st * Cfg::STAGE_BYTES;
-                uint8_t* sb = sa + Cfg::A_BYTES;
-                mbar_expect_tx(&full[st], Cfg::STAGE_BYTES);
-                if constexpr (MODE == MODE_CORR) {
-                    const int c0 = it * BK;
-                    tma_load_3d(sa, &p.mapA[0], &full[st], c0, ox0, 0);
-                    tma_load_3d(sa + TC_A_BYTES, &p.mapA2[0], &full[st], c0, ox0, 0);
-                    tma_load_2d(sb, &p.mapB, &full[st], c0, n0);
-                    tma_load_2d(sb + Cfg::B_PLANE, &p.mapBlo, &full[st], c0, n0);
-                } else {
-                    const int tap = it / kc, cc = it - tap * kc;
-                    const int r = tap / p.S, s = tap - r * p.S;
-                    const int c0 = cc * BK, x = ox0 * p.stride + s - p.pad, y = oy0 * p.stride + r - p.pad;
-                    const int kcol = tap * p.Cin + c0;
-                    if constexpr (KIND == K_SPLIT) {       // one 4-D box brings [hi tile | lo tile]
-                        if (cc < p.kc1) tma_load_4d(sa, &p.mapA[img], &full[st], c0, x, y, 0);
-                        else tma_load_4d(sa, &p.mapA2[img], &full[st], (cc - p.kc1) * BK, ox0 * p.stride2, oy0 * p.stride2, 0);
-                        tma_load_3d(sb, &p.mapB, &full[st], kcol, n0, 0);
-                    } else {
-                        tma_load_3d(sa, &p.mapA[img], &full[st], c0, x, y);
-                        tma_load_2d(sb, &p.mapB, &full[st], kcol, n0);
+            uint32_t prefetched = 0;              // images whose tensor maps have been prefetched
+            int st = 0;
+            uint32_t ph = 0;
+            for (int t = t_first; t < t_end; t += t_step) {
+                const Tile T = decode(t);
+                if (!((prefetched >> T.img) & 1u)) {
+                    prefetched |= 1u << T.img;
+                    tma_prefetch_desc(&p.mapA[T.img]);
+                    if constexpr (SLOT) {
+                        tma_prefetch_desc(&p.mapY[T.img]);
+                        if (p.residual) tma_prefetch_desc(&p.mapR[T.img]);
                     }
+                }
+                for (int it = 0; it < KI; ++it) {
+                    mbar_wait(&empty[st], ph ^ 1);
+                    uint8_t* sa = smem + st * Cfg::STAGE_BYTES;
+                    uint8_t* sb = sa + Cfg::A_BYTES;
+                    mbar_expect_tx(&full[st], Cfg::STAGE_BYTES);
+                    if constexpr (MODE == MODE_CORR) {
+                        const int c0 = it * BK;
+                        tma_load_3d(sa, &p.mapA[0], &full[st], c0, T.ox0, 0);
+                        tma_load_3d(sa + TC_A_BYTES, &p.mapA2[0], &full[st], c0, T.ox0, 0);
+                        tma_load_2d(sb, &p.mapB, &full[st], c0, T.n0);
+                        tma_load_2d(sb + Cfg::B_PLANE, &p.mapBlo, &full[st], c0, T.n0);
+                    } else {
+                        const int tap = it / kc, cc = it - tap * kc;
+                        const int r = tap / p.S, s = tap - r * p.S;
+                        const int c0 = cc * BK, x = T.ox0 * p.stride + s - p.pad, y = T.oy0 * p.stride + r - p.pad;
+                        const int kcol = tap * p.Cin + c0;
+                        if constexpr (KIND == K_SPLIT) {       // one 4-D box brings [hi tile | lo tile]
+                            if (cc < p.kc1) tma_load_4d(sa, &p.mapA[T.img], &full[st], c0, x, y, 0);
+                            else tma_load_4d(sa, &p.mapA2[T.img], &full[st], (cc - p.kc1) * BK, T.ox0 * p.stride2, T.oy0 * p.stride2, 0);
+                            tma_load_3d(sb, &p.mapB, &full[st], kcol, T.n0, 0);
+                        } else {
+                            tma_load_3d(sa, &p.mapA[T.img], &full[st], c0, x, y);
+                            tma_load_2d(sb, &p.mapB, &full[st], kcol, T.n0);
+                        }
+                    }
+                    if (++st == STAGES) { st = 0; ph ^= 1; }
+                }
+                if constexpr (SLOT) {                  // the epilogue slot: the residual tile, or just the hand-over
+                    mbar_wait(&empty[st], ph ^ 1);
+                    if (p.residual) {
+                        const int nb = boxes(T);
+                        uint8_t* slot = smem + st * Cfg::STAGE_BYTES;
+                        mbar_expect_tx(&full[st], nb * BOX_BYTES);
+                        for (int b = 0; b < nb; ++b) {
+                            if constexpr (OUT == O_SPLIT) tma_load_4d(slot + b * BOX_BYTES, &p.mapR[T.img], &full[st], T.n0 + 64 * b, T.ox0, T.oy0, 0);
+                            else tma_load_3d(slot + b * BOX_BYTES, &p.mapR[T.img], &full[st], T.n0 + 64 * b, T.ox0, T.oy0);
+                        }
+                    } else {
+                        mbar_arrive(&full[st]);
+                    }
+                    if (++st == STAGES) { st = 0; ph ^= 1; }
                 }
             }
         }
@@ -172,129 +225,174 @@ wg_kernel(const __grid_constant__ WgParams p) {
 
     // =============================== consumers: warpgroup g owns tile rows 64g .. 64g + 63 ===============================
     const int g = warp >> 2;
-    float acc[NACC][BN / 2];
-#pragma unroll
-    for (int a = 0; a < NACC; ++a)
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[a][i] = 0.f;
-    for (int it = 0; it < KI; ++it) {
-        const int st = it % STAGES, ph = (it / STAGES) & 1;
-        mbar_wait(&full[st], ph);
-        const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
-        wg_fence();
-        mma_block<KIND, BN, NACC>(acc, sa + g * (64 * 128), sa + Cfg::A_BYTES);
-        wg_commit();
-        wg_wait<1>();                             // the previous stage's MMAs are done: hand it back
-        if (it > 0) mbar_arrive(&empty[(it - 1) % STAGES]);
-    }
-    wg_wait<0>();
-#pragma unroll
-    for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
-
     // accumulator fragment: d[4j + 2h + e] = row 16 * (warp % 4) + lane / 4 + 8h, column 8j + 2 * (lane % 4) + e
     const int rbase = 64 * g + 16 * (warp & 3) + (lane >> 2);
     const int cbase = 2 * (lane & 3);
-    auto value = [&](int i) -> float {
-        if constexpr (KIND == K_SPLIT) return fmaf(acc[1][i], 0.00048828125f, acc[0][i]);
-        else return acc[0][i];
-    };
+    auto before = [](int s) { return s == 0 ? STAGES - 1 : s - 1; };
+    int st = 0;
+    uint32_t ph = 0;
+    bool stored = false;                          // the stage before `st` is an epilogue slot a TMA store may still be reading
+    for (int t = t_first; t < t_end; t += t_step) {
+        const Tile T = decode(t);
+        float acc[NACC][BN / 2];
+#pragma unroll
+        for (int a = 0; a < NACC; ++a)
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[a][i] = 0.f;
+        for (int it = 0; it < KI; ++it) {
+            mbar_wait(&full[st], ph);
+            const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
+            wg_fence();
+            mma_block<KIND, BN, NACC>(acc, sa + g * (64 * 128), sa + Cfg::A_BYTES);
+            wg_commit();
+            wg_wait<1>();                         // the previous stage's MMAs are done: hand it back
+            if (it > 0) {
+                mbar_arrive(&empty[before(st)]);
+            } else if (SLOT && stored) {          // the previous tile's slot, once its store has read it
+                if (threadIdx.x == 0) bulk_wait_read();
+                mbar_arrive(&empty[before(st)]);
+            }
+            if (++st == STAGES) { st = 0; ph ^= 1; }
+        }
+        wg_wait<0>();
+#pragma unroll
+        for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
+        mbar_arrive(&empty[before(st)]);         // the tile's last K block
 
-    if constexpr (MODE == MODE_CONV) {
+        auto value = [&](int i) -> float {
+            if constexpr (KIND == K_SPLIT) return fmaf(acc[1][i], 0.00048828125f, acc[0][i]);
+            else return acc[0][i];
+        };
+
+        if constexpr (SLOT) {
+            // element (pixel m, channel c) of the tile: box c / 64, row m, 16-byte chunk ((c % 64) / 8) ^ (m % 8); lo plane
+            // 128 rows further.  Each thread reads its residual elements and overwrites them with its outputs.
+            mbar_wait(&full[st], ph);
+            uint8_t* slot = smem + st * Cfg::STAGE_BYTES;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int m = rbase + 8 * h;
-            const int py = m / tw, px = m - py * tw;
-            const int oy = oy0 + py, ox = ox0 + px;
-            if (oy >= p.Ho[img] || ox >= p.Wo[img]) continue;
-            const long long pix = p.out_pix[img] + (long long)oy * p.Wo[img] + ox;
+            for (int h = 0; h < 2; ++h) {
+                const int m = rbase + 8 * h;
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                const int n = n0 + 8 * j + cbase;
-                if (n >= p.Cout) continue;
-                const bool two = n + 1 < p.Cout;
-                float v0 = value(4 * j + 2 * h), v1 = value(4 * j + 2 * h + 1);
-                if (p.bias) { v0 += __ldg(p.bias + n); if (two) v1 += __ldg(p.bias + n + 1); }
-                const long long o = pix * p.Cout + n;
-                if (p.residual) {
-                    if constexpr (OUT == O_F32) {
-                        const float* r = static_cast<const float*>(p.residual) + o;
-                        v0 += __ldg(r); if (two) v1 += __ldg(r + 1);
-                    } else if constexpr (OUT == O_F16) {
-                        const float2 r = __half22float2(*reinterpret_cast<const __half2*>(static_cast<const __half*>(p.residual) + o));
-                        v0 += r.x; v1 += r.y;
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int c = 8 * j + cbase, n = T.n0 + c;
+                    if (n >= p.Cout) continue;    // Cout % 8 == 0: both channels of the pair exist
+                    float v0 = value(4 * j + 2 * h), v1 = value(4 * j + 2 * h + 1);
+                    if (p.bias) { v0 += __ldg(p.bias + n); v1 += __ldg(p.bias + n + 1); }
+                    uint8_t* e = slot + (c >> 6) * BOX_BYTES + m * 128 + ((((c & 63) >> 3) ^ (m & 7)) << 4) + (c & 7) * 2;
+                    if (p.residual) {
+                        if constexpr (OUT == O_F16) {
+                            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(e));
+                            v0 += r.x; v1 += r.y;
+                        } else {
+                            const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(e));
+                            const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(e + 128 * 128));
+                            v0 += fmaf(rl.x, 0.00048828125f, rh.x); v1 += fmaf(rl.y, 0.00048828125f, rh.y);
+                        }
+                    }
+                    if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                    if constexpr (OUT == O_F16) {
+                        *reinterpret_cast<__half2*>(e) = pack_sat(v0, v1);
                     } else {
-                        const __half* r = static_cast<const __half*>(p.residual) + o;
-                        const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(r));
-                        const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(r + p.plane));
-                        v0 += fmaf(rl.x, 0.00048828125f, rh.x); v1 += fmaf(rl.y, 0.00048828125f, rh.y);
+                        __half2 hi, lo;
+                        split2(v0, v1, hi, lo);
+                        *reinterpret_cast<__half2*>(e) = hi;
+                        *reinterpret_cast<__half2*>(e + 128 * 128) = lo;
                     }
                 }
-                if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                if constexpr (OUT == O_F32) {
+            }
+            fence_proxy_async();                  // the generic-proxy writes -> visible to the TMA store
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            if (threadIdx.x == 0) {
+                const int nb = boxes(T);
+                for (int b = 0; b < nb; ++b) {
+                    if constexpr (OUT == O_SPLIT) tma_store_4d(&p.mapY[T.img], slot + b * BOX_BYTES, T.n0 + 64 * b, T.ox0, T.oy0, 0);
+                    else tma_store_3d(&p.mapY[T.img], slot + b * BOX_BYTES, T.n0 + 64 * b, T.ox0, T.oy0);
+                }
+                bulk_commit();
+            }
+            stored = true;
+            if (++st == STAGES) { st = 0; ph ^= 1; }
+        } else if constexpr (MODE == MODE_CONV) {
+            const int img = T.img, tw = T.tw;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int m = rbase + 8 * h;
+                const int py = m / tw, px = m - py * tw;
+                const int oy = T.oy0 + py, ox = T.ox0 + px;
+                if (oy >= p.Ho[img] || ox >= p.Wo[img]) continue;
+                const long long pix = p.out_pix[img] + (long long)oy * p.Wo[img] + ox;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int n = T.n0 + 8 * j + cbase;
+                    if (n >= p.Cout) continue;
+                    const bool two = n + 1 < p.Cout;
+                    float v0 = value(4 * j + 2 * h), v1 = value(4 * j + 2 * h + 1);
+                    if (p.bias) { v0 += __ldg(p.bias + n); if (two) v1 += __ldg(p.bias + n + 1); }
+                    const long long o = pix * p.Cout + n;
+                    if (p.residual) {
+                        const float* r = static_cast<const float*>(p.residual) + o;
+                        v0 += __ldg(r); if (two) v1 += __ldg(r + 1);
+                    }
+                    if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
                     if (p.round_out) { v0 = round_tf32(v0); v1 = round_tf32(v1); }
                     float* y = static_cast<float*>(p.y) + o;
                     if (two && (p.Cout & 1) == 0) *reinterpret_cast<float2*>(y) = make_float2(v0, v1);
                     else { y[0] = v0; if (two) y[1] = v1; }
-                } else if constexpr (OUT == O_F16) {
-                    *reinterpret_cast<__half2*>(static_cast<__half*>(p.y) + o) = pack_sat(v0, v1);
-                } else {
-                    __half2 hi, lo;
-                    split2(v0, v1, hi, lo);
-                    __half* y = static_cast<__half*>(p.y) + o;
-                    *reinterpret_cast<__half2*>(y) = hi;
-                    *reinterpret_cast<__half2*>(y + p.plane) = lo;
                 }
             }
-        }
-    } else {
-        // utils/outil.py:36-37: per row the best (score, smallest column) key, per column the best (score, smallest row) key.
-        // Rows: the four lanes of a quad share a row.  Columns: the eight row groups of a warp by shuffles, then the eight
-        // warps through shared memory (the stages are idle: every TMA load has been consumed).
-        unsigned long long* sCol = reinterpret_cast<unsigned long long*>(smem);       // [8 warps][BN]
-        const int row0 = ox0 + rbase, row1 = row0 + 8;
-        const bool rv0 = row0 < p.NA, rv1 = row1 < p.NA;
-        unsigned long long rb0 = 0ull, rb1 = 0ull;
-        asm volatile("bar.sync 1, 256;" ::: "memory");          // both warpgroups are past their last wgmma reads
+        } else {
+            // utils/outil.py:36-37: per row the best (score, smallest column) key, per column the best (score, smallest row) key.
+            // Rows: the four lanes of a quad share a row.  Columns: the eight row groups of a warp by shuffles, then the eight
+            // warps through shared memory (the stages are idle: every TMA load has been consumed).
+            const int n0 = T.n0;
+            unsigned long long* sCol = reinterpret_cast<unsigned long long*>(smem);       // [8 warps][BN]
+            const int row0 = T.ox0 + rbase, row1 = row0 + 8;
+            const bool rv0 = row0 < p.NA, rv1 = row1 < p.NA;
+            unsigned long long rb0 = 0ull, rb1 = 0ull;
+            asm volatile("bar.sync 1, 256;" ::: "memory");          // both warpgroups are past their last wgmma reads
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
+            for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-                const int c = 8 * j + cbase + e, col = n0 + c;
-                const bool cv = col < p.NB;
-                const float s0 = value(4 * j + e), s1 = value(4 * j + 2 + e);
-                unsigned long long ck = 0ull;
-                if (cv) {
-                    if (rv0) { const unsigned long long k = pack_key(s0, (uint32_t)col); rb0 = k > rb0 ? k : rb0; ck = pack_key(s0, (uint32_t)row0); }
-                    if (rv1) { const unsigned long long k = pack_key(s1, (uint32_t)col); rb1 = k > rb1 ? k : rb1;
-                               const unsigned long long k1 = pack_key(s1, (uint32_t)row1); ck = k1 > ck ? k1 : ck; }
+                for (int e = 0; e < 2; ++e) {
+                    const int c = 8 * j + cbase + e, col = n0 + c;
+                    const bool cv = col < p.NB;
+                    const float s0 = value(4 * j + e), s1 = value(4 * j + 2 + e);
+                    unsigned long long ck = 0ull;
+                    if (cv) {
+                        if (rv0) { const unsigned long long k = pack_key(s0, (uint32_t)col); rb0 = k > rb0 ? k : rb0; ck = pack_key(s0, (uint32_t)row0); }
+                        if (rv1) { const unsigned long long k = pack_key(s1, (uint32_t)col); rb1 = k > rb1 ? k : rb1;
+                                   const unsigned long long k1 = pack_key(s1, (uint32_t)row1); ck = k1 > ck ? k1 : ck; }
+                    }
+#pragma unroll
+                    for (int off = 4; off < 32; off <<= 1) {
+                        const unsigned long long o = __shfl_xor_sync(0xffffffffu, ck, off);
+                        ck = o > ck ? o : ck;
+                    }
+                    if (lane < 4) sCol[warp * BN + c] = ck;
                 }
-#pragma unroll
-                for (int off = 4; off < 32; off <<= 1) {
-                    const unsigned long long o = __shfl_xor_sync(0xffffffffu, ck, off);
-                    ck = o > ck ? o : ck;
-                }
-                if (lane < 4) sCol[warp * BN + c] = ck;
             }
-        }
 #pragma unroll
-        for (int off = 1; off < 4; off <<= 1) {
-            const unsigned long long o0 = __shfl_xor_sync(0xffffffffu, rb0, off), o1 = __shfl_xor_sync(0xffffffffu, rb1, off);
-            rb0 = o0 > rb0 ? o0 : rb0;
-            rb1 = o1 > rb1 ? o1 : rb1;
-        }
-        if ((lane & 3) == 0) {
-            if (rv0 && rb0 != 0ull) atomicMax(p.rowbest + row0, rb0);
-            if (rv1 && rb1 != 0ull) atomicMax(p.rowbest + row1, rb1);
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        for (int c = threadIdx.x; c < BN; c += 256) {
-            if (n0 + c >= p.NB) continue;
-            unsigned long long cb = 0ull;
+            for (int off = 1; off < 4; off <<= 1) {
+                const unsigned long long o0 = __shfl_xor_sync(0xffffffffu, rb0, off), o1 = __shfl_xor_sync(0xffffffffu, rb1, off);
+                rb0 = o0 > rb0 ? o0 : rb0;
+                rb1 = o1 > rb1 ? o1 : rb1;
+            }
+            if ((lane & 3) == 0) {
+                if (rv0 && rb0 != 0ull) atomicMax(p.rowbest + row0, rb0);
+                if (rv1 && rb1 != 0ull) atomicMax(p.rowbest + row1, rb1);
+            }
+            asm volatile("bar.sync 1, 256;" ::: "memory");
+            for (int c = threadIdx.x; c < BN; c += 256) {
+                if (n0 + c >= p.NB) continue;
+                unsigned long long cb = 0ull;
 #pragma unroll
-            for (int w = 0; w < 8; ++w) { const unsigned long long k = sCol[w * BN + c]; cb = k > cb ? k : cb; }
-            if (cb != 0ull) atomicMax(p.colbest + n0 + c, cb);
+                for (int w = 0; w < 8; ++w) { const unsigned long long k = sCol[w * BN + c]; cb = k > cb ? k : cb; }
+                if (cb != 0ull) atomicMax(p.colbest + n0 + c, cb);
+            }
         }
     }
+    if constexpr (SLOT)
+        if (threadIdx.x == 0) bulk_wait();        // the last tile's stores complete before the CTA (and its shared memory) goes
 }
 
 
@@ -620,9 +718,15 @@ static int launch_wg(const WgParams& p, dim3 grid, cudaStream_t st) {
     return 0;
 }
 
+// persistent: at most as many CTAs as fit the GPU at once, each looping over its share of the tiles
+template <int KIND, int BN, int OUT>
+static int launch_conv_bn(const WgParams& p, cudaStream_t st) {
+    const int resident = WgCfg<KIND, BN, MODE_CONV>::CTAS_PER_SM * num_sms();
+    return launch_wg<KIND, BN, MODE_CONV, OUT>(p, dim3(p.ntiles < resident ? p.ntiles : resident), st);
+}
 template <int KIND, int OUT>
-static int launch_conv(const WgParams& p, int BN, int tiles, int nt, cudaStream_t st) {
-    return BN == 128 ? launch_wg<KIND, 128, MODE_CONV, OUT>(p, dim3(tiles, nt), st) : launch_wg<KIND, 64, MODE_CONV, OUT>(p, dim3(tiles, nt), st);
+static int launch_conv(const WgParams& p, int BN, cudaStream_t st) {
+    return BN == 128 ? launch_conv_bn<KIND, 128, OUT>(p, st) : launch_conv_bn<KIND, 64, OUT>(p, st);
 }
 
 // dual: a second input (x2, its own per-image sizes hw2, Cin2 channels, sampled with stride2) whose channels continue the K axis
@@ -646,6 +750,10 @@ static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cud
         for (int i = 0; i < set.n; ++i) in2_pix[i + 1] = in2_pix[i] + (long long)dual->hw2[2 * i] * dual->hw2[2 * i + 1];
     const unsigned long long in2_plane = dual ? (unsigned long long)in2_pix[set.n] * dual->Cin2 * 2ull : 0ull;
     p.nimg = set.n;
+    const bool tma_out = kind != K_TF32 && !out32;          // fp16 / split outputs: stored (and their residual loaded) by TMA
+    const unsigned long long out_plane = (unsigned long long)set.out_pix[set.n] * cp.Cout * 2ull;
+    const char* yb = reinterpret_cast<const char*>(cp.y);
+    const char* rb = reinterpret_cast<const char*>(cp.residual);
     int tiles = 0;
     for (int i = 0; i < set.n; ++i) {
         const int tw = pick_tw(set.Ho[i], set.Wo[i]), th = 128 / tw;
@@ -663,6 +771,16 @@ static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cud
             rc = get_map4(&p.mapA2[i], static_cast<const char*>(dual->x2) + in2_pix[i] * dual->Cin2 * 2, (unsigned long long)dual->Cin2,
                           (unsigned long long)dual->hw2[2 * i + 1], (unsigned long long)dual->hw2[2 * i], 2, in2_plane, bk, (unsigned)tw,
                           (unsigned)th, 2, (unsigned)dual->stride2, 2);
+        // output and residual maps: the image's own pixels and the layer's Cout channels, so that the bounds clip partial tiles
+        const long long o = set.out_pix[i] * cp.Cout * 2;
+        for (int m = 0; m < (cp.residual ? 2 : 1) && tma_out && !rc; ++m) {
+            CUtensorMap* map = m == 0 ? &p.mapY[i] : &p.mapR[i];
+            const void* base = (m == 0 ? yb : rb) + o;
+            rc = split ? get_map4(map, base, (unsigned long long)cp.Cout, (unsigned long long)set.Wo[i], (unsigned long long)set.Ho[i], 2,
+                                  out_plane, 64, (unsigned)tw, (unsigned)th, 2, 1, 2)
+                       : get_map(map, base, (unsigned long long)cp.Cout, (unsigned long long)set.Wo[i], (unsigned long long)set.Ho[i],
+                                 64, (unsigned)tw, (unsigned)th, 1, 2);
+        }
         if (rc) return rc;
     }
     RF_REQUIRE(tiles > 0, "rf_conv2d_nhwc: empty output");
@@ -677,10 +795,11 @@ static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cud
     if (dual) { p.Cin = cp.Cin + dual->Cin2; p.stride2 = dual->stride2; }      // the kernel's K axis: both inputs
     p.plane = (long long)set.out_pix[set.n] * cp.Cout;
     p.bias = cp.bias; p.residual = cp.residual; p.y = cp.y;
-    const int nt = (cp.Cout + BN - 1) / BN;
-    if (kind == K_TF32) return launch_conv<K_TF32, O_F32>(p, BN, tiles, nt, st);
-    if (kind == K_F16) return out32 ? launch_conv<K_F16, O_F32>(p, BN, tiles, nt, st) : launch_conv<K_F16, O_F16>(p, BN, tiles, nt, st);
-    return out32 ? launch_conv<K_SPLIT, O_F32>(p, BN, tiles, nt, st) : launch_conv<K_SPLIT, O_SPLIT>(p, BN, tiles, nt, st);
+    p.tiles = tiles;
+    p.ntiles = tiles * ((cp.Cout + BN - 1) / BN);
+    if (kind == K_TF32) return launch_conv<K_TF32, O_F32>(p, BN, st);
+    if (kind == K_F16) return out32 ? launch_conv<K_F16, O_F32>(p, BN, st) : launch_conv<K_F16, O_F16>(p, BN, st);
+    return out32 ? launch_conv<K_SPLIT, O_F32>(p, BN, st) : launch_conv<K_SPLIT, O_SPLIT>(p, BN, st);
 }
 
 template <bool SPLIT>
