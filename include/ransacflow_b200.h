@@ -55,10 +55,10 @@ uint64_t rf_launch_count(void);
  * precision: 0 = exact fp32 FMA (SIMT); 1 = 3xTF32 on wgmma tensor cores (hi*hi + lo*hi + hi*lo, C % 32 == 0);
  * 2 = fp16 split on wgmma (x = hi + lo * 2^-11 in fp16, cross terms in a second accumulator, C % 64 == 0): the
  * same 22 significand bits with half the MMAs per channel.
- * Precision 2 has two launch sequences around the same correlation kernel, with identical outputs (environment
- * RF_CORR_V2, read per call): a fused split / key-zeroing launch and a fused mutual-test + compaction launch
- * (3 launches), or separate helpers (6 launches).  rf_corr_mutual_nn_launches() (host only) tells which
- * one a call with this precision would run now: it returns the number of launches. */
+ * Every precision ends in the same mutual test + compaction launch on the row / column arg-max keys.  Before the
+ * correlation, precision 0 zeroes the keys with a memset, precision 1 adds two split launches, precision 2 splits both
+ * operands and zeroes the keys in one launch.  rf_corr_mutual_nn_launches() (host only) returns the number of launches
+ * of a call with this precision: 3, 5 or 3. */
 size_t rf_corr_mutual_nn_workspace(int NA, int NB, int C, int precision);
 int rf_corr_mutual_nn_launches(int precision);
 int rf_corr_mutual_nn(const float* featA, int NA, const float* featB, int NB, int C,
@@ -68,7 +68,7 @@ int rf_corr_mutual_nn(const float* featA, int NA, const float* featB, int NB, in
 /* The same with operands their producer already split (rf_l2norm_split_nhwc writes the normalised rows as fp16 hi / lo * 2^11
  * planes): no split pass.  A_hi / A_lo [NA][C], B_hi / B_lo [NB][C] fp16, C % 64 == 0.  Three graph nodes: memset of the
  * arg-max keys, the fp16-split wgmma kernel (precision 2 of rf_corr_mutual_nn, identical arithmetic), the
- * column-driven mutual test + compaction. */
+ * mutual test + compaction. */
 size_t rf_corr_mutual_nn_presplit_workspace(int NA, int NB);
 int rf_corr_mutual_nn_presplit(const void* A_hi, const void* A_lo, int NA, const void* B_hi, const void* B_lo, int NB, int C,
                                int64_t* idx1_out, int64_t* idx2_out, int* count_out, void* ws, size_t ws_bytes, void* stream);

@@ -52,11 +52,12 @@ class ResNet50Conv4:
         self._program_split = None                # split activations ('f16x3' engine), built on first use
         self.out_channels = self.program.chan[-1]
 
-    def _build(self, kalign, fuse_downsample=False):
-        """``fuse_downsample`` (split engine): a block's conv3 and its down-sampling 1x1 run as one dual-input GEMM."""
+    def _build(self, kalign, fuse_downsample=False, fused_stem=True):
+        """``fuse_downsample`` (split engine): a block's conv3 and its down-sampling 1x1 run as one dual-input GEMM.
+        ``fused_stem`` (fp16 and split engines): the stem builds its patches in shared memory instead of im2col + 1x1 conv."""
         sd, dev = self._sd, self.device
         P = LayerProgram(3, device=dev)
-        if kalign == 64 and os.environ.get("RF_STEM_FUSED", "1") != "0":
+        if kalign == 64 and fused_stem:
             x = P.stem7_fused(0, sd["conv1.weight"], _BN(sd, "bn1"))                 # fp16 engine: patches built in shared memory
         else:
             x = P.stem(0, sd["conv1.weight"], _BN(sd, "bn1"), 2, 3, kalign)          # 7x7/2 stem as im2col + 1x1 conv
@@ -86,7 +87,7 @@ class ResNet50Conv4:
         if eng == ops.ENGINE_SPLIT:
             if self._program_split is None:
                 # the fp16 program's topology with the weights read as hi / lo planes; conv3 + down-sampling branch fused
-                self._program_split = self._build(64, fuse_downsample=os.environ.get("RF_FUSE_DOWNSAMPLE", "1") != "0")
+                self._program_split = self._build(64, fuse_downsample=True)
             out, ohw = self._program_split.run(x, eng)
         elif eng == ops.ENGINE_F16:
             if self._program_f16 is None:
@@ -175,7 +176,7 @@ class _CoarseAlignBase:
         flat = torch.cat([t.reshape(-1, 3) for t in u8], dim=0) if len(u8) > 1 else u8[0].reshape(-1, 3)
         x = Ragged(ops.preproc_u8(flat, normalize=True), hw)
         f = self.net(x)
-        if f.split and outil.corr_precision == 2 and os.environ.get("RF_CORR_PRESPLIT", "1") != "0":
+        if f.split and outil.corr_precision == 2:
             # engine 'f16x3' + fp16-split correlation: the normalisation writes the correlation's operand planes directly;
             # the fp32 views the reference exposes (featsMultiScale, featt) are rebuilt on first access (__getattr__)
             return Ragged(ops.l2norm_planes(f.data), f.hw), u8
@@ -280,9 +281,7 @@ class CoarseAlignA(_CoarseAlignBase):
                  segNet=True, resnet_state_dict=None, verbose=True):
         self._setup(nbScale, nbIter, tolerance, transform, minSize, scaleR, imageNet, segNet, resnet_state_dict, verbose)
 
-    def setPair(self, Is_org, It_org, after_preproc=None):
-        """``after_preproc`` (optional callable): invoked as soon as ``ItTensor`` / ``IsTensor`` exist, before the ResNet
-        trunk is queued - the pair pipeline uses it to start the target's fine features on a second stream."""
+    def setPair(self, Is_org, It_org):
         with torch.no_grad():
             ws, hs = self._size_of(Is_org)
             sizes = [self._target_size(ws, hs, int(self.minSize * s)) for s in self.scaleList]
@@ -296,8 +295,6 @@ class CoarseAlignA(_CoarseAlignBase):
             self.Is, self.It = self._as_pil(IsList[mid]), self._as_pil(ItR)
             self.IsTensor = self._to_tensor01(u8[mid])
             self.ItTensor = self._to_tensor01(u8[nS])
-            if after_preproc is not None:
-                after_preproc()
             feats, _ = self._features(u8)                         # 7 scales + target: one ragged batch
             self._set_source_feats(feats, nS)
             self._set_target_feats(feats, nS)

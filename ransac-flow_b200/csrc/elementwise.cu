@@ -5,7 +5,6 @@
 // (float4) where the channel count allows.
 #include <cuda_fp16.h>
 
-#include <cstdlib>
 #include <type_traits>
 
 #include "common.cuh"
@@ -975,11 +974,16 @@ using namespace rf;
 
 static inline unsigned blocks_for(long long n, int threads) { return (unsigned)((n + threads - 1) / threads); }
 
-// RF_CORR_NEIGH_V2 (read per call): 1 (default) = register-accumulating kernel with one multi-value butterfly per pixel
-// (k = 7); 0 = the one-reduction-per-tap kernel.  Same sums up to the order of the cross-lane additions.
-static int corr_neigh_v2() {
-    const char* e = getenv("RF_CORR_NEIGH_V2");
-    return e ? atoi(e) : 1;
+// CorrNeigh(x, y) into `out` (and CorrNeigh(y, x) into `out2`, nullable): the register-accumulating kernel for k = 7, the
+// one-reduction-per-tap kernel for other odd k
+static int launch_corr_neigh(const float* x, const float* y, int N, int h, int w, int C, int k, int ldo, int round_out, float* out,
+                             float* out2, void* stream) {
+    const long long P = (long long)N * h * w;
+    if (P == 0) return 0;
+    if (k == 7) corr_neigh7_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, y, N, h, w, C, ldo, round_out, out, out2);
+    else corr_neigh_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, y, N, h, w, C, k, ldo, round_out, out, out2);
+    RF_LAUNCHED();
+    return 0;
 }
 
 extern "C" int rf_maxpool2d_nhwc(const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, float* y, void* stream) {
@@ -1263,16 +1267,7 @@ extern "C" int rf_corr_neigh_pair_split(const float* x, const float* y, int N, i
                                         void* stream) {
     RF_REQUIRE((C % 4) == 0 && C <= 1024 && (k % 2) == 1 && ldo >= k * k, "rf_corr_neigh_pair_split: need C % 4 == 0, C <= 1024, odd k, ldo >= k*k");
     RF_REQUIRE(out12_split != nullptr && out12_split != both_split, "rf_corr_neigh_pair_split: outputs");
-    long long P = (long long)N * h * w;
-    if (P == 0) return 0;
-    if (k == 7 && corr_neigh_v2())
-        corr_neigh7_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, y, N, h, w, C, ldo, 3, static_cast<float*>(out12_split),
-                                                                                  static_cast<float*>(both_split));
-    else
-        corr_neigh_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, y, N, h, w, C, k, ldo, 3, static_cast<float*>(out12_split),
-                                                                                 static_cast<float*>(both_split));
-    RF_LAUNCHED();
-    return 0;
+    return launch_corr_neigh(x, y, N, h, w, C, k, ldo, 3, static_cast<float*>(out12_split), static_cast<float*>(both_split), stream);
 }
 
 extern "C" int rf_l2norm_nhwc(const float* x, long long P, int C, const uint8_t* mask, float* y, void* stream) {
@@ -1285,24 +1280,14 @@ extern "C" int rf_l2norm_nhwc(const float* x, long long P, int C, const uint8_t*
 
 extern "C" int rf_corr_neigh_nhwc(const float* x, const float* y, int N, int h, int w, int C, int k, int ldo, int round_tf32_out, float* out, void* stream) {
     RF_REQUIRE((C % 4) == 0 && C <= 1024 && (k % 2) == 1 && ldo >= k * k, "rf_corr_neigh_nhwc: need C % 4 == 0, C <= 1024, odd k, ldo >= k*k");
-    long long P = (long long)N * h * w;
-    if (P == 0) return 0;
-    if (k == 7 && corr_neigh_v2()) corr_neigh7_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, y, N, h, w, C, ldo, round_tf32_out, out, nullptr);
-    else corr_neigh_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, y, N, h, w, C, k, ldo, round_tf32_out, out, nullptr);
-    RF_LAUNCHED();
-    return 0;
+    return launch_corr_neigh(x, y, N, h, w, C, k, ldo, round_tf32_out, out, nullptr, stream);
 }
 
 extern "C" int rf_corr_neigh_pair_nhwc(const float* x, const float* y, int N, int h, int w, int C, int k, int ldo, int round_tf32_out,
                                        float* out_xy, float* out_yx, void* stream) {
     RF_REQUIRE((C % 4) == 0 && C <= 1024 && (k % 2) == 1 && ldo >= k * k, "rf_corr_neigh_pair_nhwc: need C % 4 == 0, C <= 1024, odd k, ldo >= k*k");
     RF_REQUIRE(out_xy != nullptr && out_yx != nullptr && out_xy != out_yx, "rf_corr_neigh_pair_nhwc: two distinct outputs");
-    long long P = (long long)N * h * w;
-    if (P == 0) return 0;
-    if (k == 7 && corr_neigh_v2()) corr_neigh7_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, y, N, h, w, C, ldo, round_tf32_out, out_xy, out_yx);
-    else corr_neigh_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, y, N, h, w, C, k, ldo, round_tf32_out, out_xy, out_yx);
-    RF_LAUNCHED();
-    return 0;
+    return launch_corr_neigh(x, y, N, h, w, C, k, ldo, round_tf32_out, out_xy, out_yx, stream);
 }
 
 extern "C" int rf_softmax_flow(const float* logits, int N, int h, int w, int k, float* flow_nchw, void* stream) {

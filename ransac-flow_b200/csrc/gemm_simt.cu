@@ -11,7 +11,6 @@
 // (transposed on the store so fragment reads are 128-bit and conflict free),
 // global loads of slice k+1 in flight while slice k is multiplied.
 // The wgmma tensor-core engine (gemm_tc.cu) replaces these where TF32 is allowed.
-#include <cstdlib>
 
 #include "common.cuh"
 
@@ -160,61 +159,10 @@ corr_argmax_kernel(const float* __restrict__ A, int NA, const float* __restrict_
     }
 }
 
-// mutual test (utils/outil.py:38-42), fully parallel: rowbest[i] is overwritten with (1 << 63 | j) when (i, j) is a
-// mutual nearest-neighbour pair with non-zero score, else 0
-__global__ void mutual_flag_kernel(unsigned long long* __restrict__ rowbest, const unsigned long long* __restrict__ colbest, int NA) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= NA) return;
-    unsigned long long rk = rowbest[i], out = 0ull;
-    if (rk != 0ull) {
-        uint32_t j = key_index(rk);
-        float v = key_value(rk);
-        unsigned long long ck = __ldg(colbest + j);
-        if (key_index(ck) == (uint32_t)i && (__fmul_rn(v, v) > 0.f)) out = (1ull << 63) | (unsigned long long)j;     // keepMax > 0
-    }
-    rowbest[i] = out;
-}
-
-// single CTA: order-preserving compaction of the flagged rows (utils/outil.py:43-44: nonzero() is row-major)
-__global__ void __launch_bounds__(1024)
-mutual_compact_kernel(const unsigned long long* __restrict__ flagged, int NA, long long* __restrict__ idx1, long long* __restrict__ idx2,
-                      int* __restrict__ count) {
-    __shared__ int s_scan[32];
-    __shared__ int s_off;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) s_off = 0;
-    __syncthreads();
-    for (int base = 0; base < NA; base += 1024) {
-        int i = base + tid;
-        unsigned long long f = (i < NA) ? flagged[i] : 0ull;
-        int keep = (f >> 63) ? 1 : 0;
-        int incl = keep;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            int t = __shfl_up_sync(0xffffffffu, incl, d);
-            if (lane >= d) incl += t;
-        }
-        if (lane == 31) s_scan[warp] = incl;
-        __syncthreads();
-        int wofs = 0, total = 0;
-        for (int w = 0; w < 32; ++w) { int v = s_scan[w]; if (w < warp) wofs += v; total += v; }
-        int off = s_off;
-        if (keep) {
-            int o = off + wofs + incl - 1;
-            idx1[o] = i;
-            idx2[o] = (long long)(f & 0xFFFFFFFFull);
-        }
-        __syncthreads();
-        if (tid == 0) s_off = off + total;
-        __syncthreads();
-    }
-    if (tid == 0) *count = s_off;
-}
-
-// mutual test + order-preserving compaction in ONE single-CTA kernel (the two kernels above fused; used behind the
-// persistent correlation kernel).  Warp w owns a contiguous block of rows; pass 1 counts its mutual pairs with coalesced
-// loads and ballots, the 32 warp totals are scanned, pass 2 recomputes the flags (L1 / L2 hits) and writes the pairs in
-// row order.  rowbest / colbest are left untouched.
+// mutual test (utils/outil.py:38-42) + order-preserving compaction (:43-44, nonzero() is row-major) in ONE single-CTA
+// kernel.  Warp w owns a contiguous block of rows; pass 1 counts its mutual pairs with coalesced loads and ballots, the 32
+// warp totals are scanned, pass 2 recomputes the flags (L1 / L2 hits) and writes the pairs in row order.  rowbest / colbest
+// are left untouched.
 __device__ __forceinline__ bool mutual_pair(const unsigned long long* __restrict__ rowbest, const unsigned long long* __restrict__ colbest,
                                             int i, int NA, uint32_t& j) {
     if (i >= NA) return false;
@@ -307,11 +255,11 @@ mutual_cols_compact_kernel(const unsigned long long* __restrict__ rowbest, const
     if (tid == 0) *count = total;
 }
 
+// the column-driven kernel while its row table fits in shared memory (NA <= 51200), the row-driven one above that
 static int launch_mutual_compact(const unsigned long long* rowbest, const unsigned long long* colbest, int NA, int NB, long long* idx1, long long* idx2,
                                  int* count, cudaStream_t st) {
     const size_t smem = (size_t)NA * sizeof(int);
-    const char* e = getenv("RF_COMPACT_COLS");                    // 1 (default): column-driven compaction; 0: the row-driven kernel
-    if ((e ? atoi(e) : 1) && smem <= 200 * 1024) {
+    if (smem <= 200 * 1024) {
         static bool attr[64] = {false};
         const int dev = current_device();
         if (!attr[dev]) {
@@ -513,9 +461,8 @@ using namespace rf;
 
 // tensor-core engines live in gemm_tc.cu
 int rf_corr_argmax_tc(const float* featA, int NA, const float* featB, int NB, int C,
-                      unsigned long long* rowbest, unsigned long long* colbest, void* ws, cudaStream_t st, int precision, bool v2,
+                      unsigned long long* rowbest, unsigned long long* colbest, void* ws, cudaStream_t st, int precision,
                       const void* const* presplit = nullptr);
-int rf_corr_v2_mode();
 size_t rf_corr_tc_workspace(int NA, int NB, int C);
 int rf_conv2d_tc(const ImgSet& set, const ConvParams& p, const void* w_tc, cudaStream_t st, bool f16, bool out32);
 bool rf_conv2d_tc_supported(const ConvParams& p);
@@ -532,8 +479,9 @@ extern "C" size_t rf_corr_mutual_nn_workspace(int NA, int NB, int C, int precisi
 }
 
 extern "C" int rf_corr_mutual_nn_launches(int precision) {
-    if (precision == 2 && rf_corr_v2_mode() != 0) return 3;          // split+zero, correlation, flag+compact
-    return precision == 0 ? 4 : 6;                                   // memset, [split, split,] correlation, flag, compact
+    // 0: memset, correlation, compaction; 1: memset, split, split, correlation, compaction; 2: split + key zeroing,
+    // correlation, compaction
+    return precision == 1 ? 5 : 3;
 }
 
 extern "C" int rf_corr_mutual_nn(const float* featA, int NA, const float* featB, int NB, int C,
@@ -545,14 +493,13 @@ extern "C" int rf_corr_mutual_nn(const float* featA, int NA, const float* featB,
     cudaStream_t st = as_stream(stream);
     unsigned long long* rowbest = reinterpret_cast<unsigned long long*>(ws);
     unsigned long long* colbest = rowbest + NA;
-    // precision 2 with RF_CORR_V2: one split launch that also zeroes the keys, and the mutual test
-    // and the compaction are one kernel (3 launches instead of 6)
-    const bool v2 = precision == 2 && NA > 0 && NB > 0 && rf_corr_v2_mode() != 0;
-    if (!v2) RF_CUDA(cudaMemsetAsync(ws, 0, ((size_t)NA + NB) * sizeof(unsigned long long), st));
-    if (NA > 0 && NB > 0) {
+    const bool nonempty = NA > 0 && NB > 0;
+    if (!(nonempty && precision == 2))                            // precision 2 zeroes the keys in its split launch
+        RF_CUDA(cudaMemsetAsync(ws, 0, ((size_t)NA + NB) * sizeof(unsigned long long), st));
+    if (nonempty) {
         RF_REQUIRE(precision >= 0 && precision <= 2, "rf_corr_mutual_nn: precision is 0 (fp32 SIMT), 1 (3xTF32) or 2 (fp16 split)");
         if (precision >= 1) {
-            int rc = rf_corr_argmax_tc(featA, NA, featB, NB, C, rowbest, colbest, static_cast<unsigned char*>(ws) + keys_bytes(NA, NB), st, precision, v2);
+            int rc = rf_corr_argmax_tc(featA, NA, featB, NB, C, rowbest, colbest, static_cast<unsigned char*>(ws) + keys_bytes(NA, NB), st, precision);
             if (rc) return rc;
         } else {
             dim3 grid((NB + 127) / 128, (NA + BM - 1) / BM);
@@ -560,18 +507,11 @@ extern "C" int rf_corr_mutual_nn(const float* featA, int NA, const float* featB,
             RF_LAUNCHED();
         }
     }
-    if (v2) return launch_mutual_compact(rowbest, colbest, NA, NB, (long long*)idx1_out, (long long*)idx2_out, count_out, st);
-    if (NA > 0) {
-        mutual_flag_kernel<<<(NA + 255) / 256, 256, 0, st>>>(rowbest, colbest, NA);
-        RF_LAUNCHED();
-    }
-    mutual_compact_kernel<<<1, 1024, 0, st>>>(rowbest, NA, (long long*)idx1_out, (long long*)idx2_out, count_out);
-    RF_LAUNCHED();
-    return 0;
+    return launch_mutual_compact(rowbest, colbest, NA, NB, (long long*)idx1_out, (long long*)idx2_out, count_out, st);
 }
 
 // utils/outil.py:32-45 with operands the producer already split (rf_l2norm_split_nhwc: hi = fp16(x), lo = fp16((x - hi) * 2^11)):
-// memset of the keys, the fp16-split correlation kernel, the column-driven compaction.  ws: (NA + NB) keys.
+// memset of the keys, the fp16-split correlation kernel, the mutual test + compaction.  ws: (NA + NB) keys.
 extern "C" size_t rf_corr_mutual_nn_presplit_workspace(int NA, int NB) { return keys_bytes(NA, NB) + 256; }
 
 extern "C" int rf_corr_mutual_nn_presplit(const void* A_hi, const void* A_lo, int NA, const void* B_hi, const void* B_lo, int NB, int C,
@@ -587,7 +527,7 @@ extern "C" int rf_corr_mutual_nn_presplit(const void* A_hi, const void* A_lo, in
         return 0;
     }
     const void* planes[4] = {A_hi, A_lo, B_hi, B_lo};
-    int rc = rf_corr_argmax_tc(nullptr, NA, nullptr, NB, C, rowbest, colbest, nullptr, st, 2, true, planes);
+    int rc = rf_corr_argmax_tc(nullptr, NA, nullptr, NB, C, rowbest, colbest, nullptr, st, 2, planes);
     if (rc) return rc;
     return launch_mutual_compact(rowbest, colbest, NA, NB, (long long*)idx1_out, (long long*)idx2_out, count_out, st);
 }

@@ -22,7 +22,6 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 
-#include <cstdlib>
 #include <mutex>
 #include <unordered_map>
 
@@ -584,24 +583,9 @@ __global__ void split_tf32_kernel(const float4* __restrict__ x, float4* __restri
     lo[i] = l;
 }
 
-// fp16 split for the correlation (precision 2): hi = fp16(x), lo = fp16((x - hi) * 2^11)
-__global__ void split_f16_kernel(const float4* __restrict__ x, uint2* __restrict__ hi, uint2* __restrict__ lo, long long n4) {
-    long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n4) return;
-    const float4 v = __ldg(x + i);
-    const __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
-    const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-    const __half2 l0 = __floats2half2_rn((v.x - f0.x) * 2048.f, (v.y - f0.y) * 2048.f);
-    const __half2 l1 = __floats2half2_rn((v.z - f1.x) * 2048.f, (v.w - f1.y) * 2048.f);
-    uint2 ho, lo2;
-    ho.x = *reinterpret_cast<const uint32_t*>(&h0); ho.y = *reinterpret_cast<const uint32_t*>(&h1);
-    lo2.x = *reinterpret_cast<const uint32_t*>(&l0); lo2.y = *reinterpret_cast<const uint32_t*>(&l1);
-    hi[i] = ho;
-    lo[i] = lo2;
-}
-
-// Both feature matrices in ONE launch (fp16 split as above; hi/lo of A then hi/lo of B are consecutive in the workspace),
-// and the arg-max keys zeroed by the first threads: replaces a memset node and two split launches.
+// fp16 split for the correlation (precision 2): hi = fp16(x), lo = fp16((x - hi) * 2^11), both feature matrices in ONE
+// launch (hi/lo of A then hi/lo of B are consecutive in the workspace), and the arg-max keys zeroed by the first threads:
+// replaces a memset node and two split launches.
 __global__ void split_f16_all_kernel(const float4* __restrict__ A, const float4* __restrict__ B, uint2* __restrict__ Ahi, uint2* __restrict__ Alo,
                                      uint2* __restrict__ Bhi, uint2* __restrict__ Blo, long long na4, long long nb4,
                                      unsigned long long* __restrict__ keys, long long nkeys) {
@@ -909,23 +893,15 @@ int rf_stem7_split_impl(const float* x, int nimg, const int* hw_host, const void
 
 size_t rf_corr_tc_workspace(int NA, int NB, int C) { return 2ull * ((size_t)NA + NB) * C * sizeof(float) + 1024; }
 
-// RF_CORR_V2 (read per call): 1 (default) = precision 2 splits both operands and zeroes the keys in one launch and runs the
-// mutual test + compaction as one kernel behind the correlation (3 launches); 0 = memset / split / split / correlation / flag /
-// compact (6).  Identical outputs.
-int rf_corr_v2_mode() {
-    const char* e = getenv("RF_CORR_V2");
-    return e ? atoi(e) : 1;
-}
-
-// v2 (precision 2 only): the caller has NOT zeroed rowbest / colbest (contiguous, NA + NB keys): the split launch does it.
-// presplit (precision 2, v2 only; nullable): {A hi, A lo, B hi, B lo} fp16 planes written by the producer of the features
+// Precision 2 splits both operands in one launch that also zeroes rowbest / colbest (contiguous, NA + NB keys); precision 1
+// splits them in two launches behind the caller's key memset.
+// presplit (precision 2; nullable): {A hi, A lo, B hi, B lo} fp16 planes written by the producer of the features
 // (rf_l2norm_split_nhwc): no split launch; the caller has zeroed the keys.
 int rf_corr_argmax_tc(const float* featA, int NA, const float* featB, int NB, int C,
-                      unsigned long long* rowbest, unsigned long long* colbest, void* ws, cudaStream_t st, int precision, bool v2,
+                      unsigned long long* rowbest, unsigned long long* colbest, void* ws, cudaStream_t st, int precision,
                       const void* const* presplit) {
     const bool f16 = precision == 2;
-    RF_REQUIRE(presplit == nullptr || (v2 && f16), "rf_corr_mutual_nn: pre-split operands go with the fp16-split kernel sequence");
-    RF_REQUIRE(!v2 || f16, "rf_corr_mutual_nn: the fused kernel sequence is the fp16-split one (precision 2)");
+    RF_REQUIRE(presplit == nullptr || f16, "rf_corr_mutual_nn: pre-split operands go with the fp16-split kernel (precision 2)");
     RF_REQUIRE((C % (f16 ? TC_BK_F16 : TC_BK)) == 0, "rf_corr_mutual_nn: precision 1 needs C % 32 == 0, precision 2 C % 64 == 0");
     uintptr_t base = (reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255;
     const size_t esz = f16 ? 2 : 4;
@@ -940,16 +916,11 @@ int rf_corr_argmax_tc(const float* featA, int NA, const float* featB, int NB, in
         Bhi = const_cast<char*>(static_cast<const char*>(presplit[2]));
         Blo = const_cast<char*>(static_cast<const char*>(presplit[3]));
         for (int i = 0; i < 4; ++i) RF_REQUIRE(presplit[i] != nullptr && ((uintptr_t)presplit[i] % 16) == 0, "rf_corr_mutual_nn_presplit: planes must be 16-byte aligned");
-    } else if (v2) {
+    } else if (f16) {
         RF_REQUIRE(colbest == rowbest + NA, "rf_corr_mutual_nn: arg-max keys must be contiguous");
         const long long nkeys = (long long)NA + NB, n = na4 + nb4 > nkeys ? na4 + nb4 : nkeys;
         split_f16_all_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const float4*)featA, (const float4*)featB, (uint2*)Ahi, (uint2*)Alo,
                                                                             (uint2*)Bhi, (uint2*)Blo, na4, nb4, rowbest, nkeys);
-        RF_LAUNCHED();
-    } else if (f16) {
-        split_f16_kernel<<<(unsigned)((na4 + 255) / 256), 256, 0, st>>>((const float4*)featA, (uint2*)Ahi, (uint2*)Alo, na4);
-        RF_LAUNCHED();
-        split_f16_kernel<<<(unsigned)((nb4 + 255) / 256), 256, 0, st>>>((const float4*)featB, (uint2*)Bhi, (uint2*)Blo, nb4);
         RF_LAUNCHED();
     } else {
         split_tf32_kernel<<<(unsigned)((na4 + 255) / 256), 256, 0, st>>>((const float4*)featA, (float4*)Ahi, (float4*)Alo, na4);

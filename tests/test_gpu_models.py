@@ -133,29 +133,27 @@ def test_resnet50_conv4_f16_engine(rf):
     assert np.array_equal(y1, y2)                 # tiles never mix images: bit-identical alone vs in a ragged batch
 
 
-def test_fused_stem_equals_im2col_stem(rf, monkeypatch):
-    """RF_OP_STEM7 (patches built in shared memory) against im2col + 1x1 conv on the same fp16 weights, over a ragged
-    batch with sizes that are not multiples of the 16 x 8 tile."""
+def test_trunk_fused_stem_equals_explicit_im2col_stem(rf):
+    """RF_OP_STEM7 (patches built in shared memory, what the fp16 trunk runs) against im2col + 1x1 conv on the same fp16
+    weights, over a ragged batch with sizes that are not multiples of the 16 x 8 tile."""
     from ransac_flow_b200.coarseAlignFeatMatch import ResNet50Conv4
     sd = synth.resnet50_conv4_state(3)
     g = torch.Generator().manual_seed(5)
     imgs = [torch.randn(h * w, 3, generator=g) for h, w in [(64, 96), (48, 80), (34, 50)]]
     x = rf.ops.Ragged(torch.cat(imgs).cuda(), [(64, 96), (48, 80), (34, 50)])
-    outs = {}
     rf.model.set_engine("f16")
     try:
-        for fused in ("0", "1"):
-            monkeypatch.setenv("RF_STEM_FUSED", fused)
-            net = ResNet50Conv4(sd)
-            y = net(x)
-            ops_used = [o[0] for o in net._program_f16.ops[:2]]
-            assert (5 in ops_used) == (fused == "1")
-            outs[fused] = y.data.float().cpu().numpy().copy()
+        net = ResNet50Conv4(sd)
+        fused = net(x).data.float().cpu().numpy().copy()
+        assert 5 in [o[0] for o in net._program_f16.ops[:2]]
+        plain = net._build(64, fused_stem=False)
+        assert 5 not in [o[0] for o in plain.ops[:2]]
+        im2col = plain.run(x, rf.ops.ENGINE_F16)[0].float().cpu().numpy().copy()
     finally:
         rf.model.set_engine("fp32")
-    d = np.abs(outs["0"] - outs["1"]).max()
-    print("fused vs im2col stem: max |diff| of the conv4 features = %.3g (max %.3g)" % (d, np.abs(outs["0"]).max()))
-    assert d <= 2e-3 * max(1.0, np.abs(outs["0"]).max())
+    d = np.abs(im2col - fused).max()
+    print("fused vs im2col stem: max |diff| of the conv4 features = %.3g (max %.3g)" % (d, np.abs(im2col).max()))
+    assert d <= 2e-3 * max(1.0, np.abs(im2col).max())
 
 
 @pytest.mark.parametrize("k,cin,cout,stride,pad", [(5, 2, 16, 1, 2), (3, 4, 32, 2, 1), (7, 3, 64, 2, 3), (3, 3, 64, 1, 1)])

@@ -6,6 +6,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import wgmma_ref as R
 from oracle import model_oracle as MO
 from oracle import warp_oracle as WO
 
@@ -99,34 +100,48 @@ def test_corr_neigh_pair_is_bit_identical_to_two_calls(rf, n, c, h, w, k, ldo, m
     assert torch.equal(both.data[:n * h * w], xy.data) and torch.equal(both.data[n * h * w:], yx.data)
 
 
+def corr_neigh_ref(x, y, k):
+    """fp64 CorrNeigh(x, y) of (N, C, h, w) CPU tensors as [N*h*w, k*k] rows (tap i*k + j reads y at (r + i - k//2,
+    c + j - k//2), zero outside), and the same on |x|, |y|."""
+    x, y, p = x.double(), y.double(), k // 2
+    h, w = x.shape[2], x.shape[3]
+    yp, ap = F.pad(y, (p, p, p, p)), F.pad(y.abs(), (p, p, p, p))
+    taps = [(i, j) for i in range(k) for j in range(k)]
+    ref = torch.stack([(x * yp[:, :, i:i + h, j:j + w]).sum(1) for i, j in taps], -1)
+    absref = torch.stack([(x.abs() * ap[:, :, i:i + h, j:j + w]).sum(1) for i, j in taps], -1)
+    return ref.reshape(-1, k * k), absref.reshape(-1, k * k)
+
+
 @pytest.mark.parametrize("n,c,h,w,ldo", [(1, 256, 60, 80, 64), (2, 256, 6, 8, 49), (1, 64, 5, 3, 64), (1, 1024, 4, 7, 64), (1, 256, 1, 1, 96)])
-def test_corr_neigh_register_kernel_equals_per_tap_kernel(rf, monkeypatch, n, c, h, w, ldo):
-    """corr_neigh7_kernel (49 sums in registers, one multi-value butterfly, coalesced row store; RF_CORR_NEIGH_V2=1, default)
-    == corr_neigh_kernel (one warp reduction per tap) bit for bit in every output mode, single and pair, and the split form
-    (engine 4) rebuilds the fp32 values to 2^-22."""
-    g = torch.Generator().manual_seed(n * 10 + h)
-    a = rf.ops.Ragged.from_nchw(F.normalize(torch.randn(n, c, h, w, generator=g)).cuda())
-    b = rf.ops.Ragged.from_nchw(F.normalize(torch.randn(n, c, h, w, generator=g)).cuda())
-    res = {}
-    for v2 in ("0", "1"):
-        monkeypatch.setenv("RF_CORR_NEIGH_V2", v2)
-        r = []
-        for mode in (0, 1, 2):
-            r.append(rf.ops.corr_neigh(a, b, 7, ldo, mode).data)
-            r += [t.data for t in rf.ops.corr_neigh_pair(a, b, 7, ldo, mode)]
-        c12, both = rf.ops.corr_neigh_pair_split(a, b, 7, ldo)
-        r += [c12.data, both.data]
+@pytest.mark.parametrize("k", [3, 5, 7])
+def test_corr_neigh_kernels_match_fp64_reference(rf, k, n, c, h, w, ldo):
+    """corr_neigh7_kernel (k = 7: 49 sums in registers, one multi-value butterfly, coalesced row store) and corr_neigh_kernel
+    (other odd k: one warp reduction per tap) against fp64, element by element, in every output mode (fp32, TF32-rounded, fp16),
+    single and pair: |y - ref| <= r_out |ref| + gamma_C (1 + r_out) sum |x y| + atol, with gamma_C = C u / (1 - C u) the fp32
+    accumulation bound of a C-term sum (u = 2^-24).  Padding channels are zero, the pair's halves equal the two single calls bit
+    for bit, and the split form (engine 4) rebuilds both halves to 2^-21."""
+    g = torch.Generator().manual_seed(n * 10 + h + k)
+    xa = F.normalize(torch.randn(n, c, h, w, generator=g))
+    xb = F.normalize(torch.randn(n, c, h, w, generator=g))
+    a, b = rf.ops.Ragged.from_nchw(xa.cuda()), rf.ops.Ragged.from_nchw(xb.cuda())
+    refs = {"xy": corr_neigh_ref(xa, xb, k), "yx": corr_neigh_ref(xb, xa, k)}
+    gamma = c * 2.0 ** -24 / (1 - c * 2.0 ** -24)
+    for mode, r_out, atol in ((0, 0.0, 0.0), (1, R.R_TF32, 0.0), (2, R.R_F16, R.ATOL["f16"])):
+        xy, yx = rf.ops.corr_neigh(a, b, k, ldo, mode).data, rf.ops.corr_neigh(b, a, k, ldo, mode).data
+        pxy, pyx, _ = rf.ops.corr_neigh_pair(a, b, k, ldo, mode)
         torch.cuda.synchronize()
-        res[v2] = r
-    for x0, x1 in zip(res["0"], res["1"]):
-        assert x0.shape == x1.shape and torch.equal(x0, x1)
+        assert torch.equal(pxy.data, xy) and torch.equal(pyx.data, yx), mode
+        for name, got in (("xy", xy), ("yx", yx)):
+            ref, absref = refs[name]
+            R.check(got[:, :k * k].cpu(), ref, absref, r_out, gamma * (1 + r_out), atol, "k %d mode %d %s" % (k, mode, name))
+            assert not bool(got[:, k * k:].any()), "padding channels"
     P = n * h * w
-    full = res["1"][0]                                          # fp32 CorrNeigh(a, b)
-    c12, both = res["1"][-2], res["1"][-1]
+    full, swapped = rf.ops.corr_neigh(a, b, k, ldo, 0).data, rf.ops.corr_neigh(b, a, k, ldo, 0).data
+    c12, both = rf.ops.corr_neigh_pair_split(a, b, k, ldo)
+    c12, both = c12.data, both.data
     assert c12.shape == (2, P, ldo) and both.shape == (2, 2 * P, ldo)
     assert (rf.ops.from_split(c12) - full).abs().max().item() < 2.0 ** -21
     assert torch.equal(both[:, :P], c12)
-    swapped = rf.ops.corr_neigh(b, a, 7, ldo, 0).data
     assert (rf.ops.from_split(both[:, P:].contiguous()) - swapped).abs().max().item() < 2.0 ** -21
 
 

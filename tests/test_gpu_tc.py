@@ -124,12 +124,13 @@ def test_corr_kitti_shape_both_engines_agree(rf):
 
 
 @pytest.mark.parametrize("C,NA,NB,seed", [(1024, 13065, 1200, 0), (1024, 2107, 300, 1), (64, 129, 127, 2), (256, 1, 1, 4),
-                                           (1024, 300, 1200, 5), (128, 5000, 130, 6), (64, 128, 128, 7), (192, 40000, 257, 8)])
-def test_corr_persistent_kernel_identical_to_one_tile_kernel(rf, monkeypatch, C, NA, NB, seed):
-    """Precision 2 has two launch sequences (RF_CORR_V2, read per call): fused split / key zeroing and fused mutual test +
-    compaction (3 launches) must return exactly the pairs of memset / split / split / correlation / flag / compact (6) -
-    same MMAs, same (score, smallest index) order - and both agree with the fp32 oracle up to arg-max ties below fp32
-    accumulation noise."""
+                                           (1024, 300, 1200, 5), (128, 5000, 130, 6), (64, 128, 128, 7), (192, 40000, 257, 8),
+                                           (64, 60000, 300, 9)])
+@pytest.mark.parametrize("precision", [0, 1, 2])
+def test_corr_mutual_nn_repeatable_and_matches_oracle(rf, precision, C, NA, NB, seed):
+    """Every precision ends in the same mutual test + compaction on the row / column arg-max keys (the column-driven kernel up
+    to NA = 51200, the row-driven one above): pairs in row order, the same pairs from a second call on a recycled workspace
+    (the call zeroes the keys itself), and agreement with the fp32 oracle up to arg-max ties below fp32 accumulation noise."""
     rs = np.random.RandomState(seed)
     A = np.abs(rs.randn(C, NA)).astype(np.float32)
     B = np.abs(rs.randn(C, NB)).astype(np.float32)
@@ -140,27 +141,23 @@ def test_corr_persistent_kernel_identical_to_one_tile_kernel(rf, monkeypatch, C,
     if NB > 2:
         B[:, 1] = 0                              # masked target cell: never matches
     fa, fb = torch.from_numpy(A.T.copy()).cuda(), torch.from_numpy(B.T.copy()).cuda()
-    got = {}
-    for v2 in ("0", "1"):
-        monkeypatch.setenv("RF_CORR_V2", v2)
-        assert rf._lib.lib.rf_corr_mutual_nn_launches(2) == (3 if v2 == "1" else 6)
-        for rep in range(2):                     # twice: the workspace keys must be re-zeroed by the call itself
-            i1, i2, cnt = rf.ops.corr_mutual_nn(fa, fb, 2)
+    got = []
+    for rep in range(2):                         # twice: the workspace keys must be re-zeroed by the call itself
+        i1, i2, cnt = rf.ops.corr_mutual_nn(fa, fb, precision)
         k = int(cnt.item())
-        got[v2] = (i1[:k].cpu().numpy(), i2[:k].cpu().numpy())
-    assert np.array_equal(got["0"][0], got["1"][0]) and np.array_equal(got["0"][1], got["1"][1])
-    assert np.all(np.diff(got["1"][0]) > 0)
-    if NA * NB <= 13065 * 1200:
-        o1, o2, score = OO.mutualMatching(A, B, return_score=True)
-        check_same(got["1"][0], got["1"][1], o1, o2, score)
+        got.append((i1[:k].cpu().numpy(), i2[:k].cpu().numpy()))
+    assert np.array_equal(got[0][0], got[1][0]) and np.array_equal(got[0][1], got[1][1])
+    assert np.all(np.diff(got[1][0]) > 0)
+    o1, o2, score = OO.mutualMatching(A, B, return_score=True)
+    check_same(got[1][0], got[1][1], o1, o2, score)
 
 
 @pytest.mark.parametrize("C,NA,NB,seed", [(1024, 13065, 1200, 0), (1024, 2107, 300, 1), (64, 129, 127, 2), (256, 1, 1, 4), (1024, 300, 1200, 5),
-                                           (1024, 25747, 8250, 7)])
-def test_corr_presplit_operands_and_column_compaction_identical(rf, monkeypatch, C, NA, NB, seed):
+                                           (1024, 25747, 8250, 7), (64, 60000, 300, 8)])
+def test_corr_presplit_operands_and_column_compaction_identical(rf, C, NA, NB, seed):
     """rf_corr_mutual_nn_presplit (operand planes written by rf_l2norm_split_nhwc, key memset, correlation kernel, mutual
-    test + compaction) == rf_corr_mutual_nn at precision 2 (split launch + separate compaction): identical index lists, with
-    the column-driven and the row-driven compaction kernels (RF_COMPACT_COLS)."""
+    test + compaction) == rf_corr_mutual_nn at precision 2 (split launch that zeroes the keys, correlation kernel, mutual test
+    + compaction): identical index lists, through the column-driven compaction kernel and, at NA > 51200, the row-driven one."""
     g = torch.Generator().manual_seed(seed)
     raw = torch.cat([torch.randn(NA + NB, C, generator=g).abs()]).cuda()
     raw[NA:NA + min(NA, NB) // 2] = raw[torch.randperm(NA, generator=g)[:min(NA, NB) // 2].cuda()] + 0.05 * raw[NA:NA + min(NA, NB) // 2]
@@ -170,13 +167,10 @@ def test_corr_presplit_operands_and_column_compaction_identical(rf, monkeypatch,
     rows = rf.ops.from_split(planes)                              # the fp32 values those planes stand for
     ref = rf.ops.corr_mutual_nn(rows[:NA].contiguous(), rows[NA:].contiguous(), 2)
     nref = int(ref[2].item())
-    for tail, cols in (("1", "1"), ("0", "1"), ("0", "0")):        # fused tail in the correlation kernel / column-driven / row-driven kernel
-        monkeypatch.setenv("RF_CORR_TAIL", tail)
-        monkeypatch.setenv("RF_COMPACT_COLS", cols)
-        for _ in range(2):                                        # twice: the ticket counter is re-zeroed per call
-            got = rf.ops.corr_mutual_nn_presplit(planes[0, :NA], planes[1, :NA], planes[0, NA:], planes[1, NA:])
-            n = int(got[2].item())
-            assert n == nref and torch.equal(got[0][:n], ref[0][:n]) and torch.equal(got[1][:n], ref[1][:n]), (tail, cols)
-        again = rf.ops.corr_mutual_nn(rows[:NA].contiguous(), rows[NA:].contiguous(), 2)
-        assert int(again[2].item()) == nref and torch.equal(again[0][:n], ref[0][:n])
+    for _ in range(2):                                            # twice: the keys are re-zeroed per call
+        got = rf.ops.corr_mutual_nn_presplit(planes[0, :NA], planes[1, :NA], planes[0, NA:], planes[1, NA:])
+        n = int(got[2].item())
+        assert n == nref and torch.equal(got[0][:n], ref[0][:n]) and torch.equal(got[1][:n], ref[1][:n])
+    again = rf.ops.corr_mutual_nn(rows[:NA].contiguous(), rows[NA:].contiguous(), 2)
+    assert int(again[2].item()) == nref and torch.equal(again[0][:n], ref[0][:n])
     assert nref >= 1 and (NB <= 2 or not bool((ref[1][:nref] == 1).any()))

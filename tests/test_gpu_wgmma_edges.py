@@ -158,10 +158,10 @@ def test_dual_sixteen_image_batch_equals_images_alone(rf):
         dual_check(rf, x1s + x1s[:1], x2s + x2s[:1], w1, w2, bias, 2, True)
 
 
-# ------------------------------------------------------------------ correlation: arg-max keys of precisions 1 and 2
-def corr_call(rf, A, B, mode, monkeypatch):
-    """Runs the mutual nearest-neighbour entry point with a caller-owned workspace; returns (row keys or None, column keys,
-    idx1, idx2) as numpy.  Row keys are None where the launch sequence overwrites them with mutual flags."""
+# ------------------------------------------------------------------ correlation: arg-max keys of every precision
+def corr_call(rf, A, B, mode):
+    """Runs the mutual nearest-neighbour entry point (``mode`` = its precision, or "presplit") with a caller-owned workspace;
+    returns (row keys, column keys, idx1, idx2) as numpy."""
     lib, ptr = rf._lib.lib, rf._lib.ptr
     NA, Cc = A.shape
     NB = B.shape[0]
@@ -175,20 +175,16 @@ def corr_call(rf, A, B, mode, monkeypatch):
         ws = torch.empty(wsz, device="cuda", dtype=torch.uint8)
         rf._lib.check(lib.rf_corr_mutual_nn_presplit(ptr(a[0]), ptr(a[1]), NA, ptr(b[0]), ptr(b[1]), NB, Cc, ptr(idx1), ptr(idx2), ptr(count),
                                                      ptr(ws), wsz, rf._lib.stream()))
-        rows_valid = True
     else:
-        precision = 1 if mode == 1 else 2
-        monkeypatch.setenv("RF_CORR_V2", "0" if mode == "2v1" else "1")
-        wsz = lib.rf_corr_mutual_nn_workspace(NA, NB, Cc, precision)
+        wsz = lib.rf_corr_mutual_nn_workspace(NA, NB, Cc, mode)
         ws = torch.full((wsz,), 0xAB, device="cuda", dtype=torch.uint8)      # the call must zero the keys itself
         a, b = A.cuda(), B.cuda()
         rf._lib.check(lib.rf_corr_mutual_nn(ptr(a), NA, ptr(b), NB, Cc, ptr(idx1), ptr(idx2), ptr(count), ptr(ws), wsz,
-                                            precision, rf._lib.stream()))
-        rows_valid = mode == 2
+                                            mode, rf._lib.stream()))
     torch.cuda.synchronize()
     keys = ws[:8 * (NA + NB)].view(torch.int64).cpu().numpy().view(np.uint64)
     n = int(count.item())
-    return (keys[:NA] if rows_valid else None), keys[NA:], keys[:NA], idx1[:n].cpu().numpy(), idx2[:n].cpu().numpy()
+    return keys[:NA], keys[NA:], idx1[:n].cpu().numpy(), idx2[:n].cpu().numpy()
 
 
 def check_keys(keys, S, absS, c, what):
@@ -220,6 +216,9 @@ def corr_data(case):
         A, B = rs.randn(NA, Cc), rs.randn(NB, Cc)
         A[:, 0] = -(np.abs(A[:, 0]) + 6)              # every score < 0: negative maxima on both sides
         B[:, 0] = np.abs(B[:, 0]) + 6
+    elif case in ("row1", "col1"):                      # one feature vector on one side: a single-row / single-column tile
+        NA, NB, Cc = (1, 333, 192) if case == "row1" else (333, 1, 192)
+        A, B = np.abs(rs.randn(NA, Cc)), np.abs(rs.randn(NB, Cc))
     else:
         NA, NB, Cc = 333, 270, int(case[1:])
         A, B = np.abs(rs.randn(NA, Cc)), np.abs(rs.randn(NB, Cc))
@@ -235,42 +234,36 @@ def corr_data(case):
     return torch.from_numpy(A), torch.from_numpy(B)
 
 
-@pytest.mark.parametrize("case", ["ties", "negative", "c192", "c448"])
-@pytest.mark.parametrize("mode", [1, 2, "2v1", "presplit"])
-def test_corr_argmax_keys_vs_fp64(rf, monkeypatch, mode, case):
+@pytest.mark.parametrize("case", ["ties", "negative", "c192", "c448", "row1", "col1"])
+@pytest.mark.parametrize("mode", [0, 1, 2, "presplit"])
+def test_corr_argmax_keys_vs_fp64(rf, mode, case):
     """The correlation's per-row / per-column arg-max keys (f2ord(score) << 32 | ~index) read from the workspace: scores within
-    the 3xTF32 (precision 1) or split (precision 2, pre-split planes) allowance of fp64 scores of the consumed operands, indices
-    the fp64 arg-max wherever the gap allows, exact ties to the smallest index across row and column tiles, the two keys of a
-    mutual pair with bit-identical scores, and the compacted pair list == the mutual pairs of the keys.  Sizes leave partial
-    row and column tiles; C = 64 / 192 / 448 give 1 to 14 K blocks."""
+    the fp32 (precision 0: gamma_C = C u / (1 - C u), the bound of a C-term fp32 FMA chain), 3xTF32 (precision 1) or split
+    (precision 2, pre-split planes) allowance of fp64 scores of the consumed operands, indices the fp64 arg-max wherever the
+    gap allows, exact ties to the smallest index across row and column tiles, the two keys of a mutual pair with bit-identical
+    scores, and the compacted pair list == the mutual pairs of the keys.  Sizes leave partial row and column tiles, down to a
+    single row (row1) or a single column (col1); C = 64 / 192 / 448 give 1 to 14 K blocks."""
     A, B = corr_data(case)
-    kind = "tf32x3" if mode == 1 else "split"
-    Aq = A.double() if mode == 1 else R.from_split(R.to_split(A))
-    Bq = B.double() if mode == 1 else R.from_split(R.to_split(B))
+    split = mode in (2, "presplit")
+    Aq = R.from_split(R.to_split(A)) if split else A.double()
+    Bq = R.from_split(R.to_split(B)) if split else B.double()
     S = (Aq.cuda() @ Bq.cuda().T).cpu().numpy()
     absS = (Aq.abs().cuda() @ Bq.abs().cuda().T).cpu().numpy()
-    c = R.ACC[kind]
-    rowk, colk, raw_rows, i1, i2 = corr_call(rf, A, B, mode, monkeypatch)
+    cu = A.shape[1] * 2.0 ** -24
+    c = R.ACC["split"] if split else R.ACC["tf32x3"] if mode == 1 else cu / (1 - cu)
+    rowk, colk, i1, i2 = corr_call(rf, A, B, mode)
     csc, cidx, cw = check_keys(colk, S.T, absS.T, c, "columns")
-    worst = cw
-    if rowk is not None:
-        rsc, ridx, rw = check_keys(rowk, S, absS, c, "rows")
-        worst = max(worst, rw)
-        mutual = cidx[ridx] == np.arange(len(ridx))
-        assert np.array_equal(rsc[mutual].view(np.uint32), csc[ridx[mutual]].view(np.uint32)), "mutual pair scores differ"
-        keep = mutual & (rsc.astype(np.float64) ** 2 > 0)
-        assert np.array_equal(i1, np.nonzero(keep)[0]) and np.array_equal(i2, ridx[keep])
-    else:                                               # rows overwritten by (1 << 63 | j) flags of the mutual pairs
-        flagged = (raw_rows >> np.uint64(63)) == 1
-        j = (raw_rows & np.uint64(0xFFFFFFFF)).astype(np.int64)
-        assert (cidx[j[flagged]] == np.nonzero(flagged)[0]).all()
-        assert np.array_equal(i1, np.nonzero(flagged)[0]) and np.array_equal(i2, j[flagged])
+    rsc, ridx, rw = check_keys(rowk, S, absS, c, "rows")
+    worst = max(cw, rw)
+    mutual = cidx[ridx] == np.arange(len(ridx))
+    assert np.array_equal(rsc[mutual].view(np.uint32), csc[ridx[mutual]].view(np.uint32)), "mutual pair scores differ"
+    keep = mutual & (rsc.astype(np.float64) ** 2 > 0)
+    assert np.array_equal(i1, np.nonzero(keep)[0]) and np.array_equal(i2, ridx[keep])
     if case == "ties":
         assert cidx[200] == 7, cidx[200]
-        if rowk is not None:
-            assert ridx[50] == 5, ridx[50]
-            assert ridx[7] == ridx[135] == ridx[300] and rsc[7] == rsc[135] == rsc[300]
+        assert ridx[50] == 5, ridx[50]
+        assert ridx[7] == ridx[135] == ridx[300] and rsc[7] == rsc[135] == rsc[300]
         assert csc[5] == csc[130] == csc[260] and cidx[5] == cidx[130] == cidx[260]
     if case == "negative":
-        assert (csc < 0).all() and (rowk is None or (rsc < 0).all())
+        assert (csc < 0).all() and (rsc < 0).all()
     print("correlation %s %s: worst score error / allowance %.3g, %d pairs" % (mode, case, worst, len(i1)))
