@@ -49,39 +49,14 @@ def test_conv2d_fp32(rf, cin, cout, k, stride, pad, sizes, relu, res):
         close(y.image(i).cpu(), r, 2e-5)
 
 
-def test_pool_blur_norm(rf):
-    g = torch.Generator().manual_seed(0)
-    xs = [torch.randn(1, 64, 17, 23, generator=g), torch.randn(1, 64, 8, 6, generator=g)]
-    x = ragged(rf, xs)
-    for i, t in enumerate(xs):
-        close(rf.ops.maxpool2d(x, 2, 1, 0).image(i).cpu(), F.max_pool2d(t, 2, 1), 0)
-        close(rf.ops.maxpool2d(x, 3, 2, 1).image(i).cpu(), F.max_pool2d(t, 3, 2, 1), 0)
-        close(rf.ops.blur_downsample(x, 2).image(i).cpu(), MO.blur_downsample(t, 2), 1e-6)
-        close(rf.ops.blur_downsample(x, 1).image(i).cpu(), MO.blur_downsample(t, 1), 1e-6)
-    t = torch.randn(1, 256, 6, 8, generator=g)
-    n = rf.ops.l2norm(ragged(rf, [t]).data)
-    close(n.view(1, 6, 8, 256).permute(0, 3, 1, 2).cpu(), F.normalize(t), 1e-6)
-    z = torch.zeros(3, 8).cuda()
-    assert torch.equal(rf.ops.l2norm(z), z)                               # eps clamp: 0 / 1e-12 = 0
-    mask = torch.tensor([1, 0, 1], dtype=torch.uint8).cuda()
-    m = rf.ops.l2norm(torch.ones(3, 8).cuda(), mask)
-    assert float(m[1].abs().sum()) == 0 and abs(float(m[0].norm()) - 1) < 1e-6
-
-
-def test_corr_neigh_and_heads_epilogues(rf):
+def test_corr_neigh_module_matches_oracle(rf):
+    """model.CorrNeigh(7) (NCHW in and out) against the oracle's CorrNeigh; the kernels themselves are held to fp64 below,
+    the pooling, blur, L2 normalisation and head epilogues in tests/test_gpu_layer_ops.py."""
     g = torch.Generator().manual_seed(1)
     a = F.normalize(torch.randn(2, 256, 6, 8, generator=g))
     b = F.normalize(torch.randn(2, 256, 6, 8, generator=g))
     got = rf.model.CorrNeigh(7)(a.cuda(), b.cuda()).cpu()
     close(got, MO.corr_neigh(a, b, 7), 1e-6)
-    logits = torch.randn(2, 49, 5, 9, generator=g) * 3
-    p = F.softmax(logits, dim=1)
-    gx = (torch.arange(49) % 7 - 3).float().view(1, 49, 1, 1)
-    gy = (torch.arange(49) // 7 - 3).float().view(1, 49, 1, 1)
-    ref = torch.cat(((p * gx).sum(1, keepdim=True) / 9 * 2, (p * gy).sum(1, keepdim=True) / 5 * 2), 1)
-    close(rf.ops.softmax_flow(rf.ops.Ragged.from_nchw(logits.cuda()), 7).cpu(), ref, 1e-6)
-    x = torch.randn(1000, generator=g) * 5
-    close(rf.ops.sigmoid(x.cuda()).cpu(), torch.sigmoid(x), 1e-6)
 
 
 @pytest.mark.parametrize("n,c,h,w,k,ldo,mode", [(1, 256, 60, 80, 7, 64, 2), (2, 256, 6, 8, 7, 49, 0), (1, 64, 5, 3, 7, 64, 1),

@@ -162,28 +162,6 @@ def test_split_engine_rejects_unsupported_shapes(rf):
                       rf.ops.to_split(torch.randn(8, 32).cuda()))
 
 
-def _run_program(rf, P, x, engine):
-    out, ohw = P.run(x, engine)
-    return rf.ops.Ragged(out.clone(), ohw)
-
-
-def test_split_pool_blur_ops_vs_fp32_engine(rf):
-    """maxpool / blur / poolblur on split tensors == the fp32 kernels on the same values (to split precision)."""
-    from ransac_flow_b200.program import LayerProgram
-    g = torch.Generator().manual_seed(3)
-    xs = [torch.randn(1, 64, 21, 30, generator=g), torch.randn(1, 64, 8, 9, generator=g)]
-    for build in (lambda P: P.maxpool(0, 3, 2, 1), lambda P: P.blur(0, 2), lambda P: P.poolblur(0), lambda P: P.blur(0, 1)):
-        P = LayerProgram(64)
-        build(P)
-        sx = sragged(rf, xs)
-        xr = rf.ops.Ragged(rf.ops.from_split(sx.data), sx.hw)
-        ref = _run_program(rf, P, xr, rf.ops.ENGINE_FP32)
-        got = _run_program(rf, P, sx, rf.ops.ENGINE_SPLIT)
-        assert got.split and got.hw == ref.hw
-        err = (rf.ops.from_split(got.data) - ref.data).abs().max().item()
-        assert err < 1e-6 * max(1.0, ref.data.abs().max().item()), err
-
-
 def test_resnet50_conv4_split_engine_is_fp32_grade(rf):
     """The whole trunk (43 convolutions) on the split engine against the exact-FMA fp32 engine: the normalised features
     differ by fp32-rounding-level amounts, two orders of magnitude below the fp16 / TF32 engines."""

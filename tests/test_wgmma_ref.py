@@ -97,3 +97,86 @@ def test_partial_n_tiles_on_every_engine():
         assert {72, 136, 200} <= couts, name
         if name in ("TF32", "SPLIT_OUT32"):          # fp32 outputs: odd Cout switches the float2 store to the scalar one
             assert {65, 97, 129} <= couts, name
+
+
+def test_tf32_rna_rounds_ties_away_from_zero():
+    x = torch.tensor([1.0 + 2 ** -11, -(1.0 + 2 ** -11), 1.0 + 3 * 2 ** -11, 1.0 + 2 ** -11 - 2 ** -23, 0.0, 2 ** -140 + 2 ** -149])
+    r = R.tf32_rna(x).tolist()
+    assert r[:5] == [1.0 + 2 ** -10, -(1.0 + 2 ** -10), 1.0 + 2 ** -9, 1.0, 0.0]      # ties up in magnitude; below a tie: down
+    assert R.tf32_round(x[:1]).tolist() == [1.0]                                       # ties to even differs exactly there
+    g = torch.Generator().manual_seed(3)
+    y = torch.randn(10000, generator=g) * 100
+    t = R.tf32_rna(y)
+    assert bool(R.is_tf32(t).all()) and float(((y - t) / y).abs().max()) <= 2 ** -11
+    tie = (y.view(torch.int32) & 0x1FFF) == 0x1000
+    assert torch.equal(t[~tie], R.tf32_round(y)[~tie])
+
+
+def _layer_images(seed, c, sizes):
+    g = torch.Generator().manual_seed(seed)
+    return [torch.randn(1, c, h, w, generator=g) * 3 for h, w in sizes]
+
+
+@pytest.mark.parametrize("stride", [1, 2])
+def test_blur_and_poolblur_refs_match_the_oracle(stride):
+    """blur_ref == MO.blur_downsample and poolblur_ref == MO.blur_downsample(max_pool2d(x, 2, 1), 2) within the fp32
+    rounding of the oracle's own 9-term sums (gamma_9 of the filter on |x|), at the smallest sizes and odd / even ones."""
+    import torch.nn.functional as F
+    from oracle import model_oracle as MO
+    for x in _layer_images(stride, 6, [(2, 2), (3, 3), (2, 9), (9, 2), (7, 8), (8, 7), (16, 24)]):
+        ref, absref = R.blur_ref(x, stride)
+        R.check(MO.blur_downsample(x, stride), ref, absref, 0.0, R.gamma(9), what="blur")
+        if stride == 2 and min(x.shape[2:]) >= 3:
+            ref, absref = R.poolblur_ref(x)
+            R.check(MO.blur_downsample(F.max_pool2d(x, 2, 1), 2), ref, absref, 0.0, R.gamma(9), what="poolblur")
+    # replicate instead of reflect padding is outside the bound
+    x = _layer_images(9, 4, [(5, 6)])[0]
+    ref, absref = R.blur_ref(x, stride)
+    a = torch.tensor([1.0, 2.0, 1.0])
+    f = (a[:, None] * a[None, :] / 16)[None, None].repeat(4, 1, 1, 1)
+    with pytest.raises(AssertionError):
+        R.check(F.conv2d(F.pad(x, (1, 1, 1, 1), mode="replicate"), f, stride=stride, groups=4), ref, absref, 0.0, R.gamma(9))
+
+
+def test_maxpool_and_im2col_refs_match_torch():
+    import torch.nn.functional as F
+    for x in _layer_images(4, 5, [(1, 1), (1, 7), (6, 1), (9, 12), (13, 8)]):
+        assert torch.equal(R.maxpool_ref(x, 3, 2, 1), F.max_pool2d(x, 3, 2, 1).double())
+        if min(x.shape[2:]) >= 2:
+            assert torch.equal(R.maxpool_ref(x, 2, 1, 0), F.max_pool2d(x, 2, 1, 0).double())
+        for k, s, p, kpad in ((7, 2, 3, 160), (3, 1, 1, 32), (7, 1, 3, 160), (3, 2, 1, 64), (5, 1, 2, 128)):
+            if k * k * x.shape[1] > kpad:
+                continue
+            ho, wo = R.out_hw(x.shape[2], x.shape[3], k, s, p)
+            u = F.unfold(x, k, padding=p, stride=s)[0]                                  # (C * k * k, L) in (c, r, s) order
+            u = u.view(x.shape[1], k * k, ho * wo).permute(2, 1, 0).reshape(ho * wo, -1)  # -> (r, s, c)
+            got = R.im2col_ref(x, k, s, p, kpad)
+            assert got.shape == (ho * wo, kpad) and torch.equal(got[:, :u.shape[1]], u) and not bool(got[:, u.shape[1]:].any())
+
+
+def test_l2norm_ref_matches_f_normalize():
+    import torch.nn.functional as F
+    g = torch.Generator().manual_seed(5)
+    C = 132
+    x = torch.randn(40, C, generator=g) * torch.logspace(-3, 3, 40).view(-1, 1)
+    x[3] = 0
+    x[7] = x[7] / x[7].norm() * 3e-14                 # below the eps: x / 1e-12
+    ref = R.l2norm_ref(x)
+    R.check(F.normalize(x), ref, ref, R.gamma(C) / 2 + 2 * R.U, 0.0)            # the kernels' bound
+    assert not bool(ref[3].any()) and abs(float(ref[7].norm()) - 0.03) < 1e-6
+    mask = torch.ones(40, dtype=torch.uint8)
+    mask[::3] = 0
+    m = R.l2norm_ref(x, mask)
+    assert not bool(m[::3].any()) and torch.equal(m[1::3], ref[1::3])
+
+
+@pytest.mark.parametrize("k", [3, 5, 7])
+def test_softmax_flow_ref_matches_net_flow_coarse(k, monkeypatch):
+    """softmax_flow_ref == MO.net_flow_coarse with its convolution trunk replaced by the identity (the epilogue alone), within
+    the bound the kernel is held to."""
+    from oracle import model_oracle as MO
+    monkeypatch.setattr(MO, "_trunk", lambda corr, sd: corr)
+    g = torch.Generator().manual_seed(k)
+    logits = torch.randn(2, k * k, 5, 9, generator=g) * 3
+    ref, absf = R.softmax_flow_ref(logits, k)
+    R.check(MO.net_flow_coarse(logits, None, k), ref, absf, R.U, (k * k + 8) * R.U)

@@ -15,6 +15,9 @@ Operands as consumed:
   3xTF32 (correlation precision 1): the fp32 values (hi + lo, the omitted lo * lo and the TF32 reading of lo in the allowance);
   fp16 (engines 2, 3): the fp16 values;
   split (engines 4, 5, the stem on engine 4, correlation precision 2): hi + lo * 2^-11 of the fp16 planes.
+
+The fp64 references of the SIMT layer kernels (max-pool, blur, pool + blur, im2col, L2 normalisation, the flow head's
+softmax epilogue) live here too; tests/test_gpu_layer_ops.py holds their bounds.
 """
 import ctypes as C
 
@@ -82,15 +85,26 @@ def from_split(s):
 
 
 def tf32_round(t):
-    """fp32 -> nearest TF32 value (ties to even), as FoldedConv packs the weights and round_out stores ReLU'd activations."""
+    """fp32 -> nearest TF32 value (ties to even), as FoldedConv packs the weights (model.py).  The kernels' round_out is
+    tf32_rna."""
     b = t.float().contiguous().view(torch.int32)
     return ((b + 0xFFF + ((b >> 13) & 1)) & ~0x1FFF).view(torch.float32)
+
+
+def tf32_rna(t):
+    """fp32 -> nearest TF32 value, ties away from zero: cvt.rna.tf32.f32, what round_tf32 (csrc/common.cuh) stores wherever a
+    kernel's round_out is set (ReLU'd convolution outputs, engine 1's blur / pool + blur / im2col outputs)."""
+    b = t.float().contiguous().view(torch.int32)
+    return ((b + 0x1000) & ~0x1FFF).view(torch.float32)
 
 
 def operand(x, kind):
     """(tensor the kernel reads, fp64 value it stands for) of an fp32 tensor.  TF32 operands are given to the kernel already
     TF32-representable, as the library's own producers store them (weights rounded once, activations rounded after ReLU):
-    their products are exact whatever the MMA does with the low 13 bits."""
+    their products are exact whatever the MMA does with the low 13 bits.  "f32": the fp32 values as they are (SIMT kernels)."""
+    if kind == "f32":
+        x = x.float()
+        return x, x.double()
     if kind == "tf32":
         t = tf32_round(x)
         return t, t.double()
@@ -136,6 +150,77 @@ def check(got, ref, absref, r_out, c, atol=0.0, what=""):
         raise AssertionError("%s: %d of %d elements outside |got - ref| <= %.3g |ref| + %.3g absref + %.3g; first at %s: got %r ref %r "
                              "absref %r" % (what, bad.shape[0], ok.numel(), r_out, c, atol, i, got[i].item(), ref[i].item(), absref[i].item()))
     return float((err / b.clamp_min(1e-300)).max()) if err.numel() else 0.0
+
+
+# ------------------------------------------------------------------ the layer kernels between the convolutions (elementwise.cu)
+U = 2.0 ** -24                 # fp32 unit roundoff
+EPS_L2 = float(np.float32(1e-12))
+
+
+def gamma(n):
+    """Bound on the relative error of an n-term fp32 sum or product chain: n u / (1 - n u)."""
+    return n * U / (1 - n * U)
+
+
+def _blur64(x, stride):
+    c = x.shape[1]
+    a = torch.tensor([1.0, 2.0, 1.0], dtype=torch.float64, device=x.device)
+    f = (a[:, None] * a[None, :] / 16.0).expand(c, 1, 3, 3).contiguous()
+    return F.conv2d(F.pad(x, (1, 1, 1, 1), mode="reflect"), f, stride=stride, groups=c)
+
+
+def blur_ref(x, stride):
+    """model/downsample.py: ReflectionPad2d(1) + depthwise [1 2 1]^2 / 16 at ``stride`` of (N, C, H, W), in fp64, and the same
+    filter on |x|."""
+    x = x.double()
+    return _blur64(x, stride), _blur64(x.abs(), stride)
+
+
+def poolblur_ref(x):
+    """MaxPool2d(2, stride 1), then the stride-2 blur reflecting on the (H - 1) x (W - 1) pooled map; absref on |pooled|."""
+    p = F.max_pool2d(x.double(), 2, 1)
+    return _blur64(p, 2), _blur64(p.abs(), 2)
+
+
+def maxpool_ref(x, k, stride, pad):
+    """The maximum over the in-image part of each window (the padding never wins), fp64."""
+    return F.max_pool2d(x.double(), k, stride, pad)
+
+
+def im2col_ref(x, k, stride, pad, kpad):
+    """[Ho * Wo, kpad] rows of a (1, C, H, W) image: the k x k patch of each output pixel in (r, s, c) order, zero outside the
+    image and in columns k * k * C .. kpad - 1.  Same dtype as x: values are copied, never computed."""
+    _, c, h, w = x.shape
+    ho, wo = out_hw(h, w, k, stride, pad)
+    xp = F.pad(x, (pad, pad, pad, pad))
+    taps = [xp[0, :, r:r + stride * (ho - 1) + 1:stride, s:s + stride * (wo - 1) + 1:stride] for r in range(k) for s in range(k)]
+    rows = torch.stack(taps, 0).permute(2, 3, 0, 1).reshape(ho * wo, k * k * c)      # (tap, C, Ho, Wo) -> (Ho, Wo, tap, C)
+    return F.pad(rows, (0, kpad - k * k * c))
+
+
+def l2norm_ref(x, mask=None):
+    """x / max(||x||_2, fp32(1e-12)) per row of [P, C], in fp64 (F.normalize with the kernels' fp32 eps); rows whose mask
+    is 0 are zero."""
+    x = x.double()
+    y = x / x.norm(dim=1, keepdim=True).clamp_min(EPS_L2)
+    if mask is not None:
+        y = torch.where(mask.view(-1, 1).to(y.device) != 0, y, torch.zeros_like(y))
+    return y
+
+
+def softmax_flow_ref(logits, k):
+    """NetFlowCoarse's epilogue (model/model.py; MO.net_flow_coarse after its trunk) on (N, k*k, h, w) logits, in fp64:
+    p = softmax over the k*k channels, flow = (sum p gx / w * 2, sum p gy / h * 2) with channel i*k + j at the offset
+    (gx, gy) = (j - k//2, i - k//2).  Returns (flow (N, 2, h, w), the same sums of p |g|)."""
+    lg = logits.double()
+    _, kk, h, w = lg.shape
+    p = torch.softmax(lg, 1)
+    q = torch.arange(kk, device=lg.device)
+    gx = (q % k - k // 2).double().view(1, -1, 1, 1)
+    gy = (q // k - k // 2).double().view(1, -1, 1, 1)
+    flow = torch.cat(((p * gx).sum(1, keepdim=True) / w * 2, (p * gy).sum(1, keepdim=True) / h * 2), 1)
+    absf = torch.cat(((p * gx.abs()).sum(1, keepdim=True) / w * 2, (p * gy.abs()).sum(1, keepdim=True) / h * 2), 1)
+    return flow, absf
 
 
 # ------------------------------------------------------------------ tile widths (mirror of pick_tw in csrc/gemm_tc.cu)
