@@ -742,6 +742,13 @@ __device__ __forceinline__ float unnormalize(float coord, int size, int align_co
     return align_corners ? ((coord + 1.f) / 2.f) * (float)(size - 1) : ((coord + 1.f) * (float)size - 1.f) / 2.f;
 }
 
+// torch's CUDA grid sampler moves a source coordinate that is not finite or lies beyond the int range outside the image
+// (safe_downgrade_to_int_range), so it samples nothing.  Without this a NaN coordinate would convert to pixel 0 and
+// return NaN instead of the 0 F.grid_sample returns.  (|c| = 2^31, which torch keeps, samples nothing either way.)
+__device__ __forceinline__ float in_int_range(float c) {
+    return fabsf(c) < 2147483648.f ? c : -100.f;
+}
+
 struct Strides4 { long long n, c, h, w; };
 
 __global__ void grid_sample_kernel(const float* __restrict__ in, int N, int C, int Hin, int Win, Strides4 is,
@@ -754,7 +761,7 @@ __global__ void grid_sample_kernel(const float* __restrict__ in, int N, int C, i
     int rem = (int)(t - n * hw);
     int r = rem / Wout, c = rem - r * Wout;
     float2 g = __ldg(reinterpret_cast<const float2*>(grid) + t);
-    float ix = unnormalize(g.x, Win, align_corners), iy = unnormalize(g.y, Hin, align_corners);
+    float ix = in_int_range(unnormalize(g.x, Win, align_corners)), iy = in_int_range(unnormalize(g.y, Hin, align_corners));
     float fx = floorf(ix), fy = floorf(iy);
     int x0 = (int)fx, y0 = (int)fy, x1 = x0 + 1, y1 = y0 + 1;
     float nw = (fx + 1.f - ix) * (fy + 1.f - iy), ne = (ix - fx) * (fy + 1.f - iy);

@@ -336,8 +336,10 @@ def grid_sample(inp, grid, align_corners=False):
     """F.grid_sample(inp, grid) bilinear / zeros.  Output has the memory format of the input."""
     need_cuda(inp, grid)
     inp = inp if inp.dtype == torch.float32 else inp.float()
-    grid = grid.contiguous().float()
     N, Cc, Hin, Win = inp.shape
+    if grid.dim() != 4 or grid.shape[0] != N or grid.shape[3] != 2:
+        raise ValueError("grid_sample: grid must be (N, Hout, Wout, 2) with the input's N = %d, got %s" % (N, tuple(grid.shape)))
+    grid = grid.contiguous().float()
     Hout, Wout = grid.shape[1], grid.shape[2]
     if inp.stride(1) == 1 and Cc > 1:
         out = torch.empty((N, Hout, Wout, Cc), device=inp.device, dtype=torch.float32).permute(0, 3, 1, 2)
@@ -362,7 +364,14 @@ def compose_fine(flowDown8, match12, match21, coarse, clamp=True, align_corners=
     """Fused tail of PredFlowMask.  flowDown8 (1,2,h8,w8); match12/match21 (1,1,h8,w8) or None; coarse (1,Hc,Wc,2).
     ``size`` = (H, W) of the outputs when it differs from the coarse grid's (the KITTI two-level flow)."""
     need_cuda(flowDown8, match12, match21, coarse)
+    if flowDown8.dim() != 4 or flowDown8.shape[:2] != (1, 2):
+        raise ValueError("compose_fine: flowDown8 must be (1, 2, h8, w8), got %s" % (tuple(flowDown8.shape),))
     _, _, h8, w8 = flowDown8.shape
+    for name, m in (("match12", match12), ("match21", match21)):
+        if m is not None and tuple(m.shape) != (1, 1, h8, w8):
+            raise ValueError("compose_fine: %s must be (1, 1, %d, %d), got %s" % (name, h8, w8, tuple(m.shape)))
+    if coarse.dim() != 4 or coarse.shape[0] != 1 or coarse.shape[3] != 2:
+        raise ValueError("compose_fine: coarse must be (1, Hc, Wc, 2), got %s" % (tuple(coarse.shape),))
     _, Hc, Wc, _ = coarse.shape
     H, W = (Hc, Wc) if size is None else (int(size[0]), int(size[1]))
     dev = coarse.device

@@ -42,31 +42,6 @@ def test_remove_small_cc_fuzz_vs_oracle(rf, h, w, seed):
         assert np.array_equal(got, ref), (cc_th, int((got != ref).sum()))
 
 
-@pytest.mark.parametrize("hc,wc,h,w,m21", [(48, 64, 56, 80, True), (40, 56, 40, 56, True), (96, 128, 48, 64, False), (30, 100, 47, 121, True)])
-def test_compose_fine_with_its_own_coarse_grid(rf, hc, wc, h, w, m21):
-    """rf_compose_fine_ex: the coarse grid sampled at another resolution's positions (evalKITTI/evaluation.py:296-302) vs
-    F.interpolate / F.grid_sample on the CPU."""
-    rs = np.random.RandomState(hc + w)
-    f8 = torch.from_numpy((rs.randn(1, 2, 6, 9) * 0.05).astype(np.float32))
-    m12 = torch.from_numpy(rs.rand(1, 1, 6, 9).astype(np.float32))
-    m21t = torch.from_numpy(rs.rand(1, 1, 6, 9).astype(np.float32))
-    Hm = (np.eye(3) + rs.uniform(-0.05, 0.05, (3, 3))).astype(np.float32)
-    coarse = WO.warp_grid(Hm[None], hc, wc)
-    grid = WO.base_grid(h, w)
-    flow12, flowUp = WO.compose_fine(f8, coarse, grid, clamp=True)
-    match = WO.interpolate_bilinear(m12, (h, w))
-    if m21:
-        match = match * WO.grid_sample(WO.interpolate_bilinear(m21t, (h, w)), flowUp)
-    match = match * WO.inside_mask(flow12)
-    got12, gotm, gotUp = rf.ops.compose_fine(f8.cuda(), m12.cuda(), m21t.cuda() if m21 else None, coarse.cuda(), clamp=True,
-                                             want_flowUp=True, size=(h, w))
-    assert tuple(got12.shape) == (1, h, w, 2) and tuple(gotm.shape) == (1, 1, h, w)
-    assert np.abs(gotUp.cpu().numpy() - flowUp.numpy()).max() < 5e-6
-    assert np.abs(got12.cpu().numpy() - flow12.numpy()).max() < 5e-6
-    far = (np.abs(np.abs(flow12.numpy()) - 1) > 1e-4).all(-1)[0]
-    assert np.abs(gotm.cpu().numpy() - match.numpy())[0, 0][far].max() < 5e-6
-
-
 def test_kitti_pred_flow_mask_vs_reference(rf):
     """evaluation/evalKITTI/evaluation.py:49-81 (second level: coarse flow on 48x64, outputs on 56x80) against the
     unmodified reference's golden output, fp32 engine."""

@@ -145,53 +145,6 @@ def test_device_lanczos_bit_exact_vs_pil(rf, size):
     assert np.array_equal(got, ref)
 
 
-def test_warp_grid_and_grid_sample(rf):
-    rs = np.random.RandomState(2)
-    Hs = np.stack([np.eye(3) + rs.uniform(-0.1, 0.1, (3, 3)) for _ in range(3)]).astype(np.float32)
-    g = rf.ops.warp_grid(torch.from_numpy(Hs).cuda(), 31, 45)
-    close(g.cpu(), WO.warp_grid(Hs, 31, 45), 2e-6)
-    w = rf.kornia_geometry.HomographyWarper(31, 45).warp_grid(torch.from_numpy(Hs).cuda())
-    assert torch.equal(w, g)
-    img = torch.rand(3, 3, 20, 26)
-    grid = WO.warp_grid(Hs, 31, 45) * 1.2                                  # some samples fall outside
-    for ac in (False, True):
-        ref = F.grid_sample(img, grid, mode="bilinear", padding_mode="zeros", align_corners=ac)
-        close(rf.ops.grid_sample(img.cuda(), grid.cuda(), ac).cpu(), ref, 2e-6)
-        cl = img.cuda().contiguous(memory_format=torch.channels_last)
-        close(rf.ops.grid_sample(cl, grid.cuda(), ac).cpu(), ref, 2e-6)
-    x = torch.rand(2, 2, 6, 8)
-    close(rf.ops.upsample_bilinear(x.cuda(), (48, 64)).cpu(), F.interpolate(x, size=(48, 64), mode="bilinear"), 1e-6)
-    big = torch.rand(1, 1, 48, 64)
-    close(rf.ops.upsample_bilinear(big.cuda(), (3, 4)).cpu(), F.interpolate(big, size=(3, 4), mode="bilinear"), 1e-6)
-
-
-@pytest.mark.parametrize("m21", [False, True])
-def test_compose_fine(rf, m21):
-    rs = np.random.RandomState(3)
-    H, W = 48, 64
-    f8 = torch.from_numpy((rs.randn(1, 2, 6, 8) * 0.05).astype(np.float32))
-    m12 = torch.from_numpy(rs.rand(1, 1, 6, 8).astype(np.float32))
-    m21t = torch.from_numpy(rs.rand(1, 1, 6, 8).astype(np.float32))
-    Hm = (np.eye(3) + rs.uniform(-0.1, 0.1, (3, 3))).astype(np.float32)[None]
-    coarse = WO.warp_grid(Hm, H, W)
-    grid = WO.base_grid(H, W)
-    flow12, flowUp = WO.compose_fine(f8, coarse, grid, clamp=True)
-    match = WO.interpolate_bilinear(m12, (H, W))
-    if m21:
-        match = match * WO.grid_sample(WO.interpolate_bilinear(m21t, (H, W)), flowUp)
-    match = match * WO.inside_mask(flow12)
-    g12, gm, gup = rf.ops.compose_fine(f8.cuda(), m12.cuda(), m21t.cuda() if m21 else None, coarse.cuda(), want_flowUp=True)
-    close(gup.cpu(), flowUp, 2e-6)
-    close(g12.cpu(), flow12, 5e-6)
-    # the inside-mask is a hard threshold at |flow| == 1: compare away from the threshold
-    far = (np.abs(np.abs(flow12.numpy()) - 1) > 1e-4).all(-1)[0]
-    assert np.abs(gm.cpu().numpy()[0, 0] - match.numpy()[0, 0])[far].max() < 5e-6
-    # no clamp (quick_start/align2images.py:91-95)
-    f_nc, _ = WO.compose_fine(f8, coarse, grid, clamp=False)
-    g_nc, _, _ = rf.ops.compose_fine(f8.cuda(), None, None, coarse.cuda(), clamp=False, want_match=False)
-    close(g_nc.cpu(), f_nc, 5e-6)
-
-
 def test_warp_grid_reference_internal_consistency(rf):
     """rf_warp_grid under the pin the reference itself offers for kornia 0.1.4 (see tests/test_oracle_golden.py): the identity
     (and any power-of-two multiple of it) reproduces, bit for bit, the base grid the fine flow is added to on this side

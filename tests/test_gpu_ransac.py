@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 import torch
 
+import geometry_ref as G
 from conftest import golden
 from oracle import outil_oracle as OO
 from oracle import synth
@@ -32,8 +33,7 @@ def test_golden_cases(rf, name):
     # per-hypothesis: chunk-0 homographies and reprojection errors
     us = OO.unique_samples(g["samples"])[: len(g["chunk0_H"])]
     Hd = rf.ops.homography_dlt(torch.from_numpy(g["match1"][us]).cuda(), torch.from_numpy(g["match2"][us]).cuda()).cpu().numpy()
-    cond_ok = np.abs(Hd - g["chunk0_H"]).reshape(len(us), -1).max(1) < 1e-5
-    assert cond_ok.mean() > 0.97                                   # ill-conditioned (near-collinear) samples may differ
+    G.dlt_check(Hd.reshape(len(us), 9), g["match1"][us], g["match2"][us])     # sign included wherever the bound is below 1
     err = rf.ops.prediction(torch.from_numpy(g["match1"]).cuda(), torch.from_numpy(g["match2"]).cuda(),
                             torch.from_numpy(g["chunk0_H"][:8]).cuda()).cpu().numpy()
     assert np.array_equal(err, OO.Prediction(g["match1"], g["match2"], g["chunk0_H"][:8]))   # same fp32 op order
