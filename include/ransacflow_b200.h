@@ -176,6 +176,8 @@ typedef struct rf_layer {
 } rf_layer_t;
 #define RF_LAYER_OUT_F32 1          /* conv: fp16 operands, fp32 output (RF_ENGINE_F16_OUT32; engine 4: RF_ENGINE_SPLIT_OUT32) */
 #define RF_LAYER_TF32 2             /* conv: fp32 input and output on the TF32 engine (e.g. a 49-channel head after an OUT_F32 layer) */
+#define RF_LAYER_STEM_POOL 4        /* RF_OP_STEM7 whose output only feeds the next layer, a 3x3 / stride 2 / pad 1 RF_OP_MAXPOOL: both run
+                                       as one kernel that writes the max-pool's dst slot; the stem's own dst slot is never written */
 /* engine 2: slots hold fp16 except the input of an RF_OP_IM2COL (the fp32 image; row length = Cout % 64 == 0), the
  * output of an RF_LAYER_OUT_F32 conv and the input / output of an RF_LAYER_TF32 conv; pooling and blur run in fp16. */
 /* engine 4: slots hold split tensors ([2][P][C] fp16) except the fp32 input image of an RF_OP_IM2COL / RF_OP_STEM7 and the fp32

@@ -1,5 +1,6 @@
 // Shared helpers for the ransacflow_b200 CUDA library (sm_90a only).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -40,6 +41,22 @@ inline int fail_msg(const char* msg) {
         if (!(cond)) return rf::fail_msg(msg " [" #cond "]");           \
     } while (0)
 
+// engine 4: eight fp32 values as a split tensor's hi / lo planes (`plane` elements apart), clamped to the fp16 range:
+// hi = fp16(x), lo = fp16((x - hi) * 2^11).  Shared by the pooling / blur kernels and the fused stem + max-pool.
+__device__ __forceinline__ void split_store8(__half* p, long long plane, const float (&v)[8]) {
+    uint4 th, tl;
+    __half2* h = reinterpret_cast<__half2*>(&th);
+    __half2* l = reinterpret_cast<__half2*>(&tl);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const float a = fminf(fmaxf(v[2 * e], -65504.f), 65504.f), b = fminf(fmaxf(v[2 * e + 1], -65504.f), 65504.f);
+        h[e] = __floats2half2_rn(a, b);
+        const float2 f = __half22float2(h[e]);
+        l[e] = __floats2half2_rn((a - f.x) * 2048.f, (b - f.y) * 2048.f);
+    }
+    *reinterpret_cast<uint4*>(p) = th;
+    *reinterpret_cast<uint4*>(p + plane) = tl;
+}
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
 inline int current_device() {

@@ -151,22 +151,8 @@ template <> struct Vec16<__half> {
     }
 };
 // engine 4: split tensors, two fp16 planes `plane` elements apart (x = hi + lo * 2^-11); values are rebuilt exactly in fp32,
-// results are split again (gemm_tc.cu)
+// results are split again (split_store8, common.cuh)
 struct SplitH {};
-__device__ __forceinline__ void split_store8(__half* p, long long plane, const float (&v)[8]) {
-    uint4 th, tl;
-    __half2* h = reinterpret_cast<__half2*>(&th);
-    __half2* l = reinterpret_cast<__half2*>(&tl);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        const float a = fminf(fmaxf(v[2 * e], -65504.f), 65504.f), b = fminf(fmaxf(v[2 * e + 1], -65504.f), 65504.f);
-        h[e] = __floats2half2_rn(a, b);
-        const float2 f = __half22float2(h[e]);
-        l[e] = __floats2half2_rn((a - f.x) * 2048.f, (b - f.y) * 2048.f);
-    }
-    *reinterpret_cast<uint4*>(p) = th;
-    *reinterpret_cast<uint4*>(p + plane) = tl;
-}
 __device__ __forceinline__ void split_load8(const __half* p, long long plane, float (&v)[8]) {
     const uint4 th = __ldg(reinterpret_cast<const uint4*>(p)), tl = __ldg(reinterpret_cast<const uint4*>(p + plane));
     const __half2* h = reinterpret_cast<const __half2*>(&th);

@@ -396,33 +396,52 @@ wg_kernel(const __grid_constant__ WgParams p) {
 
 
 // ------------------------------------------------------------------------------------------------------------
-// ResNet-50 stem, fused: conv 7x7 / stride 2 / pad 3 on the 3-channel fp32 image + folded BN + ReLU -> fp16 (engine 2) or split
-// (engine 4) NHWC, without an im2col matrix in HBM.  One CTA = 16 x 8 output pixels x 64 channels, 256 threads:
-//   all threads : stage the 21 x 111 input window (split into (hi, lo) pairs once), then two threads per output pixel build its
-//                 147-long (r, s, c) patch as hi / lo planes in the 128-byte-swizzled K-major layout (3 K blocks of 64; 147..191
-//                 are zeros), fence.proxy.async;
-//   warpgroups  : 64 pixels each, wgmma over the three K blocks against the weights TMA-loaded at CTA start; register epilogue.
+// ResNet-50 front end, fused: conv 7x7 / stride 2 / pad 3 on the 3-channel fp32 image + folded BN + ReLU and, with pool = 1,
+// the 3x3 / stride 2 / pad 1 max-pool on its output -> fp16 (engine 2) or split (engine 4) NHWC.  No im2col matrix goes to
+// HBM, and with pool = 1 neither does the full-resolution stem output.
+// Persistent, 256 threads, 1 CTA per SM: the weights are TMA-loaded once per CTA and stay resident.  A work unit (step) is a
+// tile of 4 stem rows x 32 stem columns (128 pixels x 64 channels); units run down column strips (steps fastest) and CTA b
+// takes the contiguous range [U b / G, U (b + 1) / G) of them.  Per step:
+//   build    : two threads per pixel build its 147-long (r, s, c) patch from the staged 13 x 69 x 3 input window (split into
+//              (hi, lo) pairs once, at staging) as hi / lo planes in the 128-byte-swizzled K-major layout (3 K blocks of 64;
+//              147..191 are zeros); K block kb + 1 is built while the wgmmas of K block kb run;
+//   MMA      : warpgroup g = pixels 64g .. 64g + 63, wgmma over the three K blocks against the resident weights;
+//   prefetch : while the MMAs run, the next step's input window is loaded into registers (staged after the MMAs);
+//   epilogue : pool = 0: bias, ReLU, conversion and stores from the registers.  pool = 1: the stem values go to a shared tile
+//              (engine 4: split and rebuilt, i.e. the values the max-pool of a split tensor reads), then the step's 2 pooled
+//              rows x 15 pooled columns are reduced there and stored with 16-byte stores.
+// Pooling: pooled column q needs stem columns 2q - 1 .. 2q + 1, so the tiles of strip s start at stem column 30 s - 1 and
+// overlap the strip to their left by one column (1/16 of the stem is computed twice); pooled row p needs stem rows
+// 2p - 1 .. 2p + 1, so each step keeps its last stem row for the next step of the strip (two alternating tiles).  A CTA whose
+// range starts inside a strip first computes the step above, without pooling it.  As in the standalone max-pool, window
+// positions outside the stem image are skipped and the maximum runs over (r, s) in the same order.
 // ------------------------------------------------------------------------------------------------------------
-constexpr int SS_TW = 16, SS_TH = 8, SS_K = 7, SS_C = 3, SS_KK = 147, SS_KB = 3;
-constexpr int SS_IN_W = ((SS_TW - 1) * 2 + SS_K) * SS_C;                  // 111 floats per staged input row
-constexpr int SS_IN_H = (SS_TH - 1) * 2 + SS_K;                           // 21 rows
-constexpr int SS_IN_LD = 112;
-constexpr int SS_THREADS = 256;
-constexpr int SS_B_PLANE = 64 * 128;                                      // one K block of 64 weight rows: 8 KB
-constexpr int SS_OFF_ALO = SS_KB * TC_A_BYTES;                            // 48 KB: lo planes of the patches
-constexpr int SS_OFF_B = 2 * SS_KB * TC_A_BYTES;                          // 96 KB
-constexpr int SS_OFF_IN = SS_OFF_B + SS_KB * 2 * SS_B_PLANE;              // 144 KB
-constexpr int SS_OFF_BAR = SS_OFF_IN + SS_IN_H * SS_IN_LD * 4;
-constexpr int SS_SMEM = SS_OFF_BAR + 64 + 1024;
-constexpr int SS_NLD = (SS_IN_H * SS_IN_W + SS_THREADS - 1) / SS_THREADS;  // window floats per thread
-static_assert(SS_SMEM <= 227 * 1024, "stem shared memory");
+constexpr int ST_TW = 32, ST_TH = 4, ST_K = 7, ST_C = 3, ST_KK = 147, ST_KB = 3;
+constexpr int ST_PW = (ST_TW - 2) / 2, ST_PH = ST_TH / 2;                // pooled columns per strip, pooled rows per step
+constexpr int ST_IN_W = ((ST_TW - 1) * 2 + ST_K) * ST_C;                  // 207 floats per staged input row
+constexpr int ST_IN_H = (ST_TH - 1) * 2 + ST_K;                           // 13 rows
+constexpr int ST_IN_LD = 208;
+constexpr int ST_THREADS = 256;
+constexpr int ST_B_PLANE = 64 * 128;                                      // one K block of 64 weight rows: 8 KB
+constexpr int ST_OFF_ALO = ST_KB * TC_A_BYTES;                            // 48 KB: lo planes of the patches
+constexpr int ST_OFF_B = 2 * ST_KB * TC_A_BYTES;                          // 96 KB
+constexpr int ST_OFF_T = ST_OFF_B + ST_KB * 2 * ST_B_PLANE;               // 144 KB: two stem tiles of 128 pixels x 64 fp32
+constexpr int ST_T_BYTES = 128 * 64 * 4;
+constexpr int ST_OFF_IN = ST_OFF_T + 2 * ST_T_BYTES;                      // 208 KB
+constexpr int ST_OFF_BAR = ST_OFF_IN + ST_IN_H * ST_IN_LD * 4;
+constexpr int ST_SMEM = ST_OFF_BAR + 64 + 1024;
+constexpr int ST_NLD = (ST_IN_H * ST_IN_W + ST_THREADS - 1) / ST_THREADS;  // window floats per thread
+static_assert(ST_SMEM <= 227 * 1024, "stem shared memory");
+static_assert(ST_PH * ST_PW * 8 <= ST_THREADS, "one thread per (pooled pixel, 8 channels) of a step");
 
 struct alignas(64) StemParams {
     CUtensorMap mapB;                     // weights (192, 64[, 2]) fp16, box (64, 64[, 2])
-    int nimg;
-    int tile_start[RF_MAX_IMGS + 1];
-    int tiles_x[RF_MAX_IMGS];
-    int H[RF_MAX_IMGS], W[RF_MAX_IMGS], Ho[RF_MAX_IMGS], Wo[RF_MAX_IMGS];
+    int nimg, pool;
+    int unit_start[RF_MAX_IMGS + 1];      // prefix sums of steps per image; [nimg ..] = all steps
+    int steps[RF_MAX_IMGS];               // steps per strip
+    int H[RF_MAX_IMGS], W[RF_MAX_IMGS];   // input image
+    int Hs[RF_MAX_IMGS], Ws[RF_MAX_IMGS]; // stem output
+    int Ho[RF_MAX_IMGS], Wo[RF_MAX_IMGS]; // stored output: pooled (pool = 1) or the stem output
     long long in_pix[RF_MAX_IMGS], out_pix[RF_MAX_IMGS];
     long long plane;                      // split output: elements from the hi to the lo plane
     const float* x;
@@ -437,8 +456,8 @@ __device__ __forceinline__ uint32_t stem_pack_split(float v) {
     return (*reinterpret_cast<uint32_t*>(&hi) & 0xFFFFu) | (*reinterpret_cast<uint32_t*>(&lo) << 16);
 }
 
-// half a patch: the 16-byte chunks 4 * HALF .. 4 * HALF + 3 of K block kb of pixel m, hi and lo planes
-template <int HALF, int kb>
+// half a patch: the 16-byte chunks 4 * HALF .. 4 * HALF + 3 of K block kb of pixel m, hi (and lo) planes
+template <bool SPLIT, int HALF, int kb>
 __device__ __forceinline__ void stem_build_half(const uint32_t* __restrict__ base, uint8_t* sA, int m) {
 #pragma unroll
     for (int cc = 0; cc < 4; ++cc) {
@@ -449,35 +468,92 @@ __device__ __forceinline__ void stem_build_half(const uint32_t* __restrict__ bas
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
             const int k0 = kb * 64 + c8 * 8 + 2 * e, k1 = k0 + 1;
-            const uint32_t a = k0 < SS_KK ? base[(k0 / 21) * SS_IN_LD + (k0 % 21)] : 0u;
-            const uint32_t b = k1 < SS_KK ? base[(k1 / 21) * SS_IN_LD + (k1 % 21)] : 0u;
+            const uint32_t a = k0 < ST_KK ? base[(k0 / 21) * ST_IN_LD + (k0 % 21)] : 0u;
+            const uint32_t b = k1 < ST_KK ? base[(k1 / 21) * ST_IN_LD + (k1 % 21)] : 0u;
             ph[e] = __byte_perm(a, b, 0x5410);          // (hi(a), hi(b))
             pl[e] = __byte_perm(a, b, 0x7632);          // (lo(a), lo(b))
         }
         uint8_t* dst = sA + kb * TC_A_BYTES + m * 128 + ((c8 ^ (m & 7)) << 4);
         *reinterpret_cast<uint4*>(dst) = oh;
-        *reinterpret_cast<uint4*>(dst + SS_OFF_ALO) = ol;
+        if constexpr (SPLIT) *reinterpret_cast<uint4*>(dst + ST_OFF_ALO) = ol;
     }
 }
 
+// K block kb of a step: build it, hand it to the async proxy, issue its wgmmas (one commit group)
+template <bool SPLIT, int kb, int NACC>
+__device__ __forceinline__ void stem_kblock(float (&acc)[NACC][32], const uint32_t* base, uint8_t* sA, const uint8_t* sB, int m, int half,
+                                            int g, uint64_t* bar_b, bool first) {
+    constexpr int NPL = SPLIT ? 2 : 1;
+    if (half == 0) stem_build_half<SPLIT, 0, kb>(base, sA, m);
+    else stem_build_half<SPLIT, 1, kb>(base, sA, m);
+    fence_proxy_async();            // generic-proxy writes -> visible to the tensor core (async proxy)
+    __syncthreads();
+    if (kb == 0 && first) mbar_wait(bar_b, 0);
+    wg_fence();
+    const uint32_t a = smem_u32(sA + kb * TC_A_BYTES + g * (64 * 128)), b = smem_u32(sB + kb * NPL * ST_B_PLANE);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint64_t ah = wg_desc(a + 32 * k), bh = wg_desc(b + 32 * k);
+        if constexpr (SPLIT) {
+            wgmma<false, 64>(acc[1], wg_desc(a + ST_OFF_ALO + 32 * k), bh);
+            wgmma<false, 64>(acc[1], ah, wg_desc(b + ST_B_PLANE + 32 * k));
+        }
+        wgmma<false, 64>(acc[0], ah, bh);
+    }
+    wg_commit();
+}
+
 template <bool SPLIT>
-__global__ void __launch_bounds__(SS_THREADS, 1)
+__global__ void __launch_bounds__(ST_THREADS, 1)
 stem7_kernel(const __grid_constant__ StemParams p) {
     constexpr int NPL = SPLIT ? 2 : 1;
+    constexpr int NACC = SPLIT ? 2 : 1;
+    constexpr int PIX_BYTES = SPLIT ? 256 : 128;    // one stem pixel in a shared tile: 64 fp32 (engine 2: fp16)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sA = smem;
-    uint8_t* sB = smem + SS_OFF_B;
-    uint32_t* sIn = reinterpret_cast<uint32_t*>(smem + SS_OFF_IN);
-    uint64_t* bar_b = reinterpret_cast<uint64_t*>(smem + SS_OFF_BAR);
-    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+    uint8_t* sB = smem + ST_OFF_B;
+    uint8_t* sT = smem + ST_OFF_T;
+    uint32_t* sIn = reinterpret_cast<uint32_t*>(smem + ST_OFF_IN);
+    uint64_t* bar_b = reinterpret_cast<uint64_t*>(smem + ST_OFF_BAR);
+    const int t = threadIdx.x, warp = t >> 5, lane = t & 31, g = warp >> 2;
+    const long long units = p.unit_start[RF_MAX_IMGS];
+    const int u_begin = (int)(units * blockIdx.x / gridDim.x), u_end = (int)(units * (blockIdx.x + 1) / gridDim.x);
 
-    int img = 0;
+    struct Unit { int img, strip, j, r0, c0; };
+    auto decode = [&](int u) {
+        Unit U;
+        U.img = 0;
 #pragma unroll
-    for (int j = 1; j < RF_MAX_IMGS; ++j) img += (j < p.nimg && (int)blockIdx.x >= p.tile_start[j]) ? 1 : 0;
-    const int tloc = blockIdx.x - p.tile_start[img];
-    const int tyi = tloc / p.tiles_x[img], txi = tloc - tyi * p.tiles_x[img];
-    const int ox0 = txi * SS_TW, oy0 = tyi * SS_TH;
+        for (int i = 1; i < RF_MAX_IMGS; ++i) U.img += (i < p.nimg && u >= p.unit_start[i]) ? 1 : 0;
+        const int loc = u - p.unit_start[U.img];
+        U.strip = loc / p.steps[U.img];
+        U.j = loc - U.strip * p.steps[U.img];
+        U.r0 = U.j * ST_TH;
+        U.c0 = p.pool ? U.strip * 2 * ST_PW - 1 : U.strip * ST_TW;
+        return U;
+    };
+    float win[ST_NLD];
+    auto load_window = [&](const Unit& U) {         // the zero-padded input window of a step, into registers
+        const int H = p.H[U.img], WC = p.W[U.img] * ST_C;
+        const float* src = p.x + p.in_pix[U.img] * ST_C;
+        const int iy0 = U.r0 * 2 - 3, col0 = (U.c0 * 2 - 3) * ST_C;
+#pragma unroll
+        for (int i = 0; i < ST_NLD; ++i) {
+            const int idx = t + i * ST_THREADS;
+            const int r = idx / ST_IN_W, jj = idx - r * ST_IN_W;
+            const int iy = iy0 + r, col = col0 + jj;
+            win[i] = (idx < ST_IN_H * ST_IN_W && iy >= 0 && iy < H && col >= 0 && col < WC) ? __ldg(src + (long long)iy * WC + col) : 0.f;
+        }
+    };
+    auto stage_window = [&]() {                     // ... split once, into shared memory
+#pragma unroll
+        for (int i = 0; i < ST_NLD; ++i) {
+            const int idx = t + i * ST_THREADS;
+            const int r = idx / ST_IN_W, jj = idx - r * ST_IN_W;
+            if (idx < ST_IN_H * ST_IN_W) sIn[r * ST_IN_LD + jj] = stem_pack_split(win[i]);
+        }
+    };
 
     if (t == 0) {
         mbar_init(bar_b, 1);
@@ -485,90 +561,131 @@ stem7_kernel(const __grid_constant__ StemParams p) {
     }
     __syncthreads();
     if (t == 0) {
-        mbar_expect_tx(bar_b, SS_KB * NPL * SS_B_PLANE);
+        mbar_expect_tx(bar_b, ST_KB * NPL * ST_B_PLANE);
 #pragma unroll
-        for (int kb = 0; kb < SS_KB; ++kb) {
-            if constexpr (SPLIT) tma_load_3d(sB + kb * 2 * SS_B_PLANE, &p.mapB, bar_b, kb * 64, 0, 0);
-            else tma_load_2d(sB + kb * SS_B_PLANE, &p.mapB, bar_b, kb * 64, 0);
+        for (int kb = 0; kb < ST_KB; ++kb) {
+            if constexpr (SPLIT) tma_load_3d(sB + kb * 2 * ST_B_PLANE, &p.mapB, bar_b, kb * 64, 0, 0);
+            else tma_load_2d(sB + kb * ST_B_PLANE, &p.mapB, bar_b, kb * 64, 0);
         }
     }
-    {   // the zero-padded input window, split once
-        const int H = p.H[img], WC = p.W[img] * SS_C;
-        const float* src = p.x + p.in_pix[img] * SS_C;
-        const int iy0 = oy0 * 2 - 3, col0 = (ox0 * 2 - 3) * SS_C;
-#pragma unroll
-        for (int i = 0; i < SS_NLD; ++i) {
-            const int idx = t + i * SS_THREADS;
-            const int r = idx / SS_IN_W, j = idx - r * SS_IN_W;
-            const int iy = iy0 + r, col = col0 + j;
-            if (idx < SS_IN_H * SS_IN_W)
-                sIn[r * SS_IN_LD + j] = stem_pack_split((iy >= 0 && iy < H && col >= 0 && col < WC) ? __ldg(src + (long long)iy * WC + col) : 0.f);
-        }
-    }
+    int u = u_begin;
+    Unit U = decode(u);
+    if (p.pool && U.j > 0) U = decode(--u);         // the step above the range: its last stem row, not pooled
+    load_window(U);
+    stage_window();
     __syncthreads();
-    {   // this pixel's patch, (r, s, c) order: element k = r*21 + s*3 + c sits at sIn[2*py + r][6*px + (k % 21)]
-        const int m = t & 127, py = m >> 4, px = m & 15;
-        const uint32_t* base = sIn + (2 * py) * SS_IN_LD + 6 * px;
-        if (t < 128) { stem_build_half<0, 0>(base, sA, m); stem_build_half<0, 1>(base, sA, m); stem_build_half<0, 2>(base, sA, m); }
-        else { stem_build_half<1, 0>(base, sA, m); stem_build_half<1, 1>(base, sA, m); stem_build_half<1, 2>(base, sA, m); }
-    }
-    fence_proxy_async();            // generic-proxy writes -> visible to the tensor core (async proxy)
-    __syncthreads();
-    mbar_wait(bar_b, 0);
 
-    const int g = warp >> 2;
-    constexpr int NACC = SPLIT ? 2 : 1;
-    float acc[NACC][32];
-#pragma unroll
-    for (int a = 0; a < NACC; ++a)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[a][i] = 0.f;
-    wg_fence();
-#pragma unroll
-    for (int kb = 0; kb < SS_KB; ++kb) {
-        const uint32_t a = smem_u32(sA + kb * TC_A_BYTES + g * (64 * 128)), b = smem_u32(sB + kb * NPL * SS_B_PLANE);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint64_t ah = wg_desc(a + 32 * k), bh = wg_desc(b + 32 * k);
-            if constexpr (SPLIT) {
-                wgmma<false, 64>(acc[1], wg_desc(a + SS_OFF_ALO + 32 * k), bh);
-                wgmma<false, 64>(acc[1], ah, wg_desc(b + SS_B_PLANE + 32 * k));
-            }
-            wgmma<false, 64>(acc[0], ah, bh);
-        }
-    }
-    wg_commit();
-    wg_wait<0>();
-#pragma unroll
-    for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
-
+    // this thread's pixel and patch half: element k = r*21 + s*3 + c of pixel (py, px) sits at sIn[2*py + r][6*px + (k % 21)]
+    const int m = t & 127, half = t >> 7;
+    const uint32_t* base = sIn + (2 * (m >> 5)) * ST_IN_LD + 6 * (m & 31);
+    // accumulator fragment: d[4j + 2h + e] = pixel rbase + 8h, channel 8j + cbase + e
     const int rbase = 64 * g + 16 * (warp & 3) + (lane >> 2), cbase = 2 * (lane & 3);
+    int buf = 0;
+    for (bool first = true; u < u_end; ++u, first = false) {
+        float acc[NACC][32];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int m = rbase + 8 * h;
-        const int oy = oy0 + (m >> 4), ox = ox0 + (m & 15);
-        if (oy >= p.Ho[img] || ox >= p.Wo[img]) continue;
-        __half* y = p.y + (p.out_pix[img] + (long long)oy * p.Wo[img] + ox) * 64;
+        for (int a = 0; a < NACC; ++a)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int n = 8 * j + cbase, i = 4 * j + 2 * h;
-            float v0 = SPLIT ? fmaf(acc[NACC - 1][i], 0.00048828125f, acc[0][i]) : acc[0][i];
-            float v1 = SPLIT ? fmaf(acc[NACC - 1][i + 1], 0.00048828125f, acc[0][i + 1]) : acc[0][i + 1];
-            if (p.bias) { v0 += __ldg(p.bias + n); v1 += __ldg(p.bias + n + 1); }
-            v0 = fmaxf(v0, 0.f);
-            v1 = fmaxf(v1, 0.f);
-            if constexpr (SPLIT) {
-                __half2 hi, lo;
-                split2(v0, v1, hi, lo);
-                *reinterpret_cast<__half2*>(y + n) = hi;
-                *reinterpret_cast<__half2*>(y + p.plane + n) = lo;
-            } else {
-                *reinterpret_cast<__half2*>(y + n) = pack_sat(v0, v1);
+            for (int i = 0; i < 32; ++i) acc[a][i] = 0.f;
+        stem_kblock<SPLIT, 0>(acc, base, sA, sB, m, half, g, bar_b, first);
+        stem_kblock<SPLIT, 1>(acc, base, sA, sB, m, half, g, bar_b, first);
+        stem_kblock<SPLIT, 2>(acc, base, sA, sB, m, half, g, bar_b, first);
+        const bool more = u + 1 < u_end;
+        Unit N = U;
+        if (more) {
+            N = decode(u + 1);
+            load_window(N);
+        }
+        wg_wait<0>();
+#pragma unroll
+        for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
+
+        const int img = U.img;
+        uint8_t* tile = sT + buf * ST_T_BYTES;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int mm = rbase + 8 * h;
+            const int oy = U.r0 + (mm >> 5), ox = U.c0 + (mm & 31);
+            __half* y = p.y + (p.out_pix[img] + (long long)oy * p.Wo[img] + ox) * 64;
+            const bool store = !p.pool && oy < p.Hs[img] && ox < p.Ws[img];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int n = 8 * j + cbase, i = 4 * j + 2 * h;
+                float v0 = SPLIT ? fmaf(acc[NACC - 1][i], 0.00048828125f, acc[0][i]) : acc[0][i];
+                float v1 = SPLIT ? fmaf(acc[NACC - 1][i + 1], 0.00048828125f, acc[0][i + 1]) : acc[0][i + 1];
+                if (p.bias) { v0 += __ldg(p.bias + n); v1 += __ldg(p.bias + n + 1); }
+                v0 = fmaxf(v0, 0.f);
+                v1 = fmaxf(v1, 0.f);
+                if constexpr (SPLIT) {
+                    __half2 hi, lo;
+                    split2(v0, v1, hi, lo);
+                    if (p.pool) {                   // rebuilt as the max-pool of a split tensor reads it
+                        const float2 fh = __half22float2(hi), fl = __half22float2(lo);
+                        *reinterpret_cast<float2*>(tile + mm * PIX_BYTES + (((n >> 2) ^ (mm & 7)) << 4) + (n & 3) * 4) =
+                            make_float2(fmaf(fl.x, 0.00048828125f, fh.x), fmaf(fl.y, 0.00048828125f, fh.y));
+                    } else if (store) {
+                        *reinterpret_cast<__half2*>(y + n) = hi;
+                        *reinterpret_cast<__half2*>(y + p.plane + n) = lo;
+                    }
+                } else {
+                    if (p.pool) *reinterpret_cast<__half2*>(tile + mm * PIX_BYTES + ((j ^ (mm & 7)) << 4) + cbase * 2) = pack_sat(v0, v1);
+                    else if (store) *reinterpret_cast<__half2*>(y + n) = pack_sat(v0, v1);
+                }
             }
         }
+        if (more) stage_window();
+        __syncthreads();
+
+        if (p.pool && u >= u_begin && t < ST_PH * ST_PW * 8) {
+            // pooled pixel (oy, ox), channels 8 oct .. 8 oct + 7: stem rows 2 oy - 1 .. 2 oy + 1 are tile rows 2 pr - 1 .. 2 pr + 1
+            // (row -1: the previous step's last row, in the other tile), stem columns 2 ox - 1 .. 2 ox + 1 are tile columns 2 pc ..
+            const int oct = t & 7, q = t >> 3, pr = q / ST_PW, pc = q - pr * ST_PW;
+            const int oy = U.j * ST_PH + pr, ox = U.strip * ST_PW + pc;
+            if (oy < p.Ho[img] && ox < p.Wo[img]) {
+                float mx[8];
+#pragma unroll
+                for (int e = 0; e < 8; ++e) mx[e] = -INFINITY;
+                const __half2 ninf = __float2half2_rn(-INFINITY);
+                __half2 mh[4] = {ninf, ninf, ninf, ninf};
+#pragma unroll
+                for (int r = 0; r < 3; ++r) {
+                    const int tr = 2 * pr - 1 + r;
+                    if (U.r0 + tr < 0 || U.r0 + tr >= p.Hs[img]) continue;
+                    const uint8_t* trow = tr < 0 ? sT + (buf ^ 1) * ST_T_BYTES + 3 * 32 * PIX_BYTES : tile + tr * 32 * PIX_BYTES;
+#pragma unroll
+                    for (int s = 0; s < 3; ++s) {
+                        const int tc = 2 * pc + s;
+                        if (U.c0 + tc < 0 || U.c0 + tc >= p.Ws[img]) continue;
+                        const uint8_t* px = trow + tc * PIX_BYTES;
+                        if constexpr (SPLIT) {
+                            const float4 a = *reinterpret_cast<const float4*>(px + (((2 * oct) ^ (tc & 7)) << 4));
+                            const float4 b = *reinterpret_cast<const float4*>(px + (((2 * oct + 1) ^ (tc & 7)) << 4));
+                            mx[0] = fmaxf(mx[0], a.x); mx[1] = fmaxf(mx[1], a.y); mx[2] = fmaxf(mx[2], a.z); mx[3] = fmaxf(mx[3], a.w);
+                            mx[4] = fmaxf(mx[4], b.x); mx[5] = fmaxf(mx[5], b.y); mx[6] = fmaxf(mx[6], b.z); mx[7] = fmaxf(mx[7], b.w);
+                        } else {
+                            const uint4 v = *reinterpret_cast<const uint4*>(px + ((oct ^ (tc & 7)) << 4));
+                            const __half2* hv = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) mh[e] = __hmax2(mh[e], hv[e]);
+                        }
+                    }
+                }
+                __half* y = p.y + (p.out_pix[img] + (long long)oy * p.Wo[img] + ox) * 64 + oct * 8;
+                if constexpr (SPLIT) {
+                    split_store8(y, p.plane, mx);
+                } else {
+                    uint4 o;
+                    __half2* ho = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) ho[e] = mh[e];
+                    *reinterpret_cast<uint4*>(y) = o;
+                }
+            }
+        }
+        buf ^= 1;
+        U = N;
     }
 }
-
 
 // hi = x with the 13 low mantissa bits cleared (exactly representable in TF32), lo = x - hi (exact in fp32)
 __global__ void split_tf32_kernel(const float4* __restrict__ x, float4* __restrict__ hi, float4* __restrict__ lo, long long n4) {
@@ -787,7 +904,7 @@ static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cud
 }
 
 template <bool SPLIT>
-static int stem_impl(const float* x, int nimg, const int* hw_host, const void* w, const float* bias, void* y, void* stream) {
+static int stem_impl(const float* x, int nimg, const int* hw_host, const void* w, const float* bias, void* y, int pool, void* stream) {
     RF_REQUIRE(x != nullptr && w != nullptr && y != nullptr, "rf_stem7: null pointer");
     RF_REQUIRE(((uintptr_t)y % 16) == 0 && ((uintptr_t)w % 16) == 0, "rf_stem7: pointers must be 16-byte aligned");
     ImgSet set;
@@ -795,27 +912,34 @@ static int stem_impl(const float* x, int nimg, const int* hw_host, const void* w
     StemParams p;
     memset(&p, 0, sizeof(p));
     p.nimg = nimg;
-    int tiles = 0;
+    p.pool = pool ? 1 : 0;
+    int units = 0;
+    long long out = 0;
     for (int i = 0; i < nimg; ++i) {
-        p.tiles_x[i] = (set.Wo[i] + SS_TW - 1) / SS_TW;
-        p.tile_start[i] = tiles;
-        tiles += p.tiles_x[i] * ((set.Ho[i] + SS_TH - 1) / SS_TH);
-        p.H[i] = set.H[i]; p.W[i] = set.W[i]; p.Ho[i] = set.Ho[i]; p.Wo[i] = set.Wo[i];
+        const int Hs = set.Ho[i], Ws = set.Wo[i];
+        const int Ho = pool ? (Hs - 1) / 2 + 1 : Hs, Wo = pool ? (Ws - 1) / 2 + 1 : Ws;      // max-pool 3 / stride 2 / pad 1
+        const int strips = pool ? (Wo + ST_PW - 1) / ST_PW : (Ws + ST_TW - 1) / ST_TW;
+        p.steps[i] = pool ? (Ho + ST_PH - 1) / ST_PH : (Hs + ST_TH - 1) / ST_TH;
+        p.unit_start[i] = units;
+        units += strips * p.steps[i];
+        p.H[i] = set.H[i]; p.W[i] = set.W[i]; p.Hs[i] = Hs; p.Ws[i] = Ws; p.Ho[i] = Ho; p.Wo[i] = Wo;
         p.in_pix[i] = set.in_pix[i];
-        p.out_pix[i] = set.out_pix[i];
+        p.out_pix[i] = out;
+        out += (long long)Ho * Wo;
     }
-    for (int i = nimg; i <= RF_MAX_IMGS; ++i) p.tile_start[i] = tiles;
+    for (int i = nimg; i <= RF_MAX_IMGS; ++i) p.unit_start[i] = units;
     int rc = SPLIT ? get_map(&p.mapB, w, 192ull, 64ull, 2, 64, 64, 2, 1, 2) : get_map(&p.mapB, w, 192ull, 64ull, 0, 64, 64, 0, 1, 2);
     if (rc) return rc;
-    p.plane = set.out_pix[nimg] * 64;
+    p.plane = out * 64;
     p.x = x; p.bias = bias; p.y = static_cast<__half*>(y);
     static bool attr[64] = {false};
     const int dev = current_device();
     if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(stem7_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SS_SMEM));
+        RF_CUDA(cudaFuncSetAttribute(stem7_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM));
         attr[dev] = true;
     }
-    stem7_kernel<SPLIT><<<tiles, SS_THREADS, SS_SMEM, as_stream(stream)>>>(p);
+    const int grid = units < num_sms() ? units : num_sms();
+    stem7_kernel<SPLIT><<<grid, ST_THREADS, ST_SMEM, as_stream(stream)>>>(p);
     RF_LAUNCHED();
     return 0;
 }
@@ -882,13 +1006,13 @@ extern "C" int rf_conv1x1_dual_split(const void* x1, const void* x2, int nimg, c
     return conv_impl(set, p, w_split, as_stream(stream), K_SPLIT, false, &dual);
 }
 
-// fused ResNet-50 stem.  x fp32 [sum HW][3], bias fp32 [64]; engine 2: w_f16 [64][192] ((r, s, c) order, zero padded), y fp16
-// [sum HoWo][64]; engine 4: w_split [2][64][192], y split [2][sum HoWo][64]
-int rf_stem7_f16_impl(const float* x, int nimg, const int* hw_host, const void* w_f16, const float* bias, void* y_f16, void* stream) {
-    return stem_impl<false>(x, nimg, hw_host, w_f16, bias, y_f16, stream);
+// fused ResNet-50 stem (pool: and its 3x3 / stride 2 / pad 1 max-pool).  x fp32 [sum HW][3], bias fp32 [64]; engine 2: w_f16
+// [64][192] ((r, s, c) order, zero padded), y fp16 [sum HoWo][64]; engine 4: w_split [2][64][192], y split [2][sum HoWo][64]
+int rf_stem7_f16_impl(const float* x, int nimg, const int* hw_host, const void* w_f16, const float* bias, int pool, void* y_f16, void* stream) {
+    return stem_impl<false>(x, nimg, hw_host, w_f16, bias, y_f16, pool, stream);
 }
-int rf_stem7_split_impl(const float* x, int nimg, const int* hw_host, const void* w_split, const float* bias, void* y_split, void* stream) {
-    return stem_impl<true>(x, nimg, hw_host, w_split, bias, y_split, stream);
+int rf_stem7_split_impl(const float* x, int nimg, const int* hw_host, const void* w_split, const float* bias, int pool, void* y_split, void* stream) {
+    return stem_impl<true>(x, nimg, hw_host, w_split, bias, y_split, pool, stream);
 }
 
 size_t rf_corr_tc_workspace(int NA, int NB, int C) { return 2ull * ((size_t)NA + NB) * C * sizeof(float) + 1024; }

@@ -10,10 +10,10 @@ int rf_im2col_impl(const float* x, int nimg, const int* hw_host, int C, int k, i
 int rf_poolblur_impl(const float* x, int nimg, const int* hw_host, int C, int round_out, float* y, void* stream);
 int rf_im2col_f16_impl(const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, int Kpad, void* y_f16, void* stream);
 int rf_maxpool_f16_impl(const void* x_f16, int nimg, const int* hw_host, int C, int k, int stride, int pad, void* y_f16, void* stream);
-int rf_stem7_f16_impl(const float* x, int nimg, const int* hw_host, const void* w_f16, const float* bias, void* y_f16, void* stream);
+int rf_stem7_f16_impl(const float* x, int nimg, const int* hw_host, const void* w_f16, const float* bias, int pool, void* y_f16, void* stream);
 int rf_blur_f16_impl(const void* x_f16, int nimg, const int* hw_host, int C, int stride, void* y_f16, void* stream);
 int rf_poolblur_f16_impl(const void* x_f16, int nimg, const int* hw_host, int C, void* y_f16, void* stream);
-int rf_stem7_split_impl(const float* x, int nimg, const int* hw_host, const void* w_split, const float* bias, void* y_split, void* stream);
+int rf_stem7_split_impl(const float* x, int nimg, const int* hw_host, const void* w_split, const float* bias, int pool, void* y_split, void* stream);
 int rf_blur_split_impl(const void* x, int nimg, const int* hw_host, int C, int stride, void* y, void* stream);
 int rf_poolblur_split_impl(const void* x, int nimg, const int* hw_host, int C, void* y, void* stream);
 int rf_maxpool_split_impl(const void* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, void* y, void* stream);
@@ -37,7 +37,27 @@ extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int
         float* y = static_cast<float*>(slots[l.dst]);
         int rc = 0;
         int k = l.k, stride = l.stride, pad = l.pad;
-        if (engine == RF_ENGINE_SPLIT) {
+        if (l.op == RF_OP_STEM7) {
+            RF_REQUIRE(engine == RF_ENGINE_SPLIT || engine == RF_ENGINE_F16, "rf_run_layers: RF_OP_STEM7 needs engine 2 or 4");
+            RF_REQUIRE(l.src == L[0].src && l.Cin == 3 && l.Cout == 64 && k == 7 && stride == 2 && pad == 3 && l.relu,
+                       "rf_run_layers: RF_OP_STEM7 is the ResNet-50 stem on the fp32 input slot");
+            const bool pool = (l.flags & RF_LAYER_STEM_POOL) != 0;
+            const rf_layer_t* mp = pool && li + 1 < n ? &L[li + 1] : nullptr;
+            RF_REQUIRE(!pool || (mp != nullptr && mp->op == RF_OP_MAXPOOL && mp->src == l.dst && mp->Cin == 64 && mp->k == 3 && mp->stride == 2 &&
+                                 mp->pad == 1 && mp->dst >= 0 && mp->dst < RF_MAX_SLOTS && mp->dst != l.src),
+                       "rf_run_layers: RF_LAYER_STEM_POOL needs the next layer to be a 3x3 / stride 2 / pad 1 max-pool of the stem's output");
+            void* out = pool ? slots[mp->dst] : y;
+            rc = engine == RF_ENGINE_SPLIT ? rf_stem7_split_impl(x, nimg, shw, l.w_f16, l.bias, pool, out, stream)
+                                           : rf_stem7_f16_impl(x, nimg, shw, l.w_f16, l.bias, pool, out, stream);
+            if (rc) return rc;
+            if (pool) {         // the stem's own slot is never written: the pair's output is the max-pool's
+                for (int i = 0; i < nimg; ++i)
+                    for (int d = 0; d < 2; ++d) hw[mp->dst][2 * i + d] = ((shw[2 * i + d] - 1) / 2 + 1 - 1) / 2 + 1;
+                known[mp->dst] = true;
+                ++li;
+                continue;
+            }
+        } else if (engine == RF_ENGINE_SPLIT) {
             // split activations ([2][P][C] fp16): the fp32 input image may only feed the stem; RF_LAYER_OUT_F32 convs write fp32
             if (l.op == RF_OP_CONV) {
                 const float* res = l.res >= 0 ? static_cast<const float*>(slots[l.res]) : nullptr;
@@ -55,10 +75,6 @@ extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int
             } else if (l.op == RF_OP_POOLBLUR) {
                 k = 4; stride = 2; pad = 1;
                 rc = rf_poolblur_split_impl(x, nimg, shw, l.Cin, y, stream);
-            } else if (l.op == RF_OP_STEM7) {
-                RF_REQUIRE(l.src == L[0].src && l.Cin == 3 && l.Cout == 64 && k == 7 && stride == 2 && pad == 3 && l.relu,
-                           "rf_run_layers: RF_OP_STEM7 is the ResNet-50 stem on the fp32 input slot");
-                rc = rf_stem7_split_impl(x, nimg, shw, l.w_f16, l.bias, y, stream);
             } else if (l.op == RF_OP_IM2COL) {
                 RF_REQUIRE(l.src == L[0].src, "rf_run_layers (engine 4): im2col reads the fp32 input slot");
                 rc = rf_im2col_split_impl(x, nimg, shw, l.Cin, k, stride, pad, l.Cout, y, stream);
@@ -82,10 +98,6 @@ extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int
             } else if (l.op == RF_OP_POOLBLUR) {
                 k = 4; stride = 2; pad = 1;
                 rc = rf_poolblur_f16_impl(x, nimg, shw, l.Cin, y, stream);
-            } else if (l.op == RF_OP_STEM7) {
-                RF_REQUIRE(l.src == L[0].src && l.Cin == 3 && l.Cout == 64 && k == 7 && stride == 2 && pad == 3 && l.relu,
-                           "rf_run_layers: RF_OP_STEM7 is the ResNet-50 stem on the fp32 input slot");
-                rc = rf_stem7_f16_impl(x, nimg, shw, l.w_f16, l.bias, y, stream);
             } else if (l.op == RF_OP_IM2COL) {
                 RF_REQUIRE(l.src == L[0].src, "rf_run_layers (engine 2): im2col reads the fp32 input slot");
                 rc = rf_im2col_f16_impl(x, nimg, shw, l.Cin, k, stride, pad, l.Cout, y, stream);

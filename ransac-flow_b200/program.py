@@ -13,7 +13,7 @@ from ._lib import check, lib, need_cuda, stream
 
 RF_OP_CONV, RF_OP_MAXPOOL, RF_OP_BLUR, RF_OP_IM2COL, RF_OP_POOLBLUR, RF_OP_STEM7, RF_OP_CONV_DUAL = 0, 1, 2, 3, 4, 5, 6
 RF_MAX_SLOTS = 32
-RF_LAYER_OUT_F32, RF_LAYER_TF32 = 1, 2
+RF_LAYER_OUT_F32, RF_LAYER_TF32, RF_LAYER_STEM_POOL = 1, 2, 4
 
 
 class rf_layer_t(C.Structure):
@@ -145,6 +145,15 @@ class LayerProgram:
                 elif o[0] not in (RF_OP_IM2COL, RF_OP_STEM7):
                     assert esize[o[1]] == 2 and (o[2] < 0 or esize[o[2]] == 2), "fp16 layer fed by an fp32 tensor"
         elems = [sum(h * w for h, w in hws[t]) * self.chan[t] * esize[t] for t in range(n_t)]        # BYTES per tensor
+        # the stem and a 3x3 / stride 2 / pad 1 max-pool that is its only reader run as one kernel (engines 2 / 4): the stem's
+        # full-resolution output is never written, so it sizes no buffer (its layer keeps a nominal slot for the wiring)
+        stem_pool = set()
+        for i, o in enumerate(self.ops[:-1]):
+            q = self.ops[i + 1]
+            if (f16 or split) and o[0] == RF_OP_STEM7 and q[0] == RF_OP_MAXPOOL and q[1] == i + 1 and tuple(q[5:8]) == (3, 2, 1) \
+                    and last_use[i + 1] == i + 1:
+                stem_pool.add(i)
+                elems[i + 1] = 0
         # slot assignment: slot 0 = external input; others from a free list
         slot_of, free, slot_elems = {0: 0}, [], [0]
         layers = (rf_layer_t * len(self.ops))()
@@ -167,7 +176,7 @@ class LayerProgram:
             if fc is not None:
                 L.w, L.w_tc = fc.w.data_ptr(), fc.w_tc.data_ptr()
                 L.w_f16 = fc.w_f16.data_ptr() if f16 else (fc.w_split.data_ptr() if split else None)
-                L.flags = self.flags.get(i, 0) if (f16 or split) else 0
+                L.flags = (self.flags.get(i, 0) | (RF_LAYER_STEM_POOL if i in stem_pool else 0)) if (f16 or split) else 0
                 L.bias = fc.bias.data_ptr() if fc.bias is not None else None
             L.src2 = -1
             if i in self.dual:

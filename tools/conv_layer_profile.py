@@ -6,7 +6,9 @@
 One eager pair (bench.py's weights, synthdata pair 0, 480x640) records every layer program it runs and the input it runs
 on: the ResNet-50 trunk on the 8-image ragged batch (7 pyramid scales + the target), the FeatureExtractor, NetFlowCoarse and
 NetMatchability.  Each program is then warmed up and run N times under torch.profiler with CUDA activities; every op of a
-program is exactly one kernel launch, so the kernels zip with `program.ops` in launch order.
+program is exactly one kernel launch, except a stem fused with the max-pool after it (RF_LAYER_STEM_POOL): one kernel for the
+two ops, timed on the stem row, with the max-pool row marked fused and the pair's own floor (the image in, the pooled output
+out) printed beside it.  The kernels zip with `program.ops` in launch order.
 
 Per layer: kernel, shape, tiles x N tiles, K blocks (KI), median time, algorithmic GFLOP and the executed TFLOP/s (3 MMAs per
 MAC on the split engine), algorithmic HBM bytes and GB/s, and which data-sheet floor bounds the layer and what share of it
@@ -171,24 +173,37 @@ def record_programs():
     return [(names.get(k[0], "program%d" % i),) + seen[k] for i, k in enumerate(order)], (coarse, net)
 
 
+def fused_pools(prog, x, engine):
+    """Indices of the max-pool ops that run inside the stem kernel before them (the compiled program's RF_LAYER_STEM_POOL)."""
+    from ransac_flow_b200.program import RF_LAYER_STEM_POOL
+    key = (tuple(x.hw), str(x.data.device), int(engine) if int(engine) in (2, 4) else 0)
+    layers = prog._compiled[key]["layers"]
+    return {i + 1 for i in range(len(prog.ops)) if layers[i].flags & RF_LAYER_STEM_POOL}
+
+
 def kernel_times(prog, x, engine, reps):
-    """Median device time (us) and name of each op's kernel over ``reps`` runs of the program."""
+    """Median device time (us) and name of each op's kernel over ``reps`` runs of the program (None for a fused max-pool)."""
     import torch
     from torch.profiler import ProfilerActivity, profile
     for _ in range(3):
         prog.run(x, engine)
     torch.cuda.synchronize()
+    fused = fused_pools(prog, x, engine)
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _ in range(reps):
             prog.run(x, engine)
         torch.cuda.synchronize()
     ev = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and not e.name.startswith(("Memcpy", "Memset"))]
     ev.sort(key=lambda e: e.time_range.start)
-    n = len(prog.ops)
+    ops = [i for i in range(len(prog.ops)) if i not in fused]       # the op each kernel of a run belongs to
+    n = len(ops)
     if len(ev) != n * reps:
-        raise SystemExit("conv_layer_profile: %d kernels for %d runs of a %d-op program: %s" % (len(ev), reps, n, sorted({e.name for e in ev})))
-    times = [[ev[r * n + i].time_range.elapsed_us() for r in range(reps)] for i in range(n)]
-    return [statistics.median(t) for t in times], [ev[i].name for i in range(n)]
+        raise SystemExit("conv_layer_profile: %d kernels for %d runs of a %d-kernel program: %s" % (len(ev), reps, n, sorted({e.name for e in ev})))
+    med, names = [None] * len(prog.ops), ["(fused into op %d)" % (i - 1) for i in range(len(prog.ops))]
+    for k, i in enumerate(ops):
+        med[i] = statistics.median([ev[r * n + k].time_range.elapsed_us() for r in range(reps)])
+        names[i] = ev[k].name
+    return med, names
 
 
 def main():
@@ -211,12 +226,21 @@ def main():
         rows = layer_model(prog.ops, x.hw, getattr(prog, "dual", {}))
         for r, us, kn in zip(rows, med, knames):
             r["kernel"], r["us"] = kn, us
+            if us is None:                                         # a max-pool fused into the stem before it
+                r["fused"] = True
+                st = rows[r["index"] - 1]
+                nbytes = st["bytes"] - st["cout"] * sum(h * w for h, w in st["out_hw"]) * ACT_BYTES + r["cout"] * sum(h * w for h, w in r["out_hw"]) * ACT_BYTES
+                t_flop = MMAS_PER_MAC * st["gflop"] * 1e9 / (PEAK_TFLOPS * 1e12)
+                st["pair_bytes"] = nbytes
+                st["pair_floor_ms"] = 1e3 * max(t_flop, nbytes / (PEAK_GBS * 1e9))
+                st["pair_floor_share"] = st["pair_floor_ms"] * 1e3 / st["us"]
+                continue
             if "floor_ms" in r:
                 r["tflops_executed"] = MMAS_PER_MAC * r["gflop"] * 1e9 / (us * 1e-6) / 1e12
                 r["gbs"] = r["bytes"] / (us * 1e-6) / 1e9
                 r["floor_share"] = r["floor_ms"] * 1e3 / us
         report["programs"].append({"name": name, "images": [list(v) for v in x.hw], "layers": rows,
-                                   "total_us": sum(med), "conv_us": sum(r["us"] for r in convs(rows)),
+                                   "total_us": sum(t for t in med if t is not None), "conv_us": sum(r["us"] for r in convs(rows)),
                                    "conv_floor_us": sum(1e3 * r["floor_ms"] for r in convs(rows))})
     report["clocks"] = sampler.stop()
     print("%s, power limit %s, max SM clock %s; SM clock during the runs: median %s MHz (%s)" % (
@@ -231,6 +255,11 @@ def main():
                 print("%3d %-9s %5d %5d %2d %1d %3s %3d %6d x %2d %3d %9.1f %8.2f %8.1f %8.2f %7.0f %6s %5.0f%%" % (
                     r["index"], r["op"], r["cin"], r["cout"], r["k"], r["stride"], "yes" if r["residual"] else "", r["bn"], r["tiles"], r["ntiles"],
                     r["KI"], r["us"], r["gflop"], r["tflops_executed"], r["bytes"] / 1e6, r["gbs"], r["bound"], 100 * r["floor_share"]))
+            elif r.get("fused"):
+                st = P["layers"][r["index"] - 1]
+                print("%3d %-9s %5d %5d %2d %1d %3s %3s %11s %3s %9s   fused into #%d: the pair's floor %.1f us (%.2f MB), reached %.0f%%" % (
+                    r["index"], r["op"], r["cin"], r["cout"], r["k"], r["stride"], "", "", "", "", "-", st["index"], 1e3 * st["pair_floor_ms"],
+                    st["pair_bytes"] / 1e6, 100 * st["pair_floor_share"]))
             else:
                 print("%3d %-9s %5d %5d %2d %1d %3s %3s %11s %3s %9.1f   (%s)" % (r["index"], r["op"], r["cin"], r["cout"], r["k"], r["stride"], "", "", "", "",
                                                                                r["us"], r["kernel"][:40]))
