@@ -1,14 +1,15 @@
 // Tensor-core engine (sm_90a): implicit-GEMM convolutions and the correlation with its row / column arg-max, on wgmma.
 //
-// One kernel template.  An output tile is 128 pixels (correlation: 128 rows of featA) x BN channels (columns of featB); a CTA
-// has 288 threads:
+// One kernel template.  An output tile is 128 pixels (correlation: 128 rows of featA) x BN channels (columns of featB); the
+// pixels are a tw x (128 / tw) rectangle of one image, or for 1x1 / stride-1 layers 128 consecutive pixels of the batch (flat
+// tiles, see conv_impl).  A CTA has 288 threads:
 //   warp 8        : TMA producer.  A = box (channels, tw, th[, 2 planes]) of the NHWC image at the tap's offset (out-of-bounds
 //                   zero fill is the zero padding, the traversal stride is the convolution stride), B = box of the K-major
 //                   weight matrix; both 128-byte swizzled, completion counted on the stage's mbarrier.
 //   warpgroups 0-1: tile rows 0..63 / 64..127.  wgmma.mma_async from the stage's descriptors into register accumulators; one
 //                   wgmma group stays in flight while the stage before it is handed back to the producer.  The epilogue
 //                   works on the registers: bias, residual, ReLU, conversion, store (convolution) or arg-max keys (correlation).
-// Convolutions are persistent: tile t (pixel tiles fastest) runs on CTA t mod gridDim.x, and the ring runs on across tile
+// Convolutions are persistent: tile t (N tiles fastest) runs on CTA t mod gridDim.x, and the ring runs on across tile
 // boundaries, so one tile's epilogue overlaps the loads of the next.  fp16 and split outputs take one more ring stage per tile
 // (the epilogue slot): the producer TMA-loads the residual tile into it, the consumers add it and write the result back in
 // place, one thread TMA-stores the slot and hands it back once the store has read it.  fp32 outputs (rows of 49 or 1 floats
@@ -22,6 +23,7 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 
+#include <climits>
 #include <mutex>
 #include <unordered_map>
 
@@ -43,7 +45,7 @@ struct alignas(64) WgParams {
     CUtensorMap mapB;                     // weights (K, Cout[, 2]); correlation: B hi (C, NB)
     CUtensorMap mapBlo;                   // correlation: B lo
     int nimg;
-    int tiles, ntiles;                    // convolution: pixel tiles of the batch, and times the N tiles
+    int ntiles;                           // convolution: pixel tiles of the batch x N tiles
     int tile_start[RF_MAX_IMGS + 1];      // prefix sums of pixel tiles per image
     int tiles_x[RF_MAX_IMGS];
     int tw[RF_MAX_IMGS];                  // tile width (tile height = 128 / tw)
@@ -128,15 +130,17 @@ wg_kernel(const __grid_constant__ WgParams p) {
     const int kc = p.Cin / BK;
     const int KI = p.R * p.S * kc;
 
-    // ---- tiles.  Convolution: tile t -> pixel tile t % tiles, N tile t / tiles, on CTA t mod gridDim.x.  Correlation: one tile
-    // per CTA, column tiles fastest, so that the CTAs sharing a 128-row slab of featA run together ----
+    // ---- tiles.  Convolution: tile t -> N tile t % nt, pixel tile t / nt, on CTA t mod gridDim.x: the N tiles of a pixel tile run
+    // on neighbouring CTAs at the same time, so its A boxes come from HBM once and from L2 for the other N tiles.  Correlation: one
+    // tile per CTA, column tiles fastest, so that the CTAs sharing a 128-row slab of featA run together ----
     const int t_first = MODE == MODE_CORR ? 0 : (int)blockIdx.x;
     const int t_step = MODE == MODE_CORR ? 1 : (int)gridDim.x;
     const int t_end = MODE == MODE_CORR ? 1 : p.ntiles;
+    const int nt = (p.Cout + BN - 1) / BN;
     struct Tile { int img, tw, ox0, oy0, n0; };
     auto decode = [&](int t) {
-        const int mtile = MODE == MODE_CORR ? (int)blockIdx.y : t % p.tiles;
-        const int ntile = MODE == MODE_CORR ? (int)blockIdx.x : t / p.tiles;
+        const int mtile = MODE == MODE_CORR ? (int)blockIdx.y : t / nt;
+        const int ntile = MODE == MODE_CORR ? (int)blockIdx.x : t - mtile * nt;
         Tile T;
         T.img = 0;
 #pragma unroll
@@ -837,7 +841,21 @@ struct SplitDual { const void* x2; const int* hw2; int Cin2, stride2; };
 
 // kind K_TF32: x / residual / y fp32, w [Cout][K] fp32.  K_F16: fp16 x / residual / w, y fp16 (out32: fp32).  K_SPLIT: x / residual /
 // y split tensors ([2][P][C] fp16, planes P * C elements apart), w [2][Cout][K] fp16 (out32: y fp32 [P][Cout], no residual).
-static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cudaStream_t st, int kind, bool out32, const SplitDual* dual) {
+static int conv_impl(const ImgSet& batch, const ConvParams& cp, const void* w, cudaStream_t st, int kind, bool out32, const SplitDual* dual) {
+    // Flat tiles: the pixels of a 1x1 / stride-1 layer are independent rows of the batch's [sum HW][C] matrix (its second input's
+    // too, at stride2 = 1), so the batch runs as ONE image of 1 x sum(HW) pixels, in tiles of 128 consecutive pixels that run on
+    // across image boundaries.  Only the batch's last tile is partial; the tensor maps' bounds clip it.  3x3 and strided layers
+    // keep per-image tw x (128 / tw) tiles, the shape their halo and traversal stride need.
+    const bool flat = cp.R == 1 && cp.S == 1 && cp.stride == 1 && cp.pad == 0 && (dual == nullptr || dual->stride2 == 1);
+    int hw_flat[2] = {1, 0};
+    ImgSet flat_set;
+    if (flat) {
+        RF_REQUIRE(batch.out_pix[batch.n] <= INT_MAX, "rf_conv2d_nhwc: more than 2^31 - 1 pixels in one batch");
+        hw_flat[1] = (int)batch.out_pix[batch.n];
+        RF_REQUIRE(make_imgset(flat_set, 1, hw_flat, 1, 1, 0) == 0, "rf_conv2d_nhwc: bad image set");
+    }
+    const ImgSet& set = flat ? flat_set : batch;
+    const int* hw2 = dual == nullptr ? nullptr : flat ? hw_flat : dual->hw2;
     WgParams p;
     memset(&p, 0, sizeof(p));
     const bool split = kind == K_SPLIT;
@@ -848,7 +866,7 @@ static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cud
     const unsigned long long in_plane = (unsigned long long)set.in_pix[set.n] * cp.Cin * 2ull;
     long long in2_pix[RF_MAX_IMGS + 1] = {0};
     if (dual)
-        for (int i = 0; i < set.n; ++i) in2_pix[i + 1] = in2_pix[i] + (long long)dual->hw2[2 * i] * dual->hw2[2 * i + 1];
+        for (int i = 0; i < set.n; ++i) in2_pix[i + 1] = in2_pix[i] + (long long)hw2[2 * i] * hw2[2 * i + 1];
     const unsigned long long in2_plane = dual ? (unsigned long long)in2_pix[set.n] * dual->Cin2 * 2ull : 0ull;
     p.nimg = set.n;
     const bool tma_out = kind != K_TF32 && !out32;          // fp16 / split outputs: stored (and their residual loaded) by TMA
@@ -857,7 +875,7 @@ static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cud
     const char* rb = reinterpret_cast<const char*>(cp.residual);
     int tiles = 0;
     for (int i = 0; i < set.n; ++i) {
-        const int tw = pick_tw(set.Ho[i], set.Wo[i]), th = 128 / tw;
+        const int tw = flat ? 128 : pick_tw(set.Ho[i], set.Wo[i]), th = 128 / tw;
         p.tw[i] = tw;
         p.tiles_x[i] = (set.Wo[i] + tw - 1) / tw;
         p.tile_start[i] = tiles;
@@ -870,7 +888,7 @@ static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cud
                                  (unsigned long long)set.H[i], bk, (unsigned)tw, (unsigned)th, (unsigned)cp.stride, esz);
         if (!rc && dual)
             rc = get_map4(&p.mapA2[i], static_cast<const char*>(dual->x2) + in2_pix[i] * dual->Cin2 * 2, (unsigned long long)dual->Cin2,
-                          (unsigned long long)dual->hw2[2 * i + 1], (unsigned long long)dual->hw2[2 * i], 2, in2_plane, bk, (unsigned)tw,
+                          (unsigned long long)hw2[2 * i + 1], (unsigned long long)hw2[2 * i], 2, in2_plane, bk, (unsigned)tw,
                           (unsigned)th, 2, (unsigned)dual->stride2, 2);
         // output and residual maps: the image's own pixels and the layer's Cout channels, so that the bounds clip partial tiles
         const long long o = set.out_pix[i] * cp.Cout * 2;
@@ -896,7 +914,6 @@ static int conv_impl(const ImgSet& set, const ConvParams& cp, const void* w, cud
     if (dual) { p.Cin = cp.Cin + dual->Cin2; p.stride2 = dual->stride2; }      // the kernel's K axis: both inputs
     p.plane = (long long)set.out_pix[set.n] * cp.Cout;
     p.bias = cp.bias; p.residual = cp.residual; p.y = cp.y;
-    p.tiles = tiles;
     p.ntiles = tiles * ((cp.Cout + BN - 1) / BN);
     if (kind == K_TF32) return launch_conv<K_TF32, O_F32>(p, BN, st);
     if (kind == K_F16) return out32 ? launch_conv<K_F16, O_F32>(p, BN, st) : launch_conv<K_F16, O_F16>(p, BN, st);

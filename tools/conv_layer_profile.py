@@ -51,6 +51,14 @@ def pick_tw(Ho, Wo):
     return best
 
 
+def pixel_tiles(ohw, flat):
+    """Pixel tiles of wg_kernel on output images ``ohw`` (conv_impl in csrc/gemm_tc.cu): with ``flat`` (1x1 / stride-1 layers)
+    tiles of 128 consecutive pixels of the whole batch, otherwise tw x (128 / tw) rectangles inside each image."""
+    if flat:
+        return (sum(h * w for h, w in ohw) + 127) // 128
+    return sum(((w + pick_tw(h, w) - 1) // pick_tw(h, w)) * ((h + 128 // pick_tw(h, w) - 1) // (128 // pick_tw(h, w))) for h, w in ohw)
+
+
 def _out(hw, k, s, p):
     return [((h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1) for h, w in hw]
 
@@ -78,13 +86,15 @@ def layer_model(ops, hw, dual=None, out_f32=()):
             nbytes = (pin * cin * ACT_BYTES if op != OP_STEM7 else pin * 3 * 4) + pout * cout * ACT_BYTES
             if res is not None and res >= 0:
                 nbytes += pout * cout * ACT_BYTES
+            flat = op != OP_STEM7 and (k, s, p) == (1, 1, 0)
             if op == OP_CONV_DUAL:
                 src2, cin2, s2 = dual[i]
                 K += cin2
                 nbytes += sum(h * w for h, w in hws[src2]) * cin2 * ACT_BYTES
+                flat = flat and s2 == 1
             flop = 2.0 * pout * cout * K
             bn = 128 if cout > 64 else 64
-            tiles = sum(((w + pick_tw(h, w) - 1) // pick_tw(h, w)) * ((h + 128 // pick_tw(h, w) - 1) // (128 // pick_tw(h, w))) for h, w in ohw)
+            tiles = pixel_tiles(ohw, flat)
             t_flop = MMAS_PER_MAC * flop / (PEAK_TFLOPS * 1e12)
             t_byte = nbytes / (PEAK_GBS * 1e9)
             r.update(K=K, KI=(K // 64) if op != OP_STEM7 else 3, tiles=tiles, ntiles=(cout + bn - 1) // bn, bn=bn, residual=res is not None and res >= 0,
