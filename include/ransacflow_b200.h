@@ -162,6 +162,8 @@ int rf_conv1x1_dual_split(const void* x1, const void* x2, int nimg, const int* h
                              fp16 / split, 64 channels) without the im2col matrix; w_f16 = [64][192] ([2][64][192] for engine 4) in
                              (r, s, c) order, zero padded */
 #define RF_OP_CONV_DUAL 6  /* engine 4 only: rf_conv1x1_dual_split; src = x1 (Cin channels), src2 = x2 (Cin2 channels, stride2), w_f16 = [2][Cout][Cin + Cin2] */
+#define RF_OP_STEM3 7      /* engine 4 only: the first conv of segNet's deep stem (segNet/segModel.py:64,108) fused: 3x3 / stride 2 / pad 1 on the
+                             3-channel fp32 input slot + bias + ReLU -> split, 64 channels, exact fp32 FMA; w = [27][64] ((r, s, c) rows) */
 #define RF_MAX_SLOTS 32
 typedef struct rf_layer {
     int op;
@@ -173,6 +175,8 @@ typedef struct rf_layer {
     const void* w_f16;              /* engine 2: [Cout][k*k*Cin] fp16; engine 4: [2][Cout][k*k*Cin] fp16 hi / lo planes (NULL otherwise) */
     int flags;                      /* engines 2 / 4: RF_LAYER_* */
     int src2, Cin2, stride2;        /* RF_OP_CONV_DUAL: second input slot, its channels and sampling stride (ignored otherwise) */
+    int dil;                        /* RF_OP_CONV dilation: 0 or 1 = none; > 1 only for 3x3 / stride 1 layers on engine 4.  Output size
+                                       (h + 2 pad - dil (k - 1) - 1) / stride + 1; out-of-image taps read zeros */
 } rf_layer_t;
 #define RF_LAYER_OUT_F32 1          /* conv: fp16 operands, fp32 output (RF_ENGINE_F16_OUT32; engine 4: RF_ENGINE_SPLIT_OUT32) */
 #define RF_LAYER_TF32 2             /* conv: fp32 input and output on the TF32 engine (e.g. a 49-channel head after an OUT_F32 layer) */
@@ -226,6 +230,34 @@ int rf_preproc_u8(const uint8_t* img, long long npix, int normalize, float* out_
 int rf_resample_u8(const uint8_t* in, int in_h, int in_w, int channels, int horizontal,
                    const int* bounds, const int* kk, int ksize, int out_size, uint8_t* out, void* stream);
 int rf_lanczos_coeffs_host(int in_size, int out_size, int* bounds_host, int* kk_host, int kk_capacity, int* ksize_out);
+/* The same tables for PIL's BILINEAR filter (triangle, support 1): Image.resize(size, BILINEAR) through rf_resample_u8, the
+ * resize of segNet/segData.py:7-17,71 (called from :53-76 getImg). */
+int rf_bilinear_coeffs_host(int in_size, int out_size, int* bounds_host, int* kk_host, int kk_capacity, int* ksize_out);
+
+/* ------------------------------------------------------------------ segNet --
+ * The decoder of the ADE20K scene-parsing network (segNet/segModel.py:218-264 PPMDeepsup, inference) and the multi-scale vote of
+ * segNet/segEval.py:23-43 getSky, on engine-4 split tensors.  The encoder (segModel.py:156-216 ResnetDilated) is an
+ * rf_run_layers program with dilated 3x3 convolutions (rf_layer_t.dil).
+ *
+ * rf_adaptive_avgpool_split: nn.AdaptiveAvgPool2d(b) (segModel.py:227) of every image of the split batch x [2][sum HW][C] for every
+ * bin count bins_host[j], in one launch.  y_host[j] (device pointer) receives the split tensor [2][nimg * b * b][C] of the b x b maps,
+ * image after image.  Bin i of n rows spans [floor(i n / b), ceil((i + 1) n / b)): bins overlap or repeat when n < b.  C % 8 == 0,
+ * nbins <= 8. */
+int rf_adaptive_avgpool_split(const void* x, int nimg, const int* hw_host, int C, const int* bins_host, int nbins, void* const* y_host,
+                              void* stream);
+/* The input of PPMDeepsup.conv_last (segModel.py:249-256) in one pass: y [2][sum HW][C5 + nbins * Cb] split, channels [0, C5) a copy
+ * of conv5 [2][sum HW][C5], channel block j the bilinear (align_corners=False) upsampling of branch j (y_host[j] of
+ * rf_adaptive_avgpool_split after its 1x1 conv: [2][nimg * b_j * b_j][Cb]) to each image's size.  C5 % 8 == Cb % 8 == 0. */
+int rf_ppm_concat_split(const void* conv5, int nimg, const int* hw_host, int C5, void* const* branches_host, const int* bins_host, int nbins,
+                        int Cb, void* y, void* stream);
+/* segEval.py:28-43 for one image.  logits fp32 [sum h_j w_j][ncls] of the distinct scales (hw_host = their sizes; the output of
+ * conv_last's final 1x1 conv on RF_ENGINE_SPLIT_OUT32); order_host[k] (k < norder) = the scale each of the reference's passes used, with
+ * repeats.  Per pixel of the H x W output: bilinear (align_corners=False) upsampling of each pass's logits, softmax over the ncls
+ * classes, scores += p / 5 in pass order (segEval.py:36), arg-max with the lowest index on ties, mask_out[p] = (pred == segId) as
+ * float (1 - that when segFg).  class_out (int32 [H][W]) and scores_out (fp32 [H][W][ncls]) are nullable debug outputs.
+ * ncls <= 160, norder <= 8. */
+int rf_seg_vote(const float* logits, int nimg, const int* hw_host, int ncls, const int* order_host, int norder, int H, int W, int segId,
+                int segFg, float* mask_out, int* class_out, float* scores_out, void* stream);
 
 /* -------------------------------------------------------------------- warp --
  * kornia 0.1.4 HomographyWarper.warp_grid: H [N][9] -> grid [N][h][w][2] */

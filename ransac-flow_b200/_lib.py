@@ -45,6 +45,10 @@ SIGNATURES = {
     "rf_preproc_u8": (i32, [vp, i64, i32, vp, vp]),
     "rf_resample_u8": (i32, [vp, i32, i32, i32, i32, vp, vp, i32, i32, vp, vp]),
     "rf_lanczos_coeffs_host": (i32, [i32, i32, vp, vp, i32, vp]),
+    "rf_bilinear_coeffs_host": (i32, [i32, i32, vp, vp, i32, vp]),
+    "rf_adaptive_avgpool_split": (i32, [vp, i32, vp, i32, vp, i32, vp, vp]),
+    "rf_ppm_concat_split": (i32, [vp, i32, vp, i32, vp, vp, i32, i32, vp, vp]),
+    "rf_seg_vote": (i32, [vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp]),
     "rf_warp_grid": (i32, [vp, i32, i32, i32, vp, vp]),
     "rf_grid_sample": (i32, [vp, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp]),
     "rf_upsample_bilinear": (i32, [vp, i32, i32, i32, i32, i32, vp, vp]),

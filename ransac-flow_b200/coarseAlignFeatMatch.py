@@ -123,14 +123,18 @@ class _CoarseAlignBase:
     resize_mode = "min"
     sample_generator = None               # getCoarse_device's RANSAC samples: torch's default CUDA generator unless set
 
-    def _setup(self, nbScale, nbIter, tolerance, transform, minSize, scaleR, imageNet, segNet, resnet_state_dict, verbose):
+    def _setup(self, nbScale, nbIter, tolerance, transform, minSize, scaleR, imageNet, segNet, resnet_state_dict, verbose,
+               segId=1, segFg=True, segnet_state_dicts=None):
         if not torch.cuda.is_available():
             raise ops._lib.RFError("CoarseAlign needs a CUDA device: ransac_flow_b200 has no CPU path")
         self.nbIter = nbIter
         self.tolerance = tolerance
         self.net = ResNet50Conv4(_load_resnet50_state(imageNet, resnet_state_dict))
         if segNet:
-            raise NotImplementedError("segNet sky masking is out of scope (SURVEY.md section 2 #9); pass segNet=False")
+            from .segnet import SegNet, segnet_weights
+            # evaluation/evalHpatch/coarseAlignFeatMatch.py:63-64, evalYFCC/coarseAlignFeatMatch.py:65-66
+            enc, dec, sds = segnet_weights(segnet_state_dicts)
+            self.segNet = SegNet(enc, dec, segId, segFg, state_dicts=sds)
         if transform == "Affine":
             self.Transform = outil.Affine
             self.nbPoint = 3
@@ -270,7 +274,10 @@ class _CoarseAlignBase:
         return (MtTensor > 0.5).squeeze()
 
     def skyFromSeg(self, path):
-        raise NotImplementedError("segNet sky masking is out of scope (SURVEY.md section 2 #9)")
+        """evaluation/evalHpatch/coarseAlignFeatMatch.py:152-153: the segNet mask of the image at ``path`` (float32 H x W)."""
+        if getattr(self, "segNet", None) is None:
+            raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
+        return self.segNet.getSky(path)
 
 
 class CoarseAlignA(_CoarseAlignBase):
@@ -278,8 +285,9 @@ class CoarseAlignA(_CoarseAlignBase):
     resize_mode = "min"
 
     def __init__(self, nbScale, nbIter, tolerance, transform, minSize, segId=2, segFg=False, scaleR=2, imageNet=True,
-                 segNet=True, resnet_state_dict=None, verbose=True):
-        self._setup(nbScale, nbIter, tolerance, transform, minSize, scaleR, imageNet, segNet, resnet_state_dict, verbose)
+                 segNet=True, resnet_state_dict=None, verbose=True, segnet_state_dicts=None):
+        self._setup(nbScale, nbIter, tolerance, transform, minSize, scaleR, imageNet, segNet, resnet_state_dict, verbose,
+                    segId, segFg, segnet_state_dicts)
 
     def setPair(self, Is_org, It_org):
         with torch.no_grad():
@@ -428,10 +436,11 @@ class CoarseAlignB(CoarseAlignC):
     resize_mode = "min"
 
     def __init__(self, nbScale, nbIter, tolerance, transform, minSize, segId=1, segFg=True, use_cuda=True, imageNet=True,
-                 segNet=True, scaleR=2, resnet_state_dict=None, verbose=True):
+                 segNet=True, scaleR=2, resnet_state_dict=None, verbose=True, segnet_state_dicts=None):
         if not use_cuda:
             raise ops._lib.RFError("use_cuda=False: ransac_flow_b200 has no CPU path")
-        self._setup(nbScale, nbIter, tolerance, transform, minSize, scaleR, imageNet, segNet, resnet_state_dict, verbose)
+        self._setup(nbScale, nbIter, tolerance, transform, minSize, scaleR, imageNet, segNet, resnet_state_dict, verbose,
+                    segId, segFg, segnet_state_dicts)
 
 
 CoarseAlign = CoarseAlignA

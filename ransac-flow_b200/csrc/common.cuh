@@ -114,6 +114,7 @@ struct ConvParams {
     float* y;
     int Cin, Cout, R, S, stride, pad, relu;
     int round_out;           // 1: round the output to TF32 (nearest) so that the tensor-core consumer's truncation is exact
+    int dil;                 // tap spacing (1 = none; > 1 only on the split engine)
     long long Mtot;          // total output pixels
     int K;                   // R*S*Cin
 };

@@ -776,13 +776,16 @@ __device__ __forceinline__ void up_coord(int dst, int in_size, int out_size, int
     l1 = src - (float)i0;
     l0 = 1.f - l1;
 }
+// the four taps weighted in ATen's order (rows of the blend first)
+__device__ __forceinline__ float up_blend(float v00, float v01, float v10, float v11, float ly0, float ly1, float lx0, float lx1) {
+    return ly0 * (lx0 * v00 + lx1 * v01) + ly1 * (lx0 * v10 + lx1 * v11);
+}
 __device__ __forceinline__ float up_sample(const float* __restrict__ p, int h, int w, int H, int W, int Y, int X) {
     int y0, y1, x0, x1;
     float ly0, ly1, lx0, lx1;
     up_coord(Y, h, H, y0, y1, ly0, ly1);
     up_coord(X, w, W, x0, x1, lx0, lx1);
-    return ly0 * (lx0 * __ldg(p + y0 * w + x0) + lx1 * __ldg(p + y0 * w + x1)) +
-           ly1 * (lx0 * __ldg(p + y1 * w + x0) + lx1 * __ldg(p + y1 * w + x1));
+    return up_blend(__ldg(p + y0 * w + x0), __ldg(p + y0 * w + x1), __ldg(p + y1 * w + x0), __ldg(p + y1 * w + x1), ly0, ly1, lx0, lx1);
 }
 
 __global__ void upsample_kernel(const float* __restrict__ in, int NC, int h, int w, int H, int W, float* __restrict__ out) {
@@ -1243,6 +1246,283 @@ int rf_im2col_split_impl(const float* x, int nimg, const int* hw_host, int C, in
     return 0;
 }
 
+// segNet's deep-stem conv1 (segNet/segModel.py:64,108): 3x3 / stride 2 / pad 1 on the 3-channel fp32 image + folded BN + ReLU ->
+// split [2][sum HoWo][64].  27 multiply-adds per output: exact fp32 FMA, one thread per (output pixel, 8 channels); the weights
+// w [27][64] ((r, s, c) rows) are staged in shared memory.  No patch matrix goes to HBM.
+__global__ void __launch_bounds__(256) stem3_split_kernel(const __grid_constant__ ImgSet set, const float* __restrict__ x, const float* __restrict__ w,
+                                                          const float* __restrict__ bias, __half* __restrict__ y, long long plane) {
+    __shared__ float sw[27 * 64];
+    for (int i = threadIdx.x; i < 27 * 64; i += blockDim.x) sw[i] = __ldg(w + i);
+    __syncthreads();
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= set.out_pix[set.n] * 8) return;
+    const long long pix = t >> 3;
+    const int c0 = (int)(t & 7) * 8;
+    const int im = find_img(set, pix);
+    const int Wo = set.Wo[im], H = set.H[im], W = set.W[im];
+    const int rem = (int)(pix - set.out_pix[im]), oy = rem / Wo, ox = rem - oy * Wo;
+    float acc[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = bias ? __ldg(bias + c0 + e) : 0.f;
+    const float* src = x + set.in_pix[im] * 3;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        const int iy = 2 * oy - 1 + r;
+        if (iy < 0 || iy >= H) continue;
+#pragma unroll
+        for (int s = 0; s < 3; ++s) {
+            const int ix = 2 * ox - 1 + s;
+            if (ix < 0 || ix >= W) continue;
+            const float* p = src + ((long long)iy * W + ix) * 3;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float v = __ldg(p + c);
+                const float* wr = sw + ((r * 3 + s) * 3 + c) * 64 + c0;
+#pragma unroll
+                for (int e = 0; e < 8; ++e) acc[e] = fmaf(v, wr[e], acc[e]);
+            }
+        }
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] = fmaxf(acc[e], 0.f);
+    split_store8(y + pix * 64 + c0, plane, acc);
+}
+
+int rf_stem3_split_impl(const float* x, int nimg, const int* hw_host, const float* w, const float* bias, void* y, void* stream) {
+    RF_REQUIRE(x != nullptr && w != nullptr && y != nullptr && ((uintptr_t)y % 16) == 0, "rf_stem3 (engine 4): null or misaligned pointer");
+    ImgSet set;
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, 3, 2, 1) == 0, "rf_stem3: bad image set");
+    const long long total = set.out_pix[nimg] * 8;
+    stem3_split_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, x, w, bias, static_cast<__half*>(y), set.out_pix[nimg] * 64);
+    RF_LAUNCHED();
+    return 0;
+}
+
+// ---- segNet decoder and vote (segNet/segModel.py:218-264, segNet/segEval.py:23-43) on split tensors ----
+#define RF_SEG_MAX_BINS 8
+struct PoolBins {
+    int nbins, bins[RF_SEG_MAX_BINS];
+    long long work_start[RF_SEG_MAX_BINS + 1];   // prefix sums of nimg * b * b * C / 8 over the bin counts
+    __half* y[RF_SEG_MAX_BINS];
+};
+
+// nn.AdaptiveAvgPool2d(b): one thread per (bin count, image, output cell, 8 channels); sums in fp32 in row-major order, then / area
+__global__ void adaptive_avgpool_split_kernel(const __grid_constant__ ImgSet set, const __half* __restrict__ x, long long in_plane, int C,
+                                              const __grid_constant__ PoolBins pb) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= pb.work_start[pb.nbins]) return;
+    int j = 0;
+#pragma unroll
+    for (int q = 1; q < RF_SEG_MAX_BINS; ++q) j += (q < pb.nbins && t >= pb.work_start[q]) ? 1 : 0;
+    const int b = pb.bins[j], C8 = C / 8;
+    const long long r = t - pb.work_start[j];
+    const int c0 = (int)(r % C8) * 8;
+    const long long cell = r / C8;                 // image * b * b + oy * b + ox
+    const int im = (int)(cell / (b * b)), oyx = (int)(cell - (long long)im * b * b), oy = oyx / b, ox = oyx - oy * b;
+    const int H = set.H[im], W = set.W[im];
+    const int y0 = (oy * H) / b, y1 = ((oy + 1) * H + b - 1) / b, x0 = (ox * W) / b, x1 = ((ox + 1) * W + b - 1) / b;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    const __half* src = x + set.in_pix[im] * C + c0;
+    for (int yy = y0; yy < y1; ++yy)
+        for (int xx = x0; xx < x1; ++xx) {
+            float v[8];
+            split_load8(src + ((long long)yy * W + xx) * C, in_plane, v);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc[e] += v[e];
+        }
+    const float area = (float)((y1 - y0) * (x1 - x0));
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] /= area;
+    split_store8(pb.y[j] + cell * C + c0, (long long)set.n * b * b * C, acc);
+}
+
+extern "C" int rf_adaptive_avgpool_split(const void* x, int nimg, const int* hw_host, int C, const int* bins_host, int nbins, void* const* y_host,
+                                         void* stream) {
+    RF_REQUIRE(x != nullptr && bins_host != nullptr && y_host != nullptr && (C % 8) == 0 && C >= 8 && nbins >= 1 && nbins <= RF_SEG_MAX_BINS,
+               "rf_adaptive_avgpool_split: bad arguments (C % 8 == 0, 1 <= nbins <= 8)");
+    ImgSet set;
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, 1, 1, 0) == 0, "rf_adaptive_avgpool_split: bad image set");
+    PoolBins pb;
+    memset(&pb, 0, sizeof(pb));
+    pb.nbins = nbins;
+    for (int j = 0; j < nbins; ++j) {
+        RF_REQUIRE(bins_host[j] >= 1 && bins_host[j] <= 64 && y_host[j] != nullptr && ((uintptr_t)y_host[j] % 16) == 0,
+                   "rf_adaptive_avgpool_split: bin counts 1..64, 16-byte aligned outputs");
+        pb.bins[j] = bins_host[j];
+        pb.y[j] = static_cast<__half*>(y_host[j]);
+        pb.work_start[j + 1] = pb.work_start[j] + (long long)nimg * bins_host[j] * bins_host[j] * (C / 8);
+    }
+    for (int j = nbins; j < RF_SEG_MAX_BINS; ++j) pb.work_start[j + 1] = pb.work_start[nbins];
+    const long long total = pb.work_start[nbins];
+    adaptive_avgpool_split_kernel<<<blocks_for(total, 128), 128, 0, as_stream(stream)>>>(set, static_cast<const __half*>(x), set.in_pix[nimg] * C, C, pb);
+    RF_LAUNCHED();
+    return 0;
+}
+
+struct PpmBranches {
+    int nbins, bins[RF_SEG_MAX_BINS];
+    const __half* src[RF_SEG_MAX_BINS];
+};
+
+// [conv5 | up(branch 0) | ... ]: one thread per (pixel, 8 output channels)
+__global__ void ppm_concat_split_kernel(const __grid_constant__ ImgSet set, const __half* __restrict__ conv5, int C5, const __grid_constant__ PpmBranches br,
+                                       int Cb, __half* __restrict__ y, int Cy) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int Cy8 = Cy / 8;
+    const long long P = set.in_pix[set.n];
+    if (t >= P * Cy8) return;
+    const long long pix = t / Cy8;
+    const int c0 = (int)(t - pix * Cy8) * 8;
+    __half* dst = y + pix * Cy + c0;
+    const long long out_plane = P * Cy;
+    if (c0 < C5) {                                  // conv5: the hi / lo halves are copied as they are
+        const __half* s = conv5 + pix * C5 + c0;
+        *reinterpret_cast<uint4*>(dst) = __ldg(reinterpret_cast<const uint4*>(s));
+        *reinterpret_cast<uint4*>(dst + out_plane) = __ldg(reinterpret_cast<const uint4*>(s + P * C5));
+        return;
+    }
+    const int j = (c0 - C5) / Cb, cb = c0 - C5 - j * Cb, b = br.bins[j];
+    int im = 0;
+#pragma unroll
+    for (int q = 1; q < RF_MAX_IMGS; ++q) im += (q < set.n && pix >= set.in_pix[q]) ? 1 : 0;
+    const int H = set.H[im], W = set.W[im];
+    const int rem = (int)(pix - set.in_pix[im]), Y = rem / W, X = rem - Y * W;
+    int y0, y1, x0, x1;
+    float ly0, ly1, lx0, lx1;
+    up_coord(Y, b, H, y0, y1, ly0, ly1);
+    up_coord(X, b, W, x0, x1, lx0, lx1);
+    const __half* s = br.src[j] + ((long long)im * b * b) * Cb + cb;
+    const long long in_plane = (long long)set.n * b * b * Cb;
+    float v00[8], v01[8], v10[8], v11[8], o[8];
+    split_load8(s + (long long)(y0 * b + x0) * Cb, in_plane, v00);
+    split_load8(s + (long long)(y0 * b + x1) * Cb, in_plane, v01);
+    split_load8(s + (long long)(y1 * b + x0) * Cb, in_plane, v10);
+    split_load8(s + (long long)(y1 * b + x1) * Cb, in_plane, v11);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) o[e] = up_blend(v00[e], v01[e], v10[e], v11[e], ly0, ly1, lx0, lx1);
+    split_store8(dst, out_plane, o);
+}
+
+extern "C" int rf_ppm_concat_split(const void* conv5, int nimg, const int* hw_host, int C5, void* const* branches_host, const int* bins_host, int nbins,
+                                   int Cb, void* y, void* stream) {
+    RF_REQUIRE(conv5 != nullptr && y != nullptr && branches_host != nullptr && bins_host != nullptr && nbins >= 1 && nbins <= RF_SEG_MAX_BINS &&
+               (C5 % 8) == 0 && (Cb % 8) == 0 && C5 >= 8 && Cb >= 8, "rf_ppm_concat_split: bad arguments (C5 % 8 == Cb % 8 == 0, 1 <= nbins <= 8)");
+    RF_REQUIRE(((uintptr_t)conv5 % 16) == 0 && ((uintptr_t)y % 16) == 0, "rf_ppm_concat_split: pointers must be 16-byte aligned");
+    ImgSet set;
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, 1, 1, 0) == 0, "rf_ppm_concat_split: bad image set");
+    PpmBranches br;
+    memset(&br, 0, sizeof(br));
+    br.nbins = nbins;
+    for (int j = 0; j < nbins; ++j) {
+        RF_REQUIRE(bins_host[j] >= 1 && branches_host[j] != nullptr && ((uintptr_t)branches_host[j] % 16) == 0,
+                   "rf_ppm_concat_split: bin counts >= 1, 16-byte aligned branches");
+        br.bins[j] = bins_host[j];
+        br.src[j] = static_cast<const __half*>(branches_host[j]);
+    }
+    const int Cy = C5 + nbins * Cb;
+    const long long total = set.in_pix[nimg] * (Cy / 8);
+    ppm_concat_split_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, static_cast<const __half*>(conv5), C5, br, Cb,
+                                                                                   static_cast<__half*>(y), Cy);
+    RF_LAUNCHED();
+    return 0;
+}
+
+#define RF_SEG_MAX_CLS 160
+#define RF_SEG_MAX_PASSES 8
+#define RF_SEG_CPL (RF_SEG_MAX_CLS / 32)           // classes per lane
+struct VotePasses { int n, img[RF_SEG_MAX_PASSES]; };
+
+// one warp per output pixel; lane l holds classes l, l + 32, ...  Per pass: bilinear logits, softmax (max, sum of exp, divide),
+// scores += p / 5.  A pass that repeats the previous pass's scale reuses its probabilities (the same values the reference recomputes).
+__global__ void __launch_bounds__(256) seg_vote_kernel(const __grid_constant__ ImgSet set, const float* __restrict__ logits, int ncls,
+                                                       const __grid_constant__ VotePasses vp, int H, int W, int segId, int segFg,
+                                                       float* __restrict__ mask, int* __restrict__ cls_out, float* __restrict__ scores_out) {
+    const long long pix = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (pix >= (long long)H * W) return;
+    const int Y = (int)(pix / W), X = (int)(pix - (long long)Y * W);
+    float score[RF_SEG_CPL], p[RF_SEG_CPL];
+#pragma unroll
+    for (int q = 0; q < RF_SEG_CPL; ++q) score[q] = p[q] = 0.f;
+    int last = -1;
+    for (int k = 0; k < vp.n; ++k) {
+        const int im = vp.img[k];
+        if (im != last) {
+            last = im;
+            const int h = set.H[im], w = set.W[im];
+            int y0, y1, x0, x1;
+            float ly0, ly1, lx0, lx1;
+            up_coord(Y, h, H, y0, y1, ly0, ly1);
+            up_coord(X, w, W, x0, x1, lx0, lx1);
+            const float* base = logits + set.in_pix[im] * ncls;
+            const float *r00 = base + (long long)(y0 * w + x0) * ncls, *r01 = base + (long long)(y0 * w + x1) * ncls;
+            const float *r10 = base + (long long)(y1 * w + x0) * ncls, *r11 = base + (long long)(y1 * w + x1) * ncls;
+            float m = -INFINITY;
+#pragma unroll
+            for (int q = 0; q < RF_SEG_CPL; ++q) {
+                const int c = lane + 32 * q;
+                p[q] = c < ncls ? up_blend(__ldg(r00 + c), __ldg(r01 + c), __ldg(r10 + c), __ldg(r11 + c), ly0, ly1, lx0, lx1) : -INFINITY;
+                m = fmaxf(m, p[q]);
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+            float s = 0.f;
+#pragma unroll
+            for (int q = 0; q < RF_SEG_CPL; ++q) {
+                p[q] = lane + 32 * q < ncls ? expf(p[q] - m) : 0.f;
+                s += p[q];
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+#pragma unroll
+            for (int q = 0; q < RF_SEG_CPL; ++q) p[q] = __fdiv_rn(p[q], s);
+        }
+#pragma unroll
+        for (int q = 0; q < RF_SEG_CPL; ++q) score[q] = __fadd_rn(score[q], __fdiv_rn(p[q], 5.f));      // segEval.py:36: scores + pred / 5
+    }
+    // first arg-max: the lane's best (lowest class on ties), then the warp's (pack_key: larger value, then lower index)
+    unsigned long long best = 0ull;
+#pragma unroll
+    for (int q = 0; q < RF_SEG_CPL; ++q) {
+        const int c = lane + 32 * q;
+        if (c < ncls) {
+            const unsigned long long key = pack_key(score[q], (uint32_t)c);
+            best = key > best ? key : best;
+            if (scores_out) scores_out[pix * ncls + c] = score[q];
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
+        best = other > best ? other : best;
+    }
+    if (lane == 0) {
+        const int pred = (int)key_index(best);
+        const float hit = pred == segId ? 1.f : 0.f;
+        mask[pix] = segFg ? 1.f - hit : hit;
+        if (cls_out) cls_out[pix] = pred;
+    }
+}
+
+extern "C" int rf_seg_vote(const float* logits, int nimg, const int* hw_host, int ncls, const int* order_host, int norder, int H, int W, int segId,
+                           int segFg, float* mask_out, int* class_out, float* scores_out, void* stream) {
+    RF_REQUIRE(logits != nullptr && mask_out != nullptr && order_host != nullptr && ncls >= 1 && ncls <= RF_SEG_MAX_CLS && norder >= 1 &&
+               norder <= RF_SEG_MAX_PASSES && H >= 1 && W >= 1, "rf_seg_vote: bad arguments (1 <= ncls <= 160, 1 <= norder <= 8)");
+    ImgSet set;
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, 1, 1, 0) == 0, "rf_seg_vote: bad image set");
+    VotePasses vp;
+    memset(&vp, 0, sizeof(vp));
+    vp.n = norder;
+    for (int k = 0; k < norder; ++k) {
+        RF_REQUIRE(order_host[k] >= 0 && order_host[k] < nimg, "rf_seg_vote: pass order names an image outside the batch");
+        vp.img[k] = order_host[k];
+    }
+    const long long threads = (long long)H * W * 32;
+    seg_vote_kernel<<<blocks_for(threads, 256), 256, 0, as_stream(stream)>>>(set, logits, ncls, vp, H, W, segId, segFg, mask_out, class_out, scores_out);
+    RF_LAUNCHED();
+    return 0;
+}
+
 extern "C" int rf_l2norm_split_nhwc(const void* x_split, long long P, int C, const uint8_t* mask, float* y, void* y_hi, void* y_lo, void* stream) {
     RF_REQUIRE((C % 8) == 0 && P >= 0, "rf_l2norm_split_nhwc: C must be a multiple of 8");
     RF_REQUIRE(((uintptr_t)x_split % 16) == 0 && ((uintptr_t)y % 16) == 0 && ((uintptr_t)y_hi % 16) == 0 && ((uintptr_t)y_lo % 16) == 0,
@@ -1348,16 +1628,23 @@ static double rf_lanczos(double x) {
     if (-3.0 <= x && x < 3.0) return rf_sinc(x) * rf_sinc(x / 3);
     return 0.0;
 }
-extern "C" int rf_lanczos_coeffs_host(int in_size, int out_size, int* bounds_host, int* kk_host, int kk_capacity, int* ksize_out) {
-    RF_REQUIRE(in_size > 0 && out_size > 0, "rf_lanczos_coeffs_host: bad sizes");
+static double rf_triangle(double x) {                      // Pillow's bilinear_filter
+    if (x < 0.0) x = -x;
+    if (x < 1.0) return 1.0 - x;
+    return 0.0;
+}
+// precompute_coeffs + normalize_coeffs_8bpc for a filter of the given support (LANCZOS 3, BILINEAR 1)
+static int pil_coeffs_host(double (*filter)(double), double filter_support, int in_size, int out_size, int* bounds_host, int* kk_host,
+                           int kk_capacity, int* ksize_out) {
+    RF_REQUIRE(in_size > 0 && out_size > 0, "rf_*_coeffs_host: bad sizes");
     double scale, filterscale;
     filterscale = scale = (double)in_size / out_size;
     if (filterscale < 1.0) filterscale = 1.0;
-    double support = 3.0 * filterscale;
+    double support = filter_support * filterscale;
     int ksize = (int)ceil(support) * 2 + 1;
     *ksize_out = ksize;
     if (kk_host == nullptr) return 0;                      // size query
-    RF_REQUIRE((long long)ksize * out_size <= kk_capacity, "rf_lanczos_coeffs_host: kk buffer too small");
+    RF_REQUIRE((long long)ksize * out_size <= kk_capacity, "rf_*_coeffs_host: kk buffer too small");
     double* k = new double[ksize];
     for (int xx = 0; xx < out_size; xx++) {
         double center = 0 + (xx + 0.5) * scale;
@@ -1370,7 +1657,7 @@ extern "C" int rf_lanczos_coeffs_host(int in_size, int out_size, int* bounds_hos
         xmax -= xmin;
         int x;
         for (x = 0; x < xmax; x++) {
-            double w = rf_lanczos((x + xmin - center + 0.5) * ss);
+            double w = filter((x + xmin - center + 0.5) * ss);
             k[x] = w;
             ww += w;
         }
@@ -1386,6 +1673,12 @@ extern "C" int rf_lanczos_coeffs_host(int in_size, int out_size, int* bounds_hos
     }
     delete[] k;
     return 0;
+}
+extern "C" int rf_lanczos_coeffs_host(int in_size, int out_size, int* bounds_host, int* kk_host, int kk_capacity, int* ksize_out) {
+    return pil_coeffs_host(rf_lanczos, 3.0, in_size, out_size, bounds_host, kk_host, kk_capacity, ksize_out);
+}
+extern "C" int rf_bilinear_coeffs_host(int in_size, int out_size, int* bounds_host, int* kk_host, int kk_capacity, int* ksize_out) {
+    return pil_coeffs_host(rf_triangle, 1.0, in_size, out_size, bounds_host, kk_host, kk_capacity, ksize_out);
 }
 
 extern "C" int rf_warp_grid(const float* H, int N, int h, int w, float* grid_out, void* stream) {

@@ -467,6 +467,8 @@ size_t rf_corr_tc_workspace(int NA, int NB, int C);
 int rf_conv2d_tc(const ImgSet& set, const ConvParams& p, const void* w_tc, cudaStream_t st, bool f16, bool out32);
 bool rf_conv2d_tc_supported(const ConvParams& p);
 int rf_conv2d_split(const ImgSet& set, const ConvParams& p, const void* w_split, cudaStream_t st, bool out32);
+int rf_conv2d_nhwc_dil(const float* x, int nimg, const int* hw_host, int Cin, const float* w, const float* w_tc, const float* bias,
+                       const float* residual, int Cout, int R, int S, int stride, int pad, int dil, int relu, int engine, float* y, void* stream);
 
 static size_t keys_bytes(int NA, int NB) {
     return (((size_t)(NA > 0 ? NA : 0) + (size_t)(NB > 0 ? NB : 0)) * sizeof(unsigned long long) + 255) / 256 * 256;
@@ -536,12 +538,19 @@ extern "C" int rf_conv2d_nhwc(const float* x, int nimg, const int* hw_host, int 
                               const float* w, const float* w_tc, const float* bias, const float* residual,
                               int Cout, int R, int S, int stride, int pad, int relu, int engine,
                               float* y, void* stream) {
-    RF_REQUIRE(R == S && R >= 1 && stride >= 1 && pad >= 0 && Cin >= 1 && Cout >= 1, "rf_conv2d_nhwc: bad conv geometry");
+    return rf_conv2d_nhwc_dil(x, nimg, hw_host, Cin, w, w_tc, bias, residual, Cout, R, S, stride, pad, 1, relu, engine, y, stream);
+}
+
+// rf_conv2d_nhwc with a tap spacing `dil` (rf_layer_t.dil): the split engine's 3x3 / stride-1 convolutions only
+int rf_conv2d_nhwc_dil(const float* x, int nimg, const int* hw_host, int Cin, const float* w, const float* w_tc, const float* bias,
+                       const float* residual, int Cout, int R, int S, int stride, int pad, int dil, int relu, int engine, float* y, void* stream) {
+    RF_REQUIRE(R == S && R >= 1 && stride >= 1 && pad >= 0 && Cin >= 1 && Cout >= 1 && dil >= 1, "rf_conv2d_nhwc: bad conv geometry");
+    RF_REQUIRE(dil == 1 || engine == RF_ENGINE_SPLIT, "rf_conv2d_nhwc: dilation needs engine 4, a 3x3 kernel and stride 1");
     ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, R, stride, pad) == 0, "rf_conv2d_nhwc: bad image set");
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, dil * (R - 1) + 1, stride, pad) == 0, "rf_conv2d_nhwc: bad image set");
     ConvParams p;
     p.x = x; p.w = w; p.bias = bias; p.residual = residual; p.y = y;
-    p.Cin = Cin; p.Cout = Cout; p.R = R; p.S = S; p.stride = stride; p.pad = pad; p.relu = relu;
+    p.Cin = Cin; p.Cout = Cout; p.R = R; p.S = S; p.stride = stride; p.pad = pad; p.relu = relu; p.dil = dil;
     p.Mtot = set.out_pix[nimg];
     p.K = R * S * Cin;
     // tensor-core engine: ReLU'd activations are the next conv's MMA operand; store them rounded to nearest TF32

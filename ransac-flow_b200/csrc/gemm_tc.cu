@@ -52,7 +52,8 @@ struct alignas(64) WgParams {
     int Ho[RF_MAX_IMGS], Wo[RF_MAX_IMGS];
     long long out_pix[RF_MAX_IMGS + 1];
     int R, S, pad, stride, Cin, Cout, relu, round_out;
-    int kc1, stride2;                     // dual-input 1x1: K blocks [0, kc1) come from mapA, the rest from mapA2 (sampled with stride2)
+    int dil;                              // tap spacing of a dilated 3x3 (1 otherwise)
+    int kc1, stride2;                    // dual-input 1x1: K blocks [0, kc1) come from mapA, the rest from mapA2 (sampled with stride2)
     long long plane;                      // split output / residual: elements from the hi to the lo plane
     const float* bias;
     const void* residual;
@@ -193,7 +194,8 @@ wg_kernel(const __grid_constant__ WgParams p) {
                     } else {
                         const int tap = it / kc, cc = it - tap * kc;
                         const int r = tap / p.S, s = tap - r * p.S;
-                        const int c0 = cc * BK, x = T.ox0 * p.stride + s - p.pad, y = T.oy0 * p.stride + r - p.pad;
+                        // dilated taps: boxes wholly or partly outside the image are zero-filled by TMA, which is the padding
+                        const int c0 = cc * BK, x = T.ox0 * p.stride + s * p.dil - p.pad, y = T.oy0 * p.stride + r * p.dil - p.pad;
                         const int kcol = tap * p.Cin + c0;
                         if constexpr (KIND == K_SPLIT) {       // one 4-D box brings [hi tile | lo tile]
                             if (cc < p.kc1) tma_load_4d(sa, &p.mapA[T.img], &full[st], c0, x, y, 0);
@@ -909,6 +911,7 @@ static int conv_impl(const ImgSet& batch, const ConvParams& cp, const void* w, c
                    : get_map(&p.mapB, w, (unsigned long long)cp.K, (unsigned long long)cp.Cout, 0, bk, (unsigned)BN, 0, 1, esz);
     if (rc) return rc;
     p.R = cp.R; p.S = cp.S; p.pad = cp.pad; p.stride = cp.stride; p.Cin = cp.Cin; p.Cout = cp.Cout; p.relu = cp.relu; p.round_out = cp.round_out;
+    p.dil = cp.dil;
     p.kc1 = cp.Cin / (int)bk;
     p.stride2 = 1;
     if (dual) { p.Cin = cp.Cin + dual->Cin2; p.stride2 = dual->stride2; }      // the kernel's K axis: both inputs
@@ -994,6 +997,7 @@ int rf_conv2d_split(const ImgSet& set, const ConvParams& cp, const void* w_split
     RF_REQUIRE(rf_conv2d_split_supported(cp), "rf_conv2d_nhwc: engine 4 needs stride 1 or 2, 1x1 or 3x3, Cin % 64 == 0");
     RF_REQUIRE(out32 || (cp.Cout % 8) == 0, "rf_conv2d_nhwc: engine 4 needs Cout % 8 == 0 for split outputs");
     RF_REQUIRE(!out32 || cp.residual == nullptr, "rf_conv2d_nhwc: engine 4 fp32 outputs take no residual");
+    RF_REQUIRE(cp.dil == 1 || (!out32 && cp.R == 3 && cp.stride == 1), "rf_conv2d_nhwc: dilation needs engine 4, a 3x3 kernel and stride 1");
     RF_REQUIRE(((uintptr_t)cp.x % 16) == 0 && ((uintptr_t)cp.y % 16) == 0 && ((uintptr_t)cp.residual % 16) == 0 && ((uintptr_t)w_split % 16) == 0,
                "rf_conv2d_nhwc: engine 4 needs 16-byte aligned pointers");
     return conv_impl(set, cp, w_split, st, K_SPLIT, out32, nullptr);
@@ -1017,6 +1021,7 @@ extern "C" int rf_conv1x1_dual_split(const void* x1, const void* x2, int nimg, c
     p.x = static_cast<const float*>(x1); p.w = nullptr; p.bias = bias; p.residual = nullptr; p.y = static_cast<float*>(y);
     p.Cin = Cin1; p.Cout = Cout; p.R = 1; p.S = 1; p.stride = 1; p.pad = 0; p.relu = relu;
     p.round_out = 0;
+    p.dil = 1;
     p.Mtot = set.out_pix[nimg];
     p.K = Cin1 + Cin2;
     SplitDual dual{x2, hw2_host, Cin2, stride2};

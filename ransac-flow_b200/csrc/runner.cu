@@ -19,6 +19,9 @@ int rf_poolblur_split_impl(const void* x, int nimg, const int* hw_host, int C, v
 int rf_maxpool_split_impl(const void* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, void* y, void* stream);
 int rf_im2col_split_impl(const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, int Kpad, void* y, void* stream);
 int rf_blur_downsample_impl(const float* x, int nimg, const int* hw_host, int C, int stride, int round_out, float* y, void* stream);
+int rf_stem3_split_impl(const float* x, int nimg, const int* hw_host, const float* w, const float* bias, void* y, void* stream);
+int rf_conv2d_nhwc_dil(const float* x, int nimg, const int* hw_host, int Cin, const float* w, const float* w_tc, const float* bias,
+                       const float* residual, int Cout, int R, int S, int stride, int pad, int dil, int relu, int engine, float* y, void* stream);
 
 extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int nimg, const int* hw_host, int engine, void* stream) {
     RF_REQUIRE(L != nullptr && n >= 1 && nimg >= 1 && nimg <= RF_MAX_IMGS, "rf_run_layers: bad arguments");
@@ -37,6 +40,9 @@ extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int
         float* y = static_cast<float*>(slots[l.dst]);
         int rc = 0;
         int k = l.k, stride = l.stride, pad = l.pad;
+        const int dil = l.dil > 1 ? l.dil : 1;
+        RF_REQUIRE(dil == 1 || (l.op == RF_OP_CONV && engine == RF_ENGINE_SPLIT && !(l.flags & RF_LAYER_OUT_F32) && k == 3 && stride == 1),
+                   "rf_run_layers: dilation is for RF_OP_CONV 3x3 / stride 1 layers with split outputs on engine 4");
         if (l.op == RF_OP_STEM7) {
             RF_REQUIRE(engine == RF_ENGINE_SPLIT || engine == RF_ENGINE_F16, "rf_run_layers: RF_OP_STEM7 needs engine 2 or 4");
             RF_REQUIRE(l.src == L[0].src && l.Cin == 3 && l.Cout == 64 && k == 7 && stride == 2 && pad == 3 && l.relu,
@@ -61,8 +67,8 @@ extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int
             // split activations ([2][P][C] fp16): the fp32 input image may only feed the stem; RF_LAYER_OUT_F32 convs write fp32
             if (l.op == RF_OP_CONV) {
                 const float* res = l.res >= 0 ? static_cast<const float*>(slots[l.res]) : nullptr;
-                rc = rf_conv2d_nhwc(x, nimg, shw, l.Cin, l.w, static_cast<const float*>(l.w_f16), l.bias, res, l.Cout, k, k, stride, pad, l.relu,
-                                    (l.flags & RF_LAYER_OUT_F32) ? RF_ENGINE_SPLIT_OUT32 : RF_ENGINE_SPLIT, y, stream);
+                rc = rf_conv2d_nhwc_dil(x, nimg, shw, l.Cin, l.w, static_cast<const float*>(l.w_f16), l.bias, res, l.Cout, k, k, stride, pad, dil,
+                                        l.relu, (l.flags & RF_LAYER_OUT_F32) ? RF_ENGINE_SPLIT_OUT32 : RF_ENGINE_SPLIT, y, stream);
             } else if (l.op == RF_OP_CONV_DUAL) {
                 RF_REQUIRE(l.src2 >= 0 && l.src2 < RF_MAX_SLOTS && known[l.src2] && l.dst != l.src2 && l.res < 0 && k == 1 && stride == 1 && pad == 0,
                            "rf_run_layers: RF_OP_CONV_DUAL needs a written second input slot, k = 1, stride 1, pad 0, no residual");
@@ -78,6 +84,10 @@ extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int
             } else if (l.op == RF_OP_IM2COL) {
                 RF_REQUIRE(l.src == L[0].src, "rf_run_layers (engine 4): im2col reads the fp32 input slot");
                 rc = rf_im2col_split_impl(x, nimg, shw, l.Cin, k, stride, pad, l.Cout, y, stream);
+            } else if (l.op == RF_OP_STEM3) {
+                RF_REQUIRE(l.src == L[0].src && l.Cin == 3 && l.Cout == 64 && k == 3 && stride == 2 && pad == 1 && l.relu,
+                           "rf_run_layers: RF_OP_STEM3 is segNet's 3x3 / stride 2 / pad 1, 3 -> 64 stem conv (+ ReLU) on the fp32 input slot");
+                rc = rf_stem3_split_impl(x, nimg, shw, l.w, l.bias, y, stream);
             } else {
                 return fail_msg("rf_run_layers: unknown op");
             }
@@ -122,8 +132,8 @@ extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int
         }
         if (rc) return rc;
         for (int i = 0; i < nimg; ++i) {
-            hw[l.dst][2 * i] = (shw[2 * i] + 2 * pad - k) / stride + 1;
-            hw[l.dst][2 * i + 1] = (shw[2 * i + 1] + 2 * pad - k) / stride + 1;
+            hw[l.dst][2 * i] = (shw[2 * i] + 2 * pad - dil * (k - 1) - 1) / stride + 1;
+            hw[l.dst][2 * i + 1] = (shw[2 * i + 1] + 2 * pad - dil * (k - 1) - 1) / stride + 1;
         }
         known[l.dst] = true;
     }

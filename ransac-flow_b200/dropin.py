@@ -41,15 +41,31 @@ def install(variant="A"):
     try:                                     # removed from SciPy >= 1.3 but still imported by the evaluation scripts
         import scipy.misc as misc
         if not hasattr(misc, "imresize"):
-            import numpy as np
-            import PIL.Image as Image
-
-            def imresize(arr, size, interp="bilinear"):
-                return np.asarray(Image.fromarray(np.asarray(arr)).resize((size[1], size[0]), Image.BILINEAR))
             misc.imresize = imresize
     except Exception:  # noqa: BLE001
         pass
     return mod
+
+
+def imresize(arr, size, interp="bilinear"):
+    """``scipy.misc.imresize`` of SciPy <= 1.2 for an (h, w) ``size``, the form the drivers use
+    (evaluation/evalHpatch/evaluation.py:180 ``imresize(It_bg, (h, w)) < 128``): an array that is not uint8 is first
+    byte-scaled to 0..255 like ``scipy.misc.bytescale`` ((x - min) * 255 / (max - min), span 1 when constant, + 0.5, truncated),
+    so a 0 / 1 float mask becomes 0 / 255; then a PIL resize to (w, h) with the chosen filter.  Returns uint8."""
+    import numpy as np
+    import PIL.Image as Image
+    a = np.asarray(arr)
+    if a.dtype != np.uint8:
+        cmin, cmax = a.min(), a.max()
+        cscale = cmax - cmin
+        if cscale == 0:
+            cscale = 1
+        scale = float(255 - 0) / cscale
+        a = ((a - cmin) * scale + 0).clip(0, 255) + 0.5
+        a = a.astype(np.uint8)
+    resample = {"nearest": Image.NEAREST, "lanczos": Image.LANCZOS, "bilinear": Image.BILINEAR, "bicubic": Image.BICUBIC,
+                "cubic": Image.BICUBIC}[interp]
+    return np.asarray(Image.fromarray(a).resize((int(size[1]), int(size[0])), resample))
 
 
 def select_engine(name=None):

@@ -412,35 +412,45 @@ def fill_nearest_matched(flow, matched, want_index=False):
     return (out, idx) if want_index else out
 
 
-# --------------------------------------------------------------------------- PIL LANCZOS on device
+# --------------------------------------------------------------------------- PIL LANCZOS / BILINEAR on device
 _coeff_cache = {}
 
 
-def lanczos_coeffs(in_size, out_size, device):
-    key = (in_size, out_size, str(device))
+def resample_coeffs(in_size, out_size, device, fn):
+    """PIL's 8bpc resampling tables (``fn``: rf_lanczos_coeffs_host or rf_bilinear_coeffs_host) as device tensors, cached."""
+    key = (in_size, out_size, str(device), fn)
     if key not in _coeff_cache:
         ks = C.c_int(0)
-        check(lib.rf_lanczos_coeffs_host(in_size, out_size, None, None, 0, C.byref(ks)))
+        check(getattr(lib, fn)(in_size, out_size, None, None, 0, C.byref(ks)))
         bounds = np.zeros(2 * out_size, dtype=np.int32)
         kk = np.zeros(ks.value * out_size, dtype=np.int32)
-        check(lib.rf_lanczos_coeffs_host(in_size, out_size, bounds.ctypes.data_as(C.c_void_p), kk.ctypes.data_as(C.c_void_p),
-                                         kk.size, C.byref(ks)))
+        check(getattr(lib, fn)(in_size, out_size, bounds.ctypes.data_as(C.c_void_p), kk.ctypes.data_as(C.c_void_p), kk.size, C.byref(ks)))
         _coeff_cache[key] = (torch.from_numpy(bounds).to(device), torch.from_numpy(kk).to(device), ks.value)
     return _coeff_cache[key]
 
 
 def resize_lanczos_u8(img, out_w, out_h):
     """PIL ``Image.resize((out_w, out_h), LANCZOS)`` on a uint8 [H, W, 3] CUDA tensor (bit-exact)."""
+    return _resize_u8(img, out_w, out_h, "rf_lanczos_coeffs_host")
+
+
+def resize_bilinear_u8(img, out_w, out_h):
+    """PIL ``Image.resize((out_w, out_h), BILINEAR)`` on a uint8 [H, W, 3] CUDA tensor (bit-exact)."""
+    return _resize_u8(img, out_w, out_h, "rf_bilinear_coeffs_host")
+
+
+def _resize_u8(img, out_w, out_h, fn):
+    """PIL's two-pass 8bpc resampling (horizontal, then vertical) with the tables ``fn`` builds."""
     need_cuda(img)
     H, W, ch = img.shape
     cur = img.contiguous()
     if out_w != W:
-        b, k, ks = lanczos_coeffs(W, out_w, img.device)
+        b, k, ks = resample_coeffs(W, out_w, img.device, fn)
         nxt = torch.empty((H, out_w, ch), device=img.device, dtype=torch.uint8)
         check(lib.rf_resample_u8(ptr(cur), H, W, ch, 1, ptr(b), ptr(k), ks, out_w, ptr(nxt), stream()))
         cur, W = nxt, out_w
     if out_h != H:
-        b, k, ks = lanczos_coeffs(H, out_h, img.device)
+        b, k, ks = resample_coeffs(H, out_h, img.device, fn)
         nxt = torch.empty((out_h, W, ch), device=img.device, dtype=torch.uint8)
         check(lib.rf_resample_u8(ptr(cur), H, W, ch, 0, ptr(b), ptr(k), ks, out_h, ptr(nxt), stream()))
         cur = nxt

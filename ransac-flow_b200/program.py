@@ -11,7 +11,7 @@ import torch
 
 from ._lib import check, lib, need_cuda, stream
 
-RF_OP_CONV, RF_OP_MAXPOOL, RF_OP_BLUR, RF_OP_IM2COL, RF_OP_POOLBLUR, RF_OP_STEM7, RF_OP_CONV_DUAL = 0, 1, 2, 3, 4, 5, 6
+RF_OP_CONV, RF_OP_MAXPOOL, RF_OP_BLUR, RF_OP_IM2COL, RF_OP_POOLBLUR, RF_OP_STEM7, RF_OP_CONV_DUAL, RF_OP_STEM3 = 0, 1, 2, 3, 4, 5, 6, 7
 RF_MAX_SLOTS = 32
 RF_LAYER_OUT_F32, RF_LAYER_TF32, RF_LAYER_STEM_POOL = 1, 2, 4
 
@@ -20,7 +20,7 @@ class rf_layer_t(C.Structure):
     _fields_ = [("op", C.c_int), ("src", C.c_int), ("dst", C.c_int), ("res", C.c_int),
                 ("Cin", C.c_int), ("Cout", C.c_int), ("k", C.c_int), ("stride", C.c_int), ("pad", C.c_int), ("relu", C.c_int),
                 ("w", C.c_void_p), ("w_tc", C.c_void_p), ("bias", C.c_void_p), ("w_f16", C.c_void_p), ("flags", C.c_int),
-                ("src2", C.c_int), ("Cin2", C.c_int), ("stride2", C.c_int)]
+                ("src2", C.c_int), ("Cin2", C.c_int), ("stride2", C.c_int), ("dil", C.c_int)]
 
 
 lib.rf_run_layers.restype = C.c_int
@@ -37,13 +37,19 @@ class LayerProgram:
         self._keep = []          # folded weights (keeps the device tensors alive)
         self.flags = {}          # op index -> RF_LAYER_* (fp16 engine only)
         self.dual = {}           # op index -> (second input tensor, its channels, its stride)   (RF_OP_CONV_DUAL, split engine only)
+        self.dil = {}            # op index -> dilation of a 3x3 / stride-1 conv (split engine only)
         self._compiled = {}
 
     # -- topology --------------------------------------------------------------------------------
-    def conv(self, src, fc, relu, res=None, out_f32=False, tf32=False):
+    def conv(self, src, fc, relu, res=None, out_f32=False, tf32=False, dil=1):
         """``out_f32`` / ``tf32`` only matter under the fp16 engine: the layer that hands fp32 to a TF32 layer, and that
-        TF32 layer (fp32 in and out; e.g. the 49- / 1-channel head outputs, which stay fp32)."""
+        TF32 layer (fp32 in and out; e.g. the 49- / 1-channel head outputs, which stay fp32).  ``dil`` > 1: a dilated 3x3 /
+        stride-1 convolution (split engine only)."""
         assert self.chan[src] == fc.cin, (self.chan[src], fc.cin)
+        if dil > 1:
+            assert fc.k == 3 and fc.stride == 1 and not (out_f32 or tf32), "dilation: 3x3 / stride 1 layers with split outputs"
+            self.split_only = True
+        self.dil[len(self.ops)] = int(dil)
         self.flags[len(self.ops)] = (RF_LAYER_OUT_F32 if out_f32 else 0) | (RF_LAYER_TF32 if tf32 else 0)
         self.ops.append((RF_OP_CONV, src, -1 if res is None else res, fc.cin, fc.cout, fc.k, fc.stride, fc.pad, int(relu), fc))
         self._keep.append(fc)
@@ -110,6 +116,18 @@ class LayerProgram:
         self.f16_only = True
         return len(self.chan) - 1
 
+    def stem3(self, src, weight, bn):
+        """Split engine only: segNet's deep-stem conv1 (3x3 / 2 / pad 1, 3 -> 64, BN, ReLU) in one exact-fp32 kernel that reads the
+        fp32 image and writes split rows (no patch matrix)."""
+        from .model import FoldedConv
+        assert tuple(weight.shape) == (64, 3, 3, 3) and self.chan[src] == 3
+        fc = FoldedConv(weight, bn, 2, pad=1, device=self.device or weight.device)
+        self.ops.append((RF_OP_STEM3, src, -1, 3, 64, 3, 2, 1, 1, fc))
+        self._keep.append(fc)
+        self.chan.append(64)
+        self.split_only = True
+        return len(self.chan) - 1
+
     def blur(self, src, stride):
         c = self.chan[src]
         self.ops.append((RF_OP_BLUR, src, -1, c, c, 3, stride, 1, 0, None))
@@ -129,9 +147,9 @@ class LayerProgram:
         last_use[n_t - 1] = len(self.ops)                       # the output outlives the program
         # pixel counts per tensor
         hws = [list(hw)]
-        for o in self.ops:
-            k, s, p = o[5], o[6], o[7]
-            hws.append([((h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1) for h, w in hws[o[1]]])
+        for i, o in enumerate(self.ops):
+            k, s, p, d = o[5], o[6], o[7], self.dil.get(i, 1)
+            hws.append([((h + 2 * p - d * (k - 1) - 1) // s + 1, (w + 2 * p - d * (k - 1) - 1) // s + 1) for h, w in hws[o[1]]])
         # element size per tensor: fp32 everywhere, except under the fp16 engine (fp32 only for the image an im2col
         # reads and around RF_LAYER_OUT_F32 / RF_LAYER_TF32 convs)
         esize = [4] * n_t          # engine 4: split tensors are 2 fp16 planes = 4 bytes per element, like the fp32 image / OUT_F32 outputs
@@ -179,6 +197,7 @@ class LayerProgram:
                 L.flags = (self.flags.get(i, 0) | (RF_LAYER_STEM_POOL if i in stem_pool else 0)) if (f16 or split) else 0
                 L.bias = fc.bias.data_ptr() if fc.bias is not None else None
             L.src2 = -1
+            L.dil = self.dil.get(i, 1)
             if i in self.dual:
                 L.src2, L.Cin2, L.stride2 = slot_of[self.dual[i][0]], self.dual[i][1], self.dual[i][2]
             for t in {o[1], o[2], self.dual[i][0] if i in self.dual else -1}:
@@ -189,7 +208,7 @@ class LayerProgram:
         out_slot = slot_of[n_t - 1]
         chw = (C.c_int * (2 * len(hw)))(*[v for p in hw for v in p])
         out_split = split and not (self.flags.get(len(self.ops) - 1, 0) & RF_LAYER_OUT_F32)
-        in_split = split and self.ops[0][0] not in (RF_OP_IM2COL, RF_OP_STEM7)
+        in_split = split and self.ops[0][0] not in (RF_OP_IM2COL, RF_OP_STEM7, RF_OP_STEM3)
         return dict(layers=layers, bufs=bufs, out_slot=out_slot, out_hw=hws[-1], out_elems=elems[-1], chw=chw, nslots=len(slot_elems),
                     out_dtype=torch.float16 if (esize[-1] == 2 or out_split) else torch.float32, out_split=out_split,
                     in_dtype=torch.float16 if (esize[0] == 2 or in_split) else torch.float32)
@@ -199,7 +218,7 @@ class LayerProgram:
         need_cuda(x.data)
         f16, split = int(engine) == 2, int(engine) == 4
         assert f16 or split or not getattr(self, "f16_only", False), "this program uses tensor-core-engine-only layers"
-        assert split or not getattr(self, "split_only", False), "this program uses split-engine-only layers (conv_dual)"
+        assert split or not getattr(self, "split_only", False), "this program uses split-engine-only layers (conv_dual, dilation)"
         key = (tuple(x.hw), str(x.data.device), int(engine) if (f16 or split) else 0)
         if key not in self._compiled:
             # compiled entries own the activation buffers; captured CUDA graphs hold raw pointers into them, so entries are

@@ -137,6 +137,77 @@ def tiny_resnet_like_state(seed=0, widths=(16, 8, 16, 32), randomize_bn=True):
     return sd
 
 
+SEGNET_LAYERS = (("layer1", 64, 3), ("layer2", 128, 4), ("layer3", 256, 6), ("layer4", 512, 3))
+
+
+def _bn_small(g, sd, p, c, gamma):
+    """An eval-mode BN drawn from the generator with its weights scaled by ``gamma``: a residual branch that adds a fraction of
+    its input's scale, so activations stay O(1..100) through 16 blocks (fp16 range) without calibrating on data."""
+    _bn(g, sd, p, c, True)
+    sd[p + ".weight"] = sd[p + ".weight"] * gamma
+
+
+def _syncbn_extras(g, sd, p, c):
+    # SynchronizedBatchNorm2d checkpoints carry these too; the network never reads them
+    sd[p + "._tmp_running_mean"] = torch.randn(c, generator=g)
+    sd[p + "._tmp_running_var"] = torch.rand(c, generator=g)
+    sd[p + "._running_iter"] = torch.ones(1)
+
+
+def segnet_encoder_state(seed=0):
+    """state_dict of segNet's ResnetDilated(resnet50) (segNet/segModel.py:59-216; key names of the ADE20K encoder checkpoint)."""
+    g = torch.Generator().manual_seed(seed + 3000)
+    sd = {}
+    for i, (cin, cout) in enumerate(((3, 64), (64, 64), (64, 128)), 1):
+        sd["conv%d.weight" % i] = _conv(g, cout, cin, 3)
+        _bn(g, sd, "bn%d" % i, cout, True)
+    _syncbn_extras(g, sd, "bn1", 64)
+    inpl = 128
+    for layer, planes, blocks in SEGNET_LAYERS:
+        for b in range(blocks):
+            p = "%s.%d" % (layer, b)
+            sd[p + ".conv1.weight"] = _conv(g, planes, inpl, 1)
+            _bn(g, sd, p + ".bn1", planes, True)
+            sd[p + ".conv2.weight"] = _conv(g, planes, planes, 3)
+            _bn(g, sd, p + ".bn2", planes, True)
+            sd[p + ".conv3.weight"] = _conv(g, planes * 4, planes, 1)
+            _bn_small(g, sd, p + ".bn3", planes * 4, 0.25)
+            if b == 0:
+                sd[p + ".downsample.0.weight"] = _conv(g, planes * 4, inpl, 1, std=math.sqrt(1.0 / inpl))
+                _bn(g, sd, p + ".downsample.1", planes * 4, True)
+            inpl = planes * 4
+    return sd
+
+
+def segnet_decoder_state(seed=0, class_bias=(3.5, 3.0)):
+    """state_dict of segNet's PPMDeepsup(150 classes, fc_dim 2048) (segNet/segModel.py:218-243; key names of the ADE20K decoder
+    checkpoint, deep-supervision weights included).  ``class_bias`` = the bias of classes 1 (building) and 2 (sky): they dominate
+    the other classes, and which of the two wins varies over the image."""
+    g = torch.Generator().manual_seed(seed + 4000)
+    sd = {}
+    for j in range(4):
+        sd["ppm.%d.1.weight" % j] = _conv(g, 512, 2048, 1, std=math.sqrt(1.0 / 2048))
+        _bn(g, sd, "ppm.%d.2" % j, 512, True)
+    sd["cbr_deepsup.0.weight"] = _conv(g, 512, 1024, 3)
+    _bn(g, sd, "cbr_deepsup.1", 512, True)
+    sd["conv_last.0.weight"] = _conv(g, 512, 4096, 3, std=math.sqrt(1.0 / (9 * 4096)))
+    _bn(g, sd, "conv_last.1", 512, True)
+    _syncbn_extras(g, sd, "conv_last.1", 512)
+    sd["conv_last.4.weight"] = _conv(g, 150, 512, 1, std=math.sqrt(1.0 / 512))
+    bias = torch.randn(150, generator=g) * 0.1
+    bias[1], bias[2] = class_bias
+    sd["conv_last.4.bias"] = bias
+    sd["conv_last_deepsup.weight"] = _conv(g, 150, 512, 1)
+    sd["conv_last_deepsup.bias"] = torch.zeros(150)
+    return sd
+
+
+def segnet_image(seed, h, w):
+    """A seeded uint8 [h, w, 3] test image for segNet (a smooth texture: region structure, not noise)."""
+    rs = np.random.RandomState(5000 + seed)
+    return np.clip(_texture(rs, h, w) + rs.normal(0, 4, (h, w, 3)), 0, 255).astype(np.uint8)
+
+
 # --------------------------------------------------------------------------
 # image pairs (SURVEY.md section 8d)
 # --------------------------------------------------------------------------
