@@ -570,6 +570,8 @@ int rf_conv2d_nhwc_dil(const float* x, int nimg, const int* hw_host, int Cin, co
     // (3-channel stems, stride-2 convs, 49-channel heads) run on the exact-fp32 SIMT engine below
     if (engine == 1 && w_tc != nullptr && rf_conv2d_tc_supported(p)) return rf_conv2d_tc(set, p, w_tc, st, false, false);
     RF_REQUIRE(((uintptr_t)x % 16) == 0 && ((uintptr_t)w % 16) == 0 && ((uintptr_t)y % 16) == 0, "rf_conv2d_nhwc: pointers must be 16-byte aligned");
+    // the epilogue reads bias + n and residual + o as float4 whenever Cout % 4 == 0
+    RF_REQUIRE(((uintptr_t)bias % 16) == 0 && ((uintptr_t)residual % 16) == 0, "rf_conv2d_nhwc: bias and residual must be 16-byte aligned");
     const bool vec = (Cin % 16) == 0;
     const bool wide = Cout >= 128;
     unsigned gx = (unsigned)((p.Mtot + BM - 1) / BM);

@@ -89,6 +89,8 @@ def conv2d(x, w_packed, bias, Cout, k, stride, pad, relu, residual=None, engine=
     """conv + folded-BN bias (+ residual) (+ ReLU) on a ragged NHWC batch."""
     need_cuda(x.data, w_packed, bias, residual.data if residual is not None else None)
     ohw = _out_hw(x.hw, k, stride, pad)
+    if residual is not None:           # the kernels read the residual at the output's pixel and channel offsets
+        assert residual.hw == ohw and residual.C == Cout, (residual.hw, residual.C, ohw, Cout)
     if int(engine) == ENGINE_F16:      # x, residual, w_tc fp16 -> y fp16
         assert x.data.dtype == torch.float16 and w_tc is not None and w_tc.dtype == torch.float16
         assert residual is None or residual.data.dtype == torch.float16

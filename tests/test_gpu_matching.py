@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 import torch
 
+import fma_ref as FR
 from conftest import golden
 from oracle import outil_oracle as OO
 
@@ -26,6 +27,13 @@ def ambiguous(score, tol=2e-6):
     s = np.sort(score, axis=0)
     cols = (s[-1] - s[-2]) < tol if score.shape[0] > 1 else np.zeros(score.shape[1], bool)
     return rows, cols
+
+
+def check_exact(i1, i2, A, B):
+    """Precision 0 is exact: the pairs are those of the fp32 FMA-chain restatement (tests/fma_ref.py), bit for bit.  A, B:
+    (C, N) features as given to mutualMatching."""
+    _, _, r1, r2 = FR.corr_keys(torch.from_numpy(np.ascontiguousarray(A.T)).cuda(), torch.from_numpy(np.ascontiguousarray(B.T)).cuda())
+    assert np.array_equal(i1, r1) and np.array_equal(i2, r2), (len(i1), len(r1))
 
 
 def check_same(i1, i2, o1, o2, score):
@@ -60,6 +68,7 @@ def test_random_features(rf, C, NA, NB, seed):
     o1, o2, score = OO.mutualMatching(A, B, return_score=True)
     i1, i2 = gpu_match(rf, A, B)
     check_same(i1, i2, o1, o2, score)
+    check_exact(i1, i2, A, B)
     if NB > 2:
         assert 1 not in i2
     assert len(i1) >= n // 2
@@ -74,6 +83,7 @@ def test_negative_scores_and_ties(rf):
     o1, o2, score = OO.mutualMatching(A, B, return_score=True)
     i1, i2 = gpu_match(rf, A, B)
     check_same(i1, i2, o1, o2, score)
+    check_exact(i1, i2, A, B)
     # exact ties: first index wins on both sides (documented tie-break)
     A2 = np.zeros((4, 6), np.float32)
     A2[0] = 1

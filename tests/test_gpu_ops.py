@@ -1,5 +1,6 @@
-"""Kernel-level parity of the conv / pooling / warp kernels against torch-CPU fp32 (the library calls the
-reference makes) and the oracle's restatements."""
+"""Kernel-level parity of the pooling / correlation / warp kernels against torch-CPU fp32 (the library calls the
+reference makes) and the oracle's restatements.  The exact-FMA convolution is held bit for bit to its FMA chains in
+tests/test_gpu_simt_exact.py."""
 import numpy as np
 import PIL.Image as Image
 import pytest
@@ -23,30 +24,6 @@ def close(a, b, tol):
     a, b = np.asarray(a), np.asarray(b)
     scale = max(1.0, float(np.abs(b).max()))
     assert np.abs(a - b).max() <= tol * scale, (np.abs(a - b).max(), scale)
-
-
-@pytest.mark.parametrize("cin,cout,k,stride,pad,sizes", [
-    (3, 64, 3, 1, 1, [(20, 28)]), (3, 64, 7, 2, 3, [(32, 48), (18, 22)]), (64, 64, 3, 1, 1, [(24, 32), (9, 7)]),
-    (64, 128, 3, 2, 1, [(24, 32)]), (64, 256, 1, 1, 0, [(13, 17), (6, 5), (1, 1)]), (256, 512, 1, 2, 0, [(14, 18)]),
-    (128, 128, 3, 1, 1, [(16, 16), (16, 16)]), (49, 512, 3, 1, 1, [(6, 8)]), (128, 49, 3, 1, 1, [(6, 8)]),
-    (128, 1, 3, 1, 1, [(6, 8), (6, 8)]), (1024, 256, 1, 1, 0, [(15, 20), (30, 40)]), (16, 20, 3, 1, 1, [(5, 5)])])
-@pytest.mark.parametrize("relu,res", [(True, False), (True, True), (False, False)])
-def test_conv2d_fp32(rf, cin, cout, k, stride, pad, sizes, relu, res):
-    g = torch.Generator().manual_seed(cin * 7 + cout + k)
-    xs = [torch.randn(1, cin, h, w, generator=g) for h, w in sizes]
-    w = torch.randn(cout, cin, k, k, generator=g) / np.sqrt(cin * k * k)
-    bias = torch.randn(cout, generator=g)
-    refs = [F.conv2d(x, w, bias, stride=stride, padding=pad) for x in xs]
-    rs = [torch.randn(r.shape, generator=g) for r in refs] if res else None
-    if res:
-        refs = [a + b for a, b in zip(refs, rs)]
-    if relu:
-        refs = [F.relu(r) for r in refs]
-    wp = w.permute(2, 3, 1, 0).reshape(k * k * cin, cout).contiguous().cuda()
-    y = rf.ops.conv2d(ragged(rf, xs), wp, bias.cuda(), cout, k, stride, pad, relu, ragged(rf, rs) if res else None, rf.ops.ENGINE_FP32)
-    for i, r in enumerate(refs):
-        assert tuple(y.image(i).shape) == tuple(r.shape)
-        close(y.image(i).cpu(), r, 2e-5)
 
 
 def test_corr_neigh_module_matches_oracle(rf):

@@ -3,8 +3,8 @@
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
+import fma_ref as FR
 import wgmma_ref as R
 from oracle import outil_oracle as OO
 from test_gpu_matching import check_same
@@ -66,14 +66,18 @@ def test_f16_engine_saturates_and_rejects_unsupported_shapes(rf):
 
 
 def test_tf32_engine_falls_back_to_fp32_kernels_for_unsupported_shapes(rf):
+    """A 3-channel 7x7 stem is not a TMA-able operand: engine 1 runs it on the exact-FMA SIMT kernel, whose output is the
+    fp32 FMA chain bit for bit (unrounded without ReLU, cvt.rna.tf32 of it with ReLU).  More shapes in
+    tests/test_gpu_simt_exact.py."""
     g = torch.Generator().manual_seed(0)
-    x = torch.randn(1, 3, 16, 16, generator=g)                       # 3-channel stem: not a TMA-able operand
+    x = torch.randn(1, 3, 16, 16, generator=g)
     w = torch.randn(64, 3, 7, 7, generator=g) / 12
-    ref = F.conv2d(x, w, stride=2, padding=3)
     wp = w.permute(2, 3, 1, 0).reshape(147, 64).contiguous().cuda()
     wtc = w.permute(0, 2, 3, 1).reshape(64, 147).contiguous().cuda()
-    y = rf.ops.conv2d(ragged(rf, [x]), wp, None, 64, 7, 2, 3, False, None, rf.ops.ENGINE_TF32, wtc)
-    assert (y.image(0).cpu() - ref).abs().max().item() < 2e-5        # exact-fp32 SIMT path
+    for relu in (False, True):
+        y = rf.ops.conv2d(ragged(rf, [x]), wp, None, 64, 7, 2, 3, relu, None, rf.ops.ENGINE_TF32, wtc)
+        ref = FR.conv_chain(x.cuda(), w.cuda(), None, None, 2, 3, relu, round_out=relu)
+        assert torch.equal(y.data.view(torch.int32), ref.view(torch.int32)), relu
 
 
 @pytest.mark.parametrize("C,NA,NB,seed", [(1024, 13065, 1200, 0), (1024, 2107, 300, 1), (64, 129, 127, 2), (256, 1, 1, 4),
