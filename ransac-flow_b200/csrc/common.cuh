@@ -59,6 +59,20 @@ __device__ __forceinline__ void split_store8(__half* p, long long plane, const f
 }
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
+// what the activation slots of a layer program (rf_run_layers) hold: fp32 (engine 0), fp32 with layer outputs rounded to TF32
+// for the tensor-core convolutions that read them (engine 1), fp16 (engine 2) or split fp16 hi / lo planes (engine 4)
+enum ActFormat { ACT_NONE = -1, ACT_F32, ACT_TF32, ACT_F16, ACT_SPLIT };
+// engines 3 and 5 are per-layer conv output modes (RF_LAYER_OUT_F32), not activation formats
+inline ActFormat act_format(int engine) {
+    switch (engine) {
+    case RF_ENGINE_FP32: return ACT_F32;
+    case RF_ENGINE_TF32: return ACT_TF32;
+    case RF_ENGINE_F16: return ACT_F16;
+    case RF_ENGINE_SPLIT: return ACT_SPLIT;
+    default: return ACT_NONE;
+    }
+}
+
 inline int current_device() {
     int dev = 0;
     cudaGetDevice(&dev);

@@ -11,114 +11,8 @@
 
 namespace rf {
 
-// ---------------------------------------------------------------------------
-// nn.MaxPool2d(k, stride, pad) on a ragged NHWC batch (model/model.py:71: k=2,s=1;
-// torchvision resnet: k=3,s=2,p=1).  One thread per (output pixel, channel quad).
-// ---------------------------------------------------------------------------
-__global__ void maxpool_kernel(const __grid_constant__ ImgSet set, const float* __restrict__ x, float* __restrict__ y,
-                               int C, int k, int stride, int pad) {
-    const int c4n = C >> 2;
-    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    long long total = set.out_pix[set.n] * c4n;
-    if (t >= total) return;
-    long long pm = t / c4n;
-    int c4 = (int)(t - pm * c4n);
-    int im = find_img(set, pm);
-    int local = (int)(pm - set.out_pix[im]);
-    int oy = local / set.Wo[im], ox = local - oy * set.Wo[im];
-    const int H = set.H[im], W = set.W[im];
-    float4 m = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
-    for (int r = 0; r < k; ++r) {
-        int iy = oy * stride - pad + r;
-        if (iy < 0 || iy >= H) continue;
-        for (int s = 0; s < k; ++s) {
-            int ix = ox * stride - pad + s;
-            if (ix < 0 || ix >= W) continue;
-            float4 v = __ldg(reinterpret_cast<const float4*>(x + (set.in_pix[im] + (long long)iy * W + ix) * C) + c4);
-            m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
-        }
-    }
-    reinterpret_cast<float4*>(y + pm * C)[c4] = m;
-}
-
-// fp16 variant (engine 2): one thread per (output pixel, 8 channels)
-__global__ void maxpool_f16_kernel(const __grid_constant__ ImgSet set, const __half* __restrict__ x, __half* __restrict__ y,
-                                   int C, int k, int stride, int pad) {
-    const int c8n = C >> 3;
-    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    long long total = set.out_pix[set.n] * c8n;
-    if (t >= total) return;
-    long long pm = t / c8n;
-    int c8 = (int)(t - pm * c8n);
-    int im = find_img(set, pm);
-    int local = (int)(pm - set.out_pix[im]);
-    int oy = local / set.Wo[im], ox = local - oy * set.Wo[im];
-    const int H = set.H[im], W = set.W[im];
-    const __half2 ninf = __float2half2_rn(-INFINITY);
-    __half2 m[4] = {ninf, ninf, ninf, ninf};
-    for (int r = 0; r < k; ++r) {
-        int iy = oy * stride - pad + r;
-        if (iy < 0 || iy >= H) continue;
-        for (int s = 0; s < k; ++s) {
-            int ix = ox * stride - pad + s;
-            if (ix < 0 || ix >= W) continue;
-            const uint4 v = __ldg(reinterpret_cast<const uint4*>(x + (set.in_pix[im] + (long long)iy * W + ix) * C) + c8);
-            const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) m[e] = __hmax2(m[e], h[e]);
-        }
-    }
-    uint4 o;
-    __half2* ho = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) ho[e] = m[e];
-    reinterpret_cast<uint4*>(y + pm * C)[c8] = o;
-}
-
-// ---------------------------------------------------------------------------
-// im2col for the few-channel stems (3 -> 64): row p of the output holds the k*k*C patch of output pixel p in
-// (r, s, c) order, zero padded to Kpad (a multiple of 32 floats = one 128-byte swizzle row), so that the stem
-// becomes a 1x1 convolution the tensor-core engine can read with TMA.  One thread per (pixel, patch element).
-// ---------------------------------------------------------------------------
-// grid: (ceil(Ho*Wo*Kpad/4 / 256), image); one thread per float4 of the output; 32-bit index math.
-template <int KC, int CC, int KPADC>      // compile-time (k, C, Kpad) for the two stems (0 = runtime values)
-__global__ void im2col_kernel(const __grid_constant__ ImgSet set, const float* __restrict__ x, float* __restrict__ y,
-                              int C_, int k_, int stride, int pad, int Kpad_, int round_out) {
-    const int C = CC ? CC : C_, k = KC ? KC : k_, Kpad = KPADC ? KPADC : Kpad_;
-    const int im = blockIdx.y;
-    const int q4 = Kpad >> 2;                                   // float4 per output row
-    const int Wo = set.Wo[im], H = set.H[im], W = set.W[im];
-    const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned total = (unsigned)(set.Ho[im] * Wo) * (unsigned)q4;
-    if (idx >= total) return;
-    const unsigned local = idx / (unsigned)q4;
-    const int e0 = (int)(idx - local * (unsigned)q4) * 4;
-    const int oy = (int)(local / (unsigned)Wo), ox = (int)(local - (unsigned)oy * (unsigned)Wo);
-    const int kkc = k * k * C, kc = k * C;
-    const float* src = x + set.in_pix[im] * C;
-    float v[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int e = e0 + j;
-        float t = 0.f;
-        if (e < kkc) {
-            const int r = e / kc, rem = e - r * kc;             // (r, s, c) order: rem = s*C + c is contiguous in the input row
-            const int iy = oy * stride - pad + r;
-            const int ixc = (ox * stride - pad) * C + rem;      // element offset inside the input row
-            if (iy >= 0 && iy < H && ixc >= 0 && ixc < W * C) t = __ldg(src + (long long)iy * W * C + ixc);
-            if (round_out) t = round_tf32(t);
-        }
-        v[j] = t;
-    }
-    reinterpret_cast<float4*>(y + (set.out_pix[im] + local) * Kpad)[e0 >> 2] = make_float4(v[0], v[1], v[2], v[3]);
-}
-
-// ---------------------------------------------------------------------------
-// model/downsample.py:12-46: ReflectionPad2d(1) + depthwise [1 2 1]x[1 2 1]/16, stride s
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ int reflect1(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
-
-// 16-byte vectors of the activation type: 4 floats or 8 halves; arithmetic is always fp32
+// 16-byte vectors of the activation type: 4 floats or 8 halves; arithmetic is always fp32.  The kernels of the layer ops
+// (max-pool, im2col, blur, pool + blur, L2 normalisation) are written once over Vec16<T>, T = float, __half or SplitH.
 template <typename T> struct Vec16;
 template <> struct Vec16<float> {
     typedef float elem;
@@ -170,6 +64,117 @@ template <> struct Vec16<SplitH> {
     static __device__ __forceinline__ void load(const __half* p, long long plane, float (&v)[8]) { split_load8(p, plane, v); }
     static __device__ __forceinline__ void store(__half* p, long long plane, const float (&v)[8], int) { split_store8(p, plane, v); }
 };
+
+// ---------------------------------------------------------------------------
+// nn.MaxPool2d(k, stride, pad) on a ragged NHWC batch (model/model.py:71: k=2,s=1; torchvision resnet: k=3,s=2,p=1).  One
+// thread per (output pixel, 16-byte vector).
+// ---------------------------------------------------------------------------
+// running maximum of 16-byte vectors, from -inf: fp32 values (split: rebuilt, and split again on the store) ...
+template <typename T> struct VecMax {
+    float m[Vec16<T>::N];
+    __device__ __forceinline__ VecMax() {
+#pragma unroll
+        for (int e = 0; e < Vec16<T>::N; ++e) m[e] = -INFINITY;
+    }
+    __device__ __forceinline__ void add(const typename Vec16<T>::elem* p, long long plane) {
+        float v[Vec16<T>::N];
+        Vec16<T>::load(p, plane, v);
+#pragma unroll
+        for (int e = 0; e < Vec16<T>::N; ++e) m[e] = fmaxf(m[e], v[e]);
+    }
+    __device__ __forceinline__ void store(typename Vec16<T>::elem* p, long long plane) const { Vec16<T>::store(p, plane, m, 0); }
+};
+// ... fp16: the packed halves with __hmax2 (half the registers of eight fp32 values)
+template <> struct VecMax<__half> {
+    __half2 m[4];
+    __device__ __forceinline__ VecMax() {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) m[e] = __float2half2_rn(-INFINITY);
+    }
+    __device__ __forceinline__ void add(const __half* p, long long) {
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(p));
+        const __half2* h = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) m[e] = __hmax2(m[e], h[e]);
+    }
+    __device__ __forceinline__ void store(__half* p, long long) const {
+        uint4 o;
+        __half2* h = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) h[e] = m[e];
+        *reinterpret_cast<uint4*>(p) = o;
+    }
+};
+
+template <typename T>
+__global__ void maxpool_kernel(const __grid_constant__ ImgSet set, const typename Vec16<T>::elem* __restrict__ x, typename Vec16<T>::elem* __restrict__ y,
+                               int C, int k, int stride, int pad, long long pin, long long pout) {
+    constexpr int VN = Vec16<T>::N;
+    const int cvn = C / VN;
+    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    long long total = set.out_pix[set.n] * cvn;
+    if (t >= total) return;
+    long long pm = t / cvn;
+    int cv = (int)(t - pm * cvn);
+    int im = find_img(set, pm);
+    int local = (int)(pm - set.out_pix[im]);
+    int oy = local / set.Wo[im], ox = local - oy * set.Wo[im];
+    const int H = set.H[im], W = set.W[im];
+    VecMax<T> m;
+    for (int r = 0; r < k; ++r) {
+        int iy = oy * stride - pad + r;
+        if (iy < 0 || iy >= H) continue;
+        for (int s = 0; s < k; ++s) {
+            int ix = ox * stride - pad + s;
+            if (ix < 0 || ix >= W) continue;
+            m.add(x + (set.in_pix[im] + (long long)iy * W + ix) * C + cv * VN, pin);
+        }
+    }
+    m.store(y + pm * C + cv * VN, pout);
+}
+
+// ---------------------------------------------------------------------------
+// im2col for the few-channel stems (3 -> 64): row p of the output holds the k*k*C patch of output pixel p in
+// (r, s, c) order, zero padded to Kpad (a multiple of 32 floats = one 128-byte swizzle row), so that the stem
+// becomes a 1x1 convolution the tensor-core engine can read with TMA.  One thread per (pixel, patch element).
+// ---------------------------------------------------------------------------
+// grid: (ceil(Ho*Wo*Kpad/4 / 256), image); one thread per float4 of the output; 32-bit index math.
+template <int KC, int CC, int KPADC>      // compile-time (k, C, Kpad) for the two stems (0 = runtime values)
+__global__ void im2col_kernel(const __grid_constant__ ImgSet set, const float* __restrict__ x, float* __restrict__ y,
+                              int C_, int k_, int stride, int pad, int Kpad_, int round_out) {
+    const int C = CC ? CC : C_, k = KC ? KC : k_, Kpad = KPADC ? KPADC : Kpad_;
+    const int im = blockIdx.y;
+    const int q4 = Kpad >> 2;                                   // float4 per output row
+    const int Wo = set.Wo[im], H = set.H[im], W = set.W[im];
+    const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned total = (unsigned)(set.Ho[im] * Wo) * (unsigned)q4;
+    if (idx >= total) return;
+    const unsigned local = idx / (unsigned)q4;
+    const int e0 = (int)(idx - local * (unsigned)q4) * 4;
+    const int oy = (int)(local / (unsigned)Wo), ox = (int)(local - (unsigned)oy * (unsigned)Wo);
+    const int kkc = k * k * C, kc = k * C;
+    const float* src = x + set.in_pix[im] * C;
+    float v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int e = e0 + j;
+        float t = 0.f;
+        if (e < kkc) {
+            const int r = e / kc, rem = e - r * kc;             // (r, s, c) order: rem = s*C + c is contiguous in the input row
+            const int iy = oy * stride - pad + r;
+            const int ixc = (ox * stride - pad) * C + rem;      // element offset inside the input row
+            if (iy >= 0 && iy < H && ixc >= 0 && ixc < W * C) t = __ldg(src + (long long)iy * W * C + ixc);
+            if (round_out) t = round_tf32(t);
+        }
+        v[j] = t;
+    }
+    reinterpret_cast<float4*>(y + (set.out_pix[im] + local) * Kpad)[e0 >> 2] = make_float4(v[0], v[1], v[2], v[3]);
+}
+
+// ---------------------------------------------------------------------------
+// model/downsample.py:12-46: ReflectionPad2d(1) + depthwise [1 2 1]x[1 2 1]/16, stride s
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ int reflect1(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 
 template <typename T>
 __global__ void blur_kernel(const __grid_constant__ ImgSet set, const typename Vec16<T>::elem* __restrict__ x, typename Vec16<T>::elem* __restrict__ y,
@@ -248,138 +253,55 @@ __global__ void poolblur_kernel(const __grid_constant__ ImgSet set, const typena
     Vec16<T>::store(y + pm * C + cv * VN, pout, acc, round_out);
 }
 
-// engine 4: max pooling on split tensors (values rebuilt in fp32, the maximum split again); one thread per (pixel, 8 channels)
-__global__ void maxpool_split_kernel(const __grid_constant__ ImgSet set, const __half* __restrict__ x, __half* __restrict__ y,
-                                     int C, int k, int stride, int pad, long long pin, long long pout) {
-    const int c8n = C >> 3;
-    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    long long total = set.out_pix[set.n] * c8n;
-    if (t >= total) return;
-    long long pm = t / c8n;
-    int c8 = (int)(t - pm * c8n);
-    int im = find_img(set, pm);
-    int local = (int)(pm - set.out_pix[im]);
-    int oy = local / set.Wo[im], ox = local - oy * set.Wo[im];
-    const int H = set.H[im], W = set.W[im];
-    float m[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) m[e] = -INFINITY;
-    for (int r = 0; r < k; ++r) {
-        int iy = oy * stride - pad + r;
-        if (iy < 0 || iy >= H) continue;
-        for (int s = 0; s < k; ++s) {
-            int ix = ox * stride - pad + s;
-            if (ix < 0 || ix >= W) continue;
-            float v[8];
-            split_load8(x + (set.in_pix[im] + (long long)iy * W + ix) * C + c8 * 8, pin, v);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) m[e] = fmaxf(m[e], v[e]);
-        }
-    }
-    split_store8(y + pm * C + c8 * 8, pout, m);
-}
-
 // ---------------------------------------------------------------------------
-// F.normalize(dim=1): one warp per pixel (coarseAlignFeatMatch.py:106,124; evaluation.py:26,184)
+// F.normalize(dim=1): one warp per pixel (coarseAlignFeatMatch.py:106,124; evaluation.py:26,184); fp32 arithmetic and
+// output whatever the input format.  `y` (nullable when the planes are written): the fp32 rows.  Split input only, `yhi` /
+// `ylo` (nullable): ALSO the normalised rows as the fp16 hi / lo * 2^11 planes the fp16-split correlation kernel reads
+// (rf_corr_mutual_nn with presplit operands), which saves its split pass.
 // ---------------------------------------------------------------------------
-__global__ void l2norm_kernel(const float* __restrict__ x, long long P, int C, const unsigned char* __restrict__ mask, float* __restrict__ y) {
+template <typename T>
+__global__ void l2norm_kernel(const typename Vec16<T>::elem* __restrict__ x, long long plane, long long P, int C,
+                              const unsigned char* __restrict__ mask, float* __restrict__ y, __half* __restrict__ yhi, __half* __restrict__ ylo) {
+    constexpr int VN = Vec16<T>::N;
+    constexpr bool planes = std::is_same<T, SplitH>::value;
     long long pix = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     int lane = threadIdx.x & 31;
     if (pix >= P) return;
-    const float4* src = reinterpret_cast<const float4*>(x + pix * C);
+    const typename Vec16<T>::elem* src = x + pix * C;
     float4* dst = reinterpret_cast<float4*>(y + pix * C);
-    const int c4n = C >> 2;
-    if (mask != nullptr && mask[pix] == 0) {
-        for (int c = lane; c < c4n; c += 32) dst[c] = make_float4(0, 0, 0, 0);
-        return;
-    }
-    float ss = 0.f;
-    for (int c = lane; c < c4n; c += 32) {
-        float4 v = __ldg(src + c);
-        ss = fmaf(v.x, v.x, ss); ss = fmaf(v.y, v.y, ss); ss = fmaf(v.z, v.z, ss); ss = fmaf(v.w, v.w, ss);
-    }
-#pragma unroll
-    for (int d = 16; d >= 1; d >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, d);
-    float denom = fmaxf(sqrtf(ss), 1e-12f);
-    for (int c = lane; c < c4n; c += 32) {
-        float4 v = __ldg(src + c);
-        dst[c] = make_float4(__fdiv_rn(v.x, denom), __fdiv_rn(v.y, denom), __fdiv_rn(v.z, denom), __fdiv_rn(v.w, denom));
-    }
-}
-
-// fp16 input (engine-2 trunk output), fp32 arithmetic and output
-__global__ void l2norm_f16_kernel(const __half* __restrict__ x, long long P, int C, const unsigned char* __restrict__ mask, float* __restrict__ y) {
-    long long pix = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    int lane = threadIdx.x & 31;
-    if (pix >= P) return;
-    const uint4* src = reinterpret_cast<const uint4*>(x + pix * C);
-    float4* dst = reinterpret_cast<float4*>(y + pix * C);
-    const int c8n = C >> 3;
-    if (mask != nullptr && mask[pix] == 0) {
-        for (int c = lane; c < 2 * c8n; c += 32) dst[c] = make_float4(0, 0, 0, 0);
-        return;
-    }
-    float ss = 0.f;
-    for (int c = lane; c < c8n; c += 32) {
-        const uint4 v = __ldg(src + c);
-        const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-        for (int e = 0; e < 4; ++e) { const float2 f = __half22float2(h[e]); ss = fmaf(f.x, f.x, ss); ss = fmaf(f.y, f.y, ss); }
-    }
-#pragma unroll
-    for (int d = 16; d >= 1; d >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, d);
-    float denom = fmaxf(sqrtf(ss), 1e-12f);
-    for (int c = lane; c < c8n; c += 32) {
-        const uint4 v = __ldg(src + c);
-        const __half2* h = reinterpret_cast<const __half2*>(&v);
-        const float2 f0 = __half22float2(h[0]), f1 = __half22float2(h[1]), f2 = __half22float2(h[2]), f3 = __half22float2(h[3]);
-        dst[2 * c] = make_float4(__fdiv_rn(f0.x, denom), __fdiv_rn(f0.y, denom), __fdiv_rn(f1.x, denom), __fdiv_rn(f1.y, denom));
-        dst[2 * c + 1] = make_float4(__fdiv_rn(f2.x, denom), __fdiv_rn(f2.y, denom), __fdiv_rn(f3.x, denom), __fdiv_rn(f3.y, denom));
-    }
-}
-
-// engine 4: split input (planes `plane` elements apart), fp32 arithmetic and output.  `yhi` / `ylo` (nullable): ALSO write
-// the normalised rows as the fp16 hi / lo * 2^11 planes the fp16-split correlation kernel reads (rf_corr_mutual_nn with
-// presplit operands), which saves its split pass.
-__global__ void l2norm_split_kernel(const __half* __restrict__ x, long long plane, long long P, int C, const unsigned char* __restrict__ mask,
-                                    float* __restrict__ y, __half* __restrict__ yhi, __half* __restrict__ ylo) {
-    long long pix = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    int lane = threadIdx.x & 31;
-    if (pix >= P) return;
-    const __half* src = x + pix * C;
-    float4* dst = reinterpret_cast<float4*>(y + pix * C);       // y == nullptr: planes only
-    const int c8n = C >> 3;
+    const int cvn = C / VN;
     if (mask != nullptr && mask[pix] == 0) {
         if (y != nullptr)
-            for (int c = lane; c < 2 * c8n; c += 32) dst[c] = make_float4(0, 0, 0, 0);
-        if (yhi != nullptr)
-            for (int c = lane; c < c8n; c += 32) {
-                reinterpret_cast<uint4*>(yhi + pix * C)[c] = make_uint4(0, 0, 0, 0);
-                reinterpret_cast<uint4*>(ylo + pix * C)[c] = make_uint4(0, 0, 0, 0);
-            }
+            for (int c = lane; c < C / 4; c += 32) dst[c] = make_float4(0, 0, 0, 0);
+        if constexpr (planes)
+            if (yhi != nullptr)
+                for (int c = lane; c < cvn; c += 32) {
+                    reinterpret_cast<uint4*>(yhi + pix * C)[c] = make_uint4(0, 0, 0, 0);
+                    reinterpret_cast<uint4*>(ylo + pix * C)[c] = make_uint4(0, 0, 0, 0);
+                }
         return;
     }
     // (a single-pass variant that keeps the row in registers measured slower: 72 vs 55 us for the three calls of a pair)
     float ss = 0.f;
-    for (int c = lane; c < c8n; c += 32) {
-        float v[8];
-        split_load8(src + c * 8, plane, v);
+    for (int c = lane; c < cvn; c += 32) {
+        float v[VN];
+        Vec16<T>::load(src + c * VN, plane, v);
 #pragma unroll
-        for (int e = 0; e < 8; ++e) ss = fmaf(v[e], v[e], ss);
+        for (int e = 0; e < VN; ++e) ss = fmaf(v[e], v[e], ss);
     }
 #pragma unroll
     for (int d = 16; d >= 1; d >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, d);
     float denom = fmaxf(sqrtf(ss), 1e-12f);
-    for (int c = lane; c < c8n; c += 32) {
-        float v[8];
-        split_load8(src + c * 8, plane, v);
+    for (int c = lane; c < cvn; c += 32) {
+        float v[VN];
+        Vec16<T>::load(src + c * VN, plane, v);
 #pragma unroll
-        for (int e = 0; e < 8; ++e) v[e] = __fdiv_rn(v[e], denom);
-        if (y != nullptr) {
-            dst[2 * c] = make_float4(v[0], v[1], v[2], v[3]);
-            dst[2 * c + 1] = make_float4(v[4], v[5], v[6], v[7]);
-        }
-        if (yhi != nullptr) split_store8(yhi + pix * C + c * 8, (ylo - yhi), v);
+        for (int e = 0; e < VN; ++e) v[e] = __fdiv_rn(v[e], denom);
+        if (y != nullptr)
+#pragma unroll
+            for (int q = 0; q < VN / 4; ++q) dst[c * (VN / 4) + q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+        if constexpr (planes)
+            if (yhi != nullptr) split_store8(yhi + pix * C + c * 8, (ylo - yhi), v);
     }
 }
 
@@ -982,54 +904,84 @@ static int launch_corr_neigh(const float* x, const float* y, int N, int h, int w
     return 0;
 }
 
-extern "C" int rf_maxpool2d_nhwc(const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, float* y, void* stream) {
-    RF_REQUIRE((C % 4) == 0 && k >= 1 && stride >= 1, "rf_maxpool2d_nhwc: C must be a multiple of 4");
+// ---- the layer ops of rf_run_layers, one launcher per op over the activation format ----
+// Vec16 width of a format: the channel count must be a multiple of it
+static int vec_width(ActFormat f) { return f == ACT_F16 || f == ACT_SPLIT ? 8 : 4; }
+
+// launch(T()) with the Vec16 type of the format: float (fp32, TF32), __half (fp16) or SplitH (split)
+template <typename Launch>
+static void for_format(ActFormat f, Launch&& launch) {
+    if (f == ACT_F16) launch(__half());
+    else if (f == ACT_SPLIT) launch(SplitH());
+    else launch(float());
+}
+
+// One thread per (output pixel, 16-byte vector).  Split planes are the whole input / output tensors apart; the other formats
+// ignore pin / pout.
+int rf_maxpool(ActFormat f, const void* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, void* y, void* stream) {
+    const int vn = vec_width(f);
+    RF_REQUIRE((C % vn) == 0 && k >= 1 && stride >= 1, "rf_maxpool: C must be a multiple of 4 (fp32) or 8 (fp16, split)");
     ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, k, stride, pad) == 0, "rf_maxpool2d_nhwc: bad image set");
-    long long total = set.out_pix[nimg] * (C / 4);
-    maxpool_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, x, y, C, k, stride, pad);
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, k, stride, pad) == 0, "rf_maxpool: bad image set");
+    const unsigned blocks = blocks_for(set.out_pix[nimg] * (C / vn), 256);
+    for_format(f, [&](auto t) {
+        typedef typename Vec16<decltype(t)>::elem E;
+        maxpool_kernel<decltype(t)><<<blocks, 256, 0, as_stream(stream)>>>(set, static_cast<const E*>(x), static_cast<E*>(y), C, k, stride, pad,
+                                                                           set.in_pix[nimg] * C, set.out_pix[nimg] * C);
+    });
     RF_LAUNCHED();
     return 0;
 }
 
-int rf_blur_downsample_impl(const float* x, int nimg, const int* hw_host, int C, int stride, int round_out, float* y, void* stream) {
-    RF_REQUIRE((C % 4) == 0 && stride >= 1, "rf_blur_downsample_nhwc: C must be a multiple of 4");
+int rf_blur(ActFormat f, const void* x, int nimg, const int* hw_host, int C, int stride, void* y, void* stream) {
+    const int vn = vec_width(f);
+    RF_REQUIRE((C % vn) == 0 && stride >= 1, "rf_blur: C must be a multiple of 4 (fp32) or 8 (fp16, split)");
     ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, 3, stride, 1) == 0, "rf_blur_downsample_nhwc: bad image set");
-    for (int i = 0; i < nimg; ++i) RF_REQUIRE(set.H[i] >= 2 && set.W[i] >= 2, "rf_blur_downsample_nhwc: reflect padding needs H, W >= 2");
-    long long total = set.out_pix[nimg] * (C / 4);
-    blur_kernel<float><<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, x, y, C, stride, round_out);
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, 3, stride, 1) == 0, "rf_blur: bad image set");
+    for (int i = 0; i < nimg; ++i) RF_REQUIRE(set.H[i] >= 2 && set.W[i] >= 2, "rf_blur: reflect padding needs H, W >= 2");
+    const unsigned blocks = blocks_for(set.out_pix[nimg] * (C / vn), 256);
+    for_format(f, [&](auto t) {
+        typedef typename Vec16<decltype(t)>::elem E;
+        blur_kernel<decltype(t)><<<blocks, 256, 0, as_stream(stream)>>>(set, static_cast<const E*>(x), static_cast<E*>(y), C, stride, f == ACT_TF32,
+                                                                        set.in_pix[nimg] * C, set.out_pix[nimg] * C);
+    });
     RF_LAUNCHED();
     return 0;
 }
 
 // output size of maxpool(2,1) + blur(stride 2): ((H-1) + 2 - 3)/2 + 1 = make_imgset with k = 4, stride 2, pad 1
-int rf_poolblur_impl(const float* x, int nimg, const int* hw_host, int C, int round_out, float* y, void* stream) {
-    RF_REQUIRE((C % 4) == 0, "rf_poolblur: C must be a multiple of 4");
+int rf_poolblur(ActFormat f, const void* x, int nimg, const int* hw_host, int C, void* y, void* stream) {
+    const int vn = vec_width(f);
+    RF_REQUIRE((C % vn) == 0, "rf_poolblur: C must be a multiple of 4 (fp32) or 8 (fp16, split)");
     ImgSet set;
     RF_REQUIRE(make_imgset(set, nimg, hw_host, 4, 2, 1) == 0, "rf_poolblur: bad image set");
     for (int i = 0; i < nimg; ++i) RF_REQUIRE(set.H[i] >= 3 && set.W[i] >= 3, "rf_poolblur: needs H, W >= 3");
-    long long total = set.out_pix[nimg] * (C / 4);
-    poolblur_kernel<float><<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, x, y, C, round_out);
+    const unsigned blocks = blocks_for(set.out_pix[nimg] * (C / vn), 256);
+    for_format(f, [&](auto t) {
+        typedef typename Vec16<decltype(t)>::elem E;
+        poolblur_kernel<decltype(t)><<<blocks, 256, 0, as_stream(stream)>>>(set, static_cast<const E*>(x), static_cast<E*>(y), C, f == ACT_TF32,
+                                                                            set.in_pix[nimg] * C, set.out_pix[nimg] * C);
+    });
     RF_LAUNCHED();
     return 0;
 }
 
+extern "C" int rf_maxpool2d_nhwc(const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, float* y, void* stream) {
+    return rf_maxpool(ACT_F32, x, nimg, hw_host, C, k, stride, pad, y, stream);
+}
+
 extern "C" int rf_blur_downsample_nhwc(const float* x, int nimg, const int* hw_host, int C, int stride, float* y, void* stream) {
-    return rf_blur_downsample_impl(x, nimg, hw_host, C, stride, 0, y, stream);
+    return rf_blur(ACT_F32, x, nimg, hw_host, C, stride, y, stream);
 }
 
 // Stem-specialised im2col: one CTA = one output row segment of TPX pixels.  The K input rows it needs are staged in
-// shared memory with coalesced loads, then the (r, s, c)-ordered patches are written as contiguous float4 rows.
-template <typename T> struct OutElem { typedef T type; };
-template <> struct OutElem<SplitH> { typedef __half type; };
-
+// shared memory with coalesced loads, then the (r, s, c)-ordered patches are written as contiguous rows of 16-byte vectors.
 template <int K, int C, int KPAD, int STRIDE, int PAD, int TPX, typename OutT = float>
 __global__ void __launch_bounds__(256)
-im2col_smem_kernel(const __grid_constant__ ImgSet set, const float* __restrict__ x, typename OutElem<OutT>::type* __restrict__ y, int round_out,
+im2col_smem_kernel(const __grid_constant__ ImgSet set, const float* __restrict__ x, typename Vec16<OutT>::elem* __restrict__ y, int round_out,
                    long long plane = 0) {
     constexpr int INW = ((TPX - 1) * STRIDE + K) * C;          // floats of one staged input row
-    constexpr int Q4 = KPAD / 4;
+    constexpr int VN = Vec16<OutT>::N, QV = KPAD / VN;
     __shared__ float sIn[K][INW + 1];
     const int im = blockIdx.z, oy = blockIdx.y, ox0 = blockIdx.x * TPX;
     const int Wo = set.Wo[im];
@@ -1055,135 +1007,66 @@ im2col_smem_kernel(const __grid_constant__ ImgSet set, const float* __restrict__
     }
     __syncthreads();
     const int npx = min(TPX, Wo - ox0);
-    if constexpr (std::is_same<OutT, SplitH>::value) {
-        // engine 4: rows of KPAD values as hi / lo planes
-        constexpr int Q8 = KPAD / 8;
-        __half* dsts = y + (set.out_pix[im] + (long long)oy * Wo + ox0) * KPAD;
-        for (int f = threadIdx.x; f < npx * Q8; f += 256) {
-            const int px = f / Q8, e0 = (f - px * Q8) * 8;
-            float v[8];
+    typename Vec16<OutT>::elem* dst = y + (set.out_pix[im] + (long long)oy * Wo + ox0) * KPAD;
+    for (int f = threadIdx.x; f < npx * QV; f += 256) {
+        const int px = f / QV, e0 = (f - px * QV) * VN;
+        float v[VN];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int e = e0 + j;
-                v[j] = (e < K * K * C) ? sIn[e / (K * C)][px * STRIDE * C + e % (K * C)] : 0.f;
-            }
-            split_store8(dsts + (long long)f * 8, plane, v);
-        }
-        return;
-    } else if constexpr (sizeof(OutT) == 2) {
-        // engine 2: rows of KPAD halves, eight per 16-byte store
-        constexpr int Q8 = KPAD / 8;
-        uint4* dst8 = reinterpret_cast<uint4*>(y + (set.out_pix[im] + (long long)oy * Wo + ox0) * KPAD);
-        for (int f = threadIdx.x; f < npx * Q8; f += 256) {
-            const int px = f / Q8, e0 = (f - px * Q8) * 8;
-            float v[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int e = e0 + j;
-                v[j] = (e < K * K * C) ? sIn[e / (K * C)][px * STRIDE * C + e % (K * C)] : 0.f;
-            }
-            uint4 o;
-            __half2* ho = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) ho[j] = __floats2half2_rn(v[2 * j], v[2 * j + 1]);
-            dst8[f] = o;
-        }
-        return;
-    }
-    float4* dst = reinterpret_cast<float4*>(y + (set.out_pix[im] + (long long)oy * Wo + ox0) * KPAD);
-    for (int f = threadIdx.x; f < npx * Q4; f += 256) {
-        const int px = f / Q4, e0 = (f - px * Q4) * 4;
-        float v[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < VN; ++j) {
             const int e = e0 + j;
             v[j] = (e < K * K * C) ? sIn[e / (K * C)][px * STRIDE * C + e % (K * C)] : 0.f;
         }
-        dst[f] = make_float4(v[0], v[1], v[2], v[3]);
+        Vec16<OutT>::store(dst + (long long)f * VN, plane, v, 0);
     }
 }
 
-int rf_im2col_impl(const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, int Kpad, int round_out,
-                   float* y, void* stream) {
+// fp32 / TF32: any shape (the two stems on the shared-memory kernel).  fp16 rows only for the ResNet-50 stem (7x7/2, Kpad 192)
+// and the FeatureExtractor stem (3x3/1, Kpad 64); split rows only for the FeatureExtractor stem.
+int rf_im2col(ActFormat f, const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, int Kpad, void* y, void* stream) {
+    const bool f32 = f == ACT_F32 || f == ACT_TF32;
+    const bool resnet = k == 7 && C == 3 && stride == 2 && pad == 3 && Kpad == (f32 ? 160 : 192);
+    const bool fe = k == 3 && C == 3 && stride == 1 && pad == 1 && Kpad == (f32 ? 32 : 64);
+    RF_REQUIRE(f != ACT_F16 || resnet || fe, "rf_im2col (fp16): only the ResNet-50 stem (7x7/2, Kpad 192) and the FeatureExtractor stem (3x3/1, Kpad 64)");
+    RF_REQUIRE(f != ACT_SPLIT || fe, "rf_im2col (split): only the FeatureExtractor stem (3x3/1, Kpad 64)");
     RF_REQUIRE(Kpad >= k * k * C && C >= 1, "rf_im2col: Kpad too small");
     ImgSet set;
     RF_REQUIRE(make_imgset(set, nimg, hw_host, k, stride, pad) == 0, "rf_im2col: bad image set");
     RF_REQUIRE((Kpad & 3) == 0, "rf_im2col: Kpad must be a multiple of 4");
     long long maxq = 0;
+    int maxHo = 0, maxWo = 0;
     for (int i = 0; i < nimg; ++i) {
-        long long q = (long long)set.Ho[i] * set.Wo[i] * (Kpad / 4);
-        RF_REQUIRE(q < (1ll << 31), "rf_im2col: image too large for 32-bit indexing");
-        if (q > maxq) maxq = q;
+        const long long q = (long long)set.Ho[i] * set.Wo[i] * (Kpad / 4);
+        RF_REQUIRE(!f32 || q < (1ll << 31), "rf_im2col: image too large for 32-bit indexing");
+        maxq = q > maxq ? q : maxq;
+        maxHo = set.Ho[i] > maxHo ? set.Ho[i] : maxHo;
+        maxWo = set.Wo[i] > maxWo ? set.Wo[i] : maxWo;
     }
-    int maxHo = 0, maxWo = 0;
-    for (int i = 0; i < nimg; ++i) { maxHo = set.Ho[i] > maxHo ? set.Ho[i] : maxHo; maxWo = set.Wo[i] > maxWo ? set.Wo[i] : maxWo; }
-    if (k == 7 && C == 3 && Kpad == 160 && stride == 2 && pad == 3) {          // ResNet-50 stem
-        im2col_smem_kernel<7, 3, 160, 2, 3, 64><<<dim3((maxWo + 63) / 64, maxHo, nimg), 256, 0, as_stream(stream)>>>(set, x, y, round_out);
-        RF_LAUNCHED();
-        return 0;
+    const int round_out = f == ACT_TF32;
+    const dim3 grid_resnet((maxWo + 63) / 64, maxHo, nimg), grid_fe((maxWo + 127) / 128, maxHo, nimg);
+    cudaStream_t st = as_stream(stream);
+    float* y32 = static_cast<float*>(y);
+    __half* y16 = static_cast<__half*>(y);
+    if (f == ACT_SPLIT) im2col_smem_kernel<3, 3, 64, 1, 1, 128, SplitH><<<grid_fe, 256, 0, st>>>(set, x, y16, 0, set.out_pix[nimg] * 64);
+    else if (f == ACT_F16 && resnet) im2col_smem_kernel<7, 3, 192, 2, 3, 64, __half><<<grid_resnet, 256, 0, st>>>(set, x, y16, 0);
+    else if (f == ACT_F16) im2col_smem_kernel<3, 3, 64, 1, 1, 128, __half><<<grid_fe, 256, 0, st>>>(set, x, y16, 0);
+    else if (resnet) im2col_smem_kernel<7, 3, 160, 2, 3, 64><<<grid_resnet, 256, 0, st>>>(set, x, y32, round_out);
+    else if (fe) im2col_smem_kernel<3, 3, 32, 1, 1, 128><<<grid_fe, 256, 0, st>>>(set, x, y32, round_out);
+    else {
+        const dim3 grid(blocks_for(maxq, 256), nimg);
+        if (k == 7 && C == 3 && Kpad == 160) im2col_kernel<7, 3, 160><<<grid, 256, 0, st>>>(set, x, y32, C, k, stride, pad, Kpad, round_out);
+        else if (k == 3 && C == 3 && Kpad == 32) im2col_kernel<3, 3, 32><<<grid, 256, 0, st>>>(set, x, y32, C, k, stride, pad, Kpad, round_out);
+        else im2col_kernel<0, 0, 0><<<grid, 256, 0, st>>>(set, x, y32, C, k, stride, pad, Kpad, round_out);
     }
-    if (k == 3 && C == 3 && Kpad == 32 && stride == 1 && pad == 1) {           // FeatureExtractor stem
-        im2col_smem_kernel<3, 3, 32, 1, 1, 128><<<dim3((maxWo + 127) / 128, maxHo, nimg), 256, 0, as_stream(stream)>>>(set, x, y, round_out);
-        RF_LAUNCHED();
-        return 0;
-    }
-    dim3 grid(blocks_for(maxq, 256), nimg);
-    if (k == 7 && C == 3 && Kpad == 160) im2col_kernel<7, 3, 160><<<grid, 256, 0, as_stream(stream)>>>(set, x, y, C, k, stride, pad, Kpad, round_out);
-    else if (k == 3 && C == 3 && Kpad == 32) im2col_kernel<3, 3, 32><<<grid, 256, 0, as_stream(stream)>>>(set, x, y, C, k, stride, pad, Kpad, round_out);
-    else im2col_kernel<0, 0, 0><<<grid, 256, 0, as_stream(stream)>>>(set, x, y, C, k, stride, pad, Kpad, round_out);
     RF_LAUNCHED();
     return 0;
 }
 
-// engine 2 (fp16 activations): the ResNet-50 stem's patches as rows of 192 halves; max pooling in fp16
-int rf_im2col_f16_impl(const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, int Kpad, void* y_f16, void* stream) {
-    const bool resnet = (k == 7 && C == 3 && Kpad == 192 && stride == 2 && pad == 3);
-    const bool fe = (k == 3 && C == 3 && Kpad == 64 && stride == 1 && pad == 1);
-    RF_REQUIRE(resnet || fe, "rf_im2col (engine 2): only the ResNet-50 stem (7x7/2, Kpad 192) and the FeatureExtractor stem (3x3/1, Kpad 64)");
-    ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, k, stride, pad) == 0, "rf_im2col: bad image set");
-    int maxHo = 0, maxWo = 0;
-    for (int i = 0; i < nimg; ++i) { maxHo = set.Ho[i] > maxHo ? set.Ho[i] : maxHo; maxWo = set.Wo[i] > maxWo ? set.Wo[i] : maxWo; }
-    if (fe) {
-        im2col_smem_kernel<3, 3, 64, 1, 1, 128, __half><<<dim3((maxWo + 127) / 128, maxHo, nimg), 256, 0, as_stream(stream)>>>(
-            set, x, static_cast<__half*>(y_f16), 0);
-        RF_LAUNCHED();
-        return 0;
-    }
-    im2col_smem_kernel<7, 3, 192, 2, 3, 64, __half><<<dim3((maxWo + 63) / 64, maxHo, nimg), 256, 0, as_stream(stream)>>>(
-        set, x, static_cast<__half*>(y_f16), 0);
-    RF_LAUNCHED();
-    return 0;
-}
-
-int rf_blur_f16_impl(const void* x_f16, int nimg, const int* hw_host, int C, int stride, void* y_f16, void* stream) {
-    RF_REQUIRE((C % 8) == 0 && stride >= 1, "rf_blur (engine 2): C must be a multiple of 8");
-    ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, 3, stride, 1) == 0, "rf_blur: bad image set");
-    for (int i = 0; i < nimg; ++i) RF_REQUIRE(set.H[i] >= 2 && set.W[i] >= 2, "rf_blur: reflect padding needs H, W >= 2");
-    long long total = set.out_pix[nimg] * (C / 8);
-    blur_kernel<__half><<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, static_cast<const __half*>(x_f16), static_cast<__half*>(y_f16), C, stride, 0);
-    RF_LAUNCHED();
-    return 0;
-}
-
-int rf_poolblur_f16_impl(const void* x_f16, int nimg, const int* hw_host, int C, void* y_f16, void* stream) {
-    RF_REQUIRE((C % 8) == 0, "rf_poolblur (engine 2): C must be a multiple of 8");
-    ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, 4, 2, 1) == 0, "rf_poolblur: bad image set");
-    for (int i = 0; i < nimg; ++i) RF_REQUIRE(set.H[i] >= 3 && set.W[i] >= 3, "rf_poolblur: needs H, W >= 3");
-    long long total = set.out_pix[nimg] * (C / 8);
-    poolblur_kernel<__half><<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, static_cast<const __half*>(x_f16), static_cast<__half*>(y_f16), C, 0);
-    RF_LAUNCHED();
-    return 0;
-}
-
-int rf_maxpool_f16_impl(const void* x_f16, int nimg, const int* hw_host, int C, int k, int stride, int pad, void* y_f16, void* stream) {
-    RF_REQUIRE((C % 8) == 0 && k >= 1 && stride >= 1, "rf_maxpool (engine 2): C must be a multiple of 8");
-    ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, k, stride, pad) == 0, "rf_maxpool: bad image set");
-    long long total = set.out_pix[nimg] * (C / 8);
-    maxpool_f16_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, static_cast<const __half*>(x_f16), static_cast<__half*>(y_f16), C, k, stride, pad);
+// P rows of C channels (C a multiple of the format's Vec16 width; split planes P * C elements apart) -> fp32 rows / split planes
+template <typename T>
+static int launch_l2norm(const void* x, long long P, int C, const uint8_t* mask, float* y, void* y_hi, void* y_lo, void* stream) {
+    if (P == 0) return 0;
+    l2norm_kernel<T><<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(static_cast<const typename Vec16<T>::elem*>(x), P * C, P, C, mask, y,
+                                                                              static_cast<__half*>(y_hi), static_cast<__half*>(y_lo));
     RF_LAUNCHED();
     return 0;
 }
@@ -1191,59 +1074,7 @@ int rf_maxpool_f16_impl(const void* x_f16, int nimg, const int* hw_host, int C, 
 extern "C" int rf_l2norm_f16_nhwc(const void* x_f16, long long P, int C, const uint8_t* mask, float* y, void* stream) {
     RF_REQUIRE((C % 8) == 0 && P >= 0, "rf_l2norm_f16_nhwc: C must be a multiple of 8");
     RF_REQUIRE(((uintptr_t)x_f16 % 16) == 0 && ((uintptr_t)y % 16) == 0, "rf_l2norm_f16_nhwc: pointers must be 16-byte aligned");
-    if (P == 0) return 0;
-    l2norm_f16_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(static_cast<const __half*>(x_f16), P, C, mask, y);
-    RF_LAUNCHED();
-    return 0;
-}
-
-// ---- engine 4 (split tensors: [2][P][C] fp16 planes) ----
-int rf_blur_split_impl(const void* x, int nimg, const int* hw_host, int C, int stride, void* y, void* stream) {
-    RF_REQUIRE((C % 8) == 0 && stride >= 1, "rf_blur (engine 4): C must be a multiple of 8");
-    ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, 3, stride, 1) == 0, "rf_blur: bad image set");
-    for (int i = 0; i < nimg; ++i) RF_REQUIRE(set.H[i] >= 2 && set.W[i] >= 2, "rf_blur: reflect padding needs H, W >= 2");
-    long long total = set.out_pix[nimg] * (C / 8);
-    blur_kernel<SplitH><<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, static_cast<const __half*>(x), static_cast<__half*>(y), C, stride, 0,
-                                                                              set.in_pix[nimg] * C, set.out_pix[nimg] * C);
-    RF_LAUNCHED();
-    return 0;
-}
-
-int rf_poolblur_split_impl(const void* x, int nimg, const int* hw_host, int C, void* y, void* stream) {
-    RF_REQUIRE((C % 8) == 0, "rf_poolblur (engine 4): C must be a multiple of 8");
-    ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, 4, 2, 1) == 0, "rf_poolblur: bad image set");
-    for (int i = 0; i < nimg; ++i) RF_REQUIRE(set.H[i] >= 3 && set.W[i] >= 3, "rf_poolblur: needs H, W >= 3");
-    long long total = set.out_pix[nimg] * (C / 8);
-    poolblur_kernel<SplitH><<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, static_cast<const __half*>(x), static_cast<__half*>(y), C, 0,
-                                                                                  set.in_pix[nimg] * C, set.out_pix[nimg] * C);
-    RF_LAUNCHED();
-    return 0;
-}
-
-int rf_maxpool_split_impl(const void* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, void* y, void* stream) {
-    RF_REQUIRE((C % 8) == 0 && k >= 1 && stride >= 1, "rf_maxpool (engine 4): C must be a multiple of 8");
-    ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, k, stride, pad) == 0, "rf_maxpool: bad image set");
-    long long total = set.out_pix[nimg] * (C / 8);
-    maxpool_split_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(set, static_cast<const __half*>(x), static_cast<__half*>(y), C, k, stride, pad,
-                                                                               set.in_pix[nimg] * C, set.out_pix[nimg] * C);
-    RF_LAUNCHED();
-    return 0;
-}
-
-// FeatureExtractor stem patches (3x3 / 1 / pad 1, 27 -> 64 columns) as a split tensor
-int rf_im2col_split_impl(const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, int Kpad, void* y, void* stream) {
-    RF_REQUIRE(k == 3 && C == 3 && Kpad == 64 && stride == 1 && pad == 1, "rf_im2col (engine 4): only the FeatureExtractor stem (3x3/1, Kpad 64)");
-    ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, k, stride, pad) == 0, "rf_im2col: bad image set");
-    int maxHo = 0, maxWo = 0;
-    for (int i = 0; i < nimg; ++i) { maxHo = set.Ho[i] > maxHo ? set.Ho[i] : maxHo; maxWo = set.Wo[i] > maxWo ? set.Wo[i] : maxWo; }
-    im2col_smem_kernel<3, 3, 64, 1, 1, 128, SplitH><<<dim3((maxWo + 127) / 128, maxHo, nimg), 256, 0, as_stream(stream)>>>(
-        set, x, static_cast<__half*>(y), 0, set.out_pix[nimg] * 64);
-    RF_LAUNCHED();
-    return 0;
+    return launch_l2norm<__half>(x_f16, P, C, mask, y, nullptr, nullptr, stream);
 }
 
 // segNet's deep-stem conv1 (segNet/segModel.py:64,108): 3x3 / stride 2 / pad 1 on the 3-channel fp32 image + folded BN + ReLU ->
@@ -1288,7 +1119,7 @@ __global__ void __launch_bounds__(256) stem3_split_kernel(const __grid_constant_
     split_store8(y + pix * 64 + c0, plane, acc);
 }
 
-int rf_stem3_split_impl(const float* x, int nimg, const int* hw_host, const float* w, const float* bias, void* y, void* stream) {
+int rf_stem3(const float* x, int nimg, const int* hw_host, const float* w, const float* bias, void* y, void* stream) {
     RF_REQUIRE(x != nullptr && w != nullptr && y != nullptr && ((uintptr_t)y % 16) == 0, "rf_stem3 (engine 4): null or misaligned pointer");
     ImgSet set;
     RF_REQUIRE(make_imgset(set, nimg, hw_host, 3, 2, 1) == 0, "rf_stem3: bad image set");
@@ -1529,11 +1360,7 @@ extern "C" int rf_l2norm_split_nhwc(const void* x_split, long long P, int C, con
                "rf_l2norm_split_nhwc: pointers must be 16-byte aligned");
     RF_REQUIRE((y_hi == nullptr) == (y_lo == nullptr), "rf_l2norm_split_nhwc: y_hi and y_lo go together");
     RF_REQUIRE(y != nullptr || y_hi != nullptr, "rf_l2norm_split_nhwc: no output");
-    if (P == 0) return 0;
-    l2norm_split_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(static_cast<const __half*>(x_split), P * C, P, C, mask, y,
-                                                                               static_cast<__half*>(y_hi), static_cast<__half*>(y_lo));
-    RF_LAUNCHED();
-    return 0;
+    return launch_l2norm<SplitH>(x_split, P, C, mask, y, y_hi, y_lo, stream);
 }
 
 extern "C" int rf_corr_neigh_pair_split(const float* x, const float* y, int N, int h, int w, int C, int k, int ldo, void* out12_split, void* both_split,
@@ -1545,10 +1372,7 @@ extern "C" int rf_corr_neigh_pair_split(const float* x, const float* y, int N, i
 
 extern "C" int rf_l2norm_nhwc(const float* x, long long P, int C, const uint8_t* mask, float* y, void* stream) {
     RF_REQUIRE((C % 4) == 0 && P >= 0, "rf_l2norm_nhwc: C must be a multiple of 4");
-    if (P == 0) return 0;
-    l2norm_kernel<<<blocks_for(P * 32, 256), 256, 0, as_stream(stream)>>>(x, P, C, mask, y);
-    RF_LAUNCHED();
-    return 0;
+    return launch_l2norm<float>(x, P, C, mask, y, nullptr, nullptr, stream);
 }
 
 extern "C" int rf_corr_neigh_nhwc(const float* x, const float* y, int N, int h, int w, int C, int k, int ldo, int round_tf32_out, float* out, void* stream) {

@@ -1028,13 +1028,10 @@ extern "C" int rf_conv1x1_dual_split(const void* x1, const void* x2, int nimg, c
     return conv_impl(set, p, w_split, as_stream(stream), K_SPLIT, false, &dual);
 }
 
-// fused ResNet-50 stem (pool: and its 3x3 / stride 2 / pad 1 max-pool).  x fp32 [sum HW][3], bias fp32 [64]; engine 2: w_f16
-// [64][192] ((r, s, c) order, zero padded), y fp16 [sum HoWo][64]; engine 4: w_split [2][64][192], y split [2][sum HoWo][64]
-int rf_stem7_f16_impl(const float* x, int nimg, const int* hw_host, const void* w_f16, const float* bias, int pool, void* y_f16, void* stream) {
-    return stem_impl<false>(x, nimg, hw_host, w_f16, bias, y_f16, pool, stream);
-}
-int rf_stem7_split_impl(const float* x, int nimg, const int* hw_host, const void* w_split, const float* bias, int pool, void* y_split, void* stream) {
-    return stem_impl<true>(x, nimg, hw_host, w_split, bias, y_split, pool, stream);
+// fused ResNet-50 stem (pool: and its 3x3 / stride 2 / pad 1 max-pool).  x fp32 [sum HW][3], bias fp32 [64]; fp16 (engine 2):
+// w [64][192] ((r, s, c) order, zero padded), y fp16 [sum HoWo][64]; split (engine 4): w [2][64][192], y split [2][sum HoWo][64]
+int rf_stem7(ActFormat f, const float* x, int nimg, const int* hw_host, const void* w, const float* bias, int pool, void* y, void* stream) {
+    return f == ACT_SPLIT ? stem_impl<true>(x, nimg, hw_host, w, bias, y, pool, stream) : stem_impl<false>(x, nimg, hw_host, w, bias, y, pool, stream);
 }
 
 size_t rf_corr_tc_workspace(int NA, int NB, int C) { return 2ull * ((size_t)NA + NB) * C * sizeof(float) + 1024; }

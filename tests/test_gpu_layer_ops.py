@@ -315,6 +315,47 @@ def test_layer_op_refusals_launch_nothing(rf, engine, op, c, size):
     assert rf._lib.launch_count() == n0
 
 
+def engine_only_program(op):
+    """One-op programs whose ops the library runs on some activation formats only; the Python-side guards are switched off so
+    that the library's own check is the one exercised."""
+    from ransac_flow_b200.model import FoldedConv
+    from ransac_flow_b200.program import LayerProgram
+    g = torch.Generator().manual_seed(5)
+    if op == "maxpool":
+        return build(("maxpool", 3, 2, 1), 8), 8
+    if op == "conv_dual":
+        fa, fb = (FoldedConv(torch.randn(64, 64, 1, 1, generator=g) / 8, None, 1, pad=0, device="cuda") for _ in range(2))
+        P = LayerProgram(64, device="cuda")
+        P.conv_dual(0, 0, FoldedConv.concat_k(fa, fb), 1, relu=True)
+        P.split_only = False
+        return P, 64
+    P = LayerProgram(3, device="cuda")
+    if op == "stem3":
+        P.stem3(0, torch.randn(64, 3, 3, 3, generator=g) / 5, None)
+        P.split_only = False
+    else:
+        P.stem7_fused(0, torch.randn(64, 3, 7, 7, generator=g) / 12, None)
+        P.f16_only = False
+    return P, 3
+
+
+# RF_OP_STEM3 / RF_OP_CONV_DUAL: engine 4 only; RF_OP_STEM7: engines 2 / 4; engines 3 and 5 are conv output modes, not formats
+ENGINE_REFUSALS = [("stem3", 0), ("stem3", 1), ("stem3", 2), ("conv_dual", 0), ("conv_dual", 1), ("conv_dual", 2),
+                   ("stem7", 0), ("stem7", 1), ("maxpool", 3), ("maxpool", 5)]
+
+
+@pytest.mark.parametrize("op,engine", ENGINE_REFUSALS)
+def test_layer_op_engine_refusals_launch_nothing(rf, op, engine):
+    P, c = engine_only_program(op)
+    dtype = torch.float16 if engine == 2 and op != "stem7" else torch.float32
+    x = rf.ops.Ragged(torch.zeros(16 * 16, c, device="cuda", dtype=dtype), [(16, 16)])
+    torch.cuda.synchronize()
+    n0 = rf._lib.launch_count()
+    with pytest.raises(rf._lib.RFError):
+        P.run(x, engine)
+    assert rf._lib.launch_count() == n0
+
+
 # ------------------------------------------------------------------ L2 normalisation (rf_l2norm_nhwc / _f16_nhwc / _split_nhwc)
 def l2_rows(seed, P, C, eps_rows):
     """Rows over six decades of scale, a row of zeros and, for fp32 inputs, rows with norms in (1e-14, 1e-13) (the eps branch:
