@@ -187,8 +187,8 @@ class _CoarseAlignBase:
         return Ragged(ops.l2norm(f.data), f.hw), u8
 
     def _pyramid(self, I_org, sizes):
-        """Resize ``I_org`` to each (w, h) in ``sizes``: PIL on the host, or the device resampler."""
-        if self.device_preproc:
+        """Resize ``I_org`` to each (w, h) in ``sizes``: PIL on the host, or the device resampler (always for a CUDA image)."""
+        if self.device_preproc or torch.is_tensor(I_org):
             src = I_org if torch.is_tensor(I_org) else self._to_device_u8(I_org)
             return [ops.resize_lanczos_u8(src, w, h) for (w, h) in sizes]
         return [I_org.resize((w, h), resample=Image.LANCZOS) for (w, h) in sizes]
@@ -273,6 +273,25 @@ class _CoarseAlignBase:
         MtTensor = ops.upsample_bilinear(MtExtend, (self.W2, self.H2))
         return (MtTensor > 0.5).squeeze()
 
+    def _valid16(self, Mt):
+        """The target cells a ``getCoarse_device`` mask keeps (uint8, 1 = kept), or None when nothing is masked.  ``Mt``: a
+        device-resident float mask (1 = masked) or a host array as ``getCoarse`` takes it."""
+        if torch.is_tensor(Mt):
+            MtTensor = ops.upsample_bilinear((1 - Mt).reshape(1, 1, Mt.shape[-2], Mt.shape[-1]).float(), (self.W2, self.H2))
+            return (MtTensor > 0.5).reshape(-1).to(torch.uint8).contiguous()
+        if Mt is not None and np.any(Mt):
+            return self._mask16(Mt).reshape(-1).to(torch.uint8).contiguous()
+        return None
+
+    def _ransac_device(self, match1, match2, cnt, samples=None):
+        """RANSAC on a device-resident match list of ``cnt`` matches (no host synchronisation): the reference's seeded
+        stream (``SAMPLES_PHILOX64``) or an injected (nbIter, 4) index table.  Returns (H [9], nbInlier [1], mask, status [1])."""
+        if samples is not None:
+            raw, mode = torch.as_tensor(samples, dtype=torch.int64).to(match1.device).contiguous(), ops.SAMPLES_MOD
+        else:
+            raw, mode = ops.philox_words(self.nbIter, self.nbPoint, match1.device, self.sample_generator), ops.SAMPLES_PHILOX64
+        return ops.ransac_homography(match1, match2, raw, self.tolerance, 100, cnt, mode)
+
     def skyFromSeg(self, path):
         """evaluation/evalHpatch/coarseAlignFeatMatch.py:152-153: the segNet mask of the image at ``path`` (float32 H x W)."""
         if getattr(self, "segNet", None) is None:
@@ -339,20 +358,10 @@ class CoarseAlignA(_CoarseAlignBase):
         inside a replayed CUDA graph.  ``samples`` (optional, (nbIter, 4) int64 indices): injected sample table instead
         (parity tests drive both paths with the oracle's ``last_samples``)."""
         with torch.no_grad():
-            valid16 = None
-            if torch.is_tensor(Mt):                          # device-resident mask (480x640 float, 1 = masked)
-                MtTensor = ops.upsample_bilinear((1 - Mt).reshape(1, 1, Mt.shape[-2], Mt.shape[-1]).float(), (self.W2, self.H2))
-                valid16 = (MtTensor > 0.5).reshape(-1).to(torch.uint8).contiguous()
-            elif Mt is not None and np.any(Mt):
-                valid16 = self._mask16(Mt).reshape(-1).to(torch.uint8).contiguous()
             match1, match2, _, cnt = ops.build_matches(self._idx1, self._idx2, self._count, self.WMultiScale, self.HMultiScale,
-                                                       self.Wt, self.Ht, valid16)
+                                                       self.Wt, self.Ht, self._valid16(Mt))
             self.match1, self.match2, self._match_count = match1, match2, cnt
-            if samples is not None:
-                raw, mode = torch.as_tensor(samples, dtype=torch.int64).to(match1.device).contiguous(), ops.SAMPLES_MOD
-            else:
-                raw, mode = ops.philox_words(self.nbIter, self.nbPoint, match1.device, self.sample_generator), ops.SAMPLES_PHILOX64
-            H, nb, mask, status = ops.ransac_homography(match1, match2, raw, self.tolerance, 100, cnt, mode)
+            H, nb, mask, status = self._ransac_device(match1, match2, cnt, samples)
             return H, nb, mask, status, cnt
 
     def getCoarse(self, Mt):
@@ -407,6 +416,80 @@ class CoarseAlignC(_CoarseAlignBase):
         flat = torch.cat([t.reshape(-1, 3) for t in u8], dim=0) if len(u8) > 1 else u8[0].reshape(-1, 3)
         f = self.net(Ragged(ops.preproc_u8(flat, normalize=True), hw))
         return Ragged(f.data.clone(), f.hw), u8        # the program owns its output buffer: keep a private copy
+
+    # -- evalYFCC's four-rotation target search (evaluation/evalYFCC/evaluation.py:191-212), device-resident ----------
+    def _set_rotated_pair(self, Is_org, It_org):
+        """``setSource(Is)`` and ``setTarget`` of the target rotated by 0 / 90 / 180 / 270 degrees, as ONE ragged batch of
+        len(scaleList) + 4 images through the trunk.  ``It.rotate(90 k, expand=True)`` is ``np.rot90(a, k)`` (a pure
+        permutation of the pixels), here ``torch.rot90`` on the device; each rotation is then resized by the bit-exact
+        LANCZOS resampler, in PIL's order (rotate, then resize).  Every rotation keeps its un-normalised conv4 features (the
+        masked re-matching of ``getCoarse`` needs them); ``_select_target(k)`` makes rotation k the current target."""
+        with torch.no_grad():
+            ws, hs = self._size_of(Is_org)
+            IsList = self._pyramid(Is_org, [self._target_size(ws, hs, int(self.minSize * s)) for s in self.scaleList])
+            t = It_org if torch.is_tensor(It_org) else self._to_device_u8(It_org)
+            ItList = []
+            for k in range(4):
+                r = torch.rot90(t, k, dims=(0, 1)).contiguous() if k else t
+                ItList.append(ops.resize_lanczos_u8(r, *self._target_size(int(r.shape[1]), int(r.shape[0]), self.minSize)))
+            feats_raw, u8 = self._features_raw(IsList + ItList)
+            nS = len(IsList)
+            mid = len(self.scaleList) // 2
+            self.Is = self._as_pil(IsList[mid])
+            self.IsTensor = self._to_tensor01(u8[mid])
+            # every row is normalised on its own, so normalising the batch gives each image what it gets alone
+            normed = Ragged(ops.l2norm(feats_raw.data), feats_raw.hw)
+            if feats_raw.split and outil.corr_precision == 2:
+                self._set_source_feats(Ragged(ops.l2norm_planes(feats_raw.data), feats_raw.hw), nS)      # as ``_features``
+            else:
+                self._set_source_feats(normed, nS)
+            o = feats_raw.offsets()
+            rows = (lambda a, b: feats_raw.data[:, a:b].contiguous()) if feats_raw.split else (lambda a, b: feats_raw.data[a:b])
+            self._rot = [dict(u8=u8[nS + k], raw=Ragged(rows(o[nS + k], o[nS + k + 1]), [feats_raw.hw[nS + k]]), normed=normed, i=nS + k)
+                         for k in range(4)]
+            self._select_target(0)
+
+    def _select_target(self, k):
+        """Rotation ``k`` of ``_set_rotated_pair`` becomes the current target: what ``setTarget`` of that rotation sets
+        (``It``, ``ItTensor``, ``featt``, ``W2`` / ``H2``, ``Wt`` / ``Ht`` / ``WtInt`` / ``HtInt``), without recomputing it.
+        The trunk computes each image of a ragged batch bit for bit as it computes that image alone (DESIGN section 2)."""
+        r = self._rot[k]
+        self.It = self._as_pil(r["u8"])
+        self.ItTensor = self._to_tensor01(r["u8"])
+        self._featt_raw = r["raw"]
+        self._set_target_feats(r["normed"], r["i"])
+
+    def rotated_target_size(self, k):
+        """(w, h) of rotation ``k`` of the resized target (``_set_rotated_pair``)."""
+        u8 = self._rot[k]["u8"]
+        return int(u8.shape[1]), int(u8.shape[0])
+
+    def _match_device(self, Mt=None):
+        """coarseAlignFeatMatch.py (B) :153-186 up to the match lists, on the device: the target's raw features with the
+        masked cells zeroed, re-normalised (:143 / :157-162), mutual matching against the source pyramid, the matched cells'
+        coordinates.  Returns (match1, match2, kept target cells, count [1] int32) without a host synchronisation (the mutual
+        pairs stay in ``_idx1`` / ``_idx2`` / ``_count``)."""
+        valid16 = self._valid16(Mt)
+        raw = self._featt_raw.data
+        if raw.dim() == 3 and "_src_planes" in self.__dict__:      # split engine + fp16-split correlation: planes end to end
+            tp, sp = ops.l2norm_planes(raw, valid16), self._src_planes
+            idx1, idx2, count = ops.corr_mutual_nn_presplit(sp[0], sp[1], tp[0], tp[1])
+        else:
+            idx1, idx2, count = ops.corr_mutual_nn(self._feats_rows, ops.l2norm(raw, valid16), outil.corr_precision)
+        match1, match2, kept, cnt = ops.build_matches(idx1, idx2, count, self.WMultiScale, self.HMultiScale, self.Wt, self.Ht, None)
+        self._idx1, self._idx2, self._count = idx1, idx2, count
+        self.match1, self.match2, self._match_count = match1, match2, cnt
+        return match1, match2, kept, cnt
+
+    def getCoarse_device(self, Mt=None, samples=None):
+        """Device-resident ``getCoarse`` (masked re-matching, then RANSAC) without a host synchronisation: returns
+        (H [9], nbInlier [1], inlier mask [NB], status [1], match_count [1]) as CUDA tensors, like
+        ``CoarseAlignA.getCoarse_device``.  Same match lists, H and inlier mask as ``getCoarse`` for the same samples;
+        ``samples`` None draws the reference's own stream (``SAMPLES_PHILOX64``)."""
+        with torch.no_grad():
+            match1, match2, _, cnt = self._match_device(Mt)
+            H, nb, mask, status = self._ransac_device(match1, match2, cnt, samples)
+            return H, nb, mask, status, cnt
 
     def getCoarse(self, Mt):
         with torch.no_grad():

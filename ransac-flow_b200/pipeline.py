@@ -458,6 +458,14 @@ def align_pair_device(coarseModel, network, Is, It, maxCoarse=0, maskRegionTh=0.
     end.  Same outputs as ``align_pair`` (plus ``nbMatch`` per hypothesis), and under a seed the same RANSAC samples per
     hypothesis.  ``samples``: optional list of injected (nbIter, 4) index tables, one per ``getCoarse`` call."""
     coarseModel.setPair(Is, It)
+    return _hypotheses_device(coarseModel, network, maxCoarse, maskRegionTh, with_match21, It_bg, samples)
+
+
+def _hypotheses_device(coarseModel, network, maxCoarse, maskRegionTh, with_match21, It_bg, samples, rewind_too_few=False):
+    """The hypothesis loop of ``align_pair_device`` on the pair / target ``coarseModel`` currently holds.
+    ``rewind_too_few``: a ``getCoarse`` with fewer than 4 matches returns None before RANSAC draws its samples (variant B
+    :179-180, utils/outil.py:120), so the generator state the device draw advanced is put back (the stream of the next pair
+    is then the reference's)."""
     Itw, Ith = coarseModel.target_size
     dev = coarseModel.ItTensor.device
     bg = torch.ones((Ith, Itw), device=dev) if It_bg is None else torch.as_tensor(It_bg, dtype=torch.float32, device=dev)
@@ -465,8 +473,12 @@ def align_pair_device(coarseModel, network, Is, It, maxCoarse=0, maskRegionTh=0.
     Mask = torch.zeros((Ith, Itw), device=dev)
     acc = []
     nbCoarse = ncall = 0
+    gen = None
+    if rewind_too_few and samples is None:
+        gen = coarseModel.sample_generator or torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
     while nbCoarse <= maxCoarse:
         fgMask = ((Mask + (1 - bg)) > 0.5).float()
+        state = gen.get_state() if gen is not None else None
         Hd, nb, mask, status, cnt = coarseModel.getCoarse_device(fgMask if nbCoarse > 0 or It_bg is not None else None,
                                                                  None if samples is None else samples[ncall])
         ncall += 1
@@ -479,11 +491,15 @@ def align_pair_device(coarseModel, network, Is, It, maxCoarse=0, maskRegionTh=0.
         st = int(ctl[0])
         if st == 2:
             raise TypeError("'NoneType' object is not subscriptable")     # utils/outil.py:162
+        if st == 3 and state is not None:
+            gen.set_state(state)
         if st != 0:
             break                                                          # bestPara is None (evaluation.py:215-216)
         if float(ctl[1]) > maskRegionTh or nbCoarse == 0:
             acc.append((Hd, f8, mboth, flow12, match, int(ctl[2])))
-            matchFine = match[0, 0] if nbCoarse == 0 else match[0, 0] * (1 - fgMask)
+            # evaluation.py:235 tests len(...) == 0 after the append: always masked (a no-op on the first hypothesis unless
+            # a background mask is given)
+            matchFine = match[0, 0] * (1 - fgMask)
             nbCoarse += 1
             Mask = ((Mask + matchFine) >= 1.0).float()
         else:
@@ -499,6 +515,141 @@ def align_pair_device(coarseModel, network, Is, It, maxCoarse=0, maskRegionTh=0.
                 matchDown8=host[:, 9 + n8:9 + 2 * n8].reshape(len(acc), 2, f8shape[2], f8shape[3]),
                 flow12=[a[3] for a in acc], match=[host[i, 9 + 2 * n8:].reshape(Ith, Itw) for i in range(len(acc))],
                 nbMatch=[a[5] for a in acc])
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# YFCC: four-rotation target search + re-matching hypothesis loop (evaluation/evalYFCC/evaluation.py:179-274)
+# ------------------------------------------------------------------------------------------------------------------
+YFCC_ANGLES = (0, 90, 180, 270)
+
+
+def yfcc_background(It_bg, k, size):
+    """evaluation/evalYFCC/evaluation.py:193 / :200 / :212 for rotation ``k``: the segNet map of the unrotated target (or
+    None: all ones) rotated by ``np.rot90``, resized by SciPy 1.2's ``imresize`` (byte-scaling) to ``size`` = (w, h),
+    ``< 128``.  float32 (h, w), 1 = kept (not sky)."""
+    from .dropin import imresize
+    w, h = size
+    if It_bg is None:                      # imresize of a constant map byte-scales to 0: every cell < 128
+        return np.ones((h, w), dtype=np.float32)
+    return (imresize(np.rot90(np.asarray(It_bg, dtype=np.float32), k), (h, w)) < 128).astype(np.float32)
+
+
+def rotation_draws(counts, nbPoint=4):
+    """The rotations (in the reference's order) whose ``getCoarse`` reaches ``outil.RANSAC`` and draws its samples: those
+    with at least ``nbPoint`` matches (evalYFCC/coarseAlignFeatMatch.py:179-180 returns None before the draw)."""
+    return [k for k in range(len(counts)) if int(counts[k]) >= nbPoint]
+
+
+def rotation_scores(ran, status, inliers):
+    """evaluation/evalYFCC/evaluation.py:203-206: the score of every rotation - the inlier count of RANSAC's hypothesis
+    for the rotations ``ran`` (RF_RANSAC_* ``status``), 0 where RANSAC returned None or did not run.  RF_RANSAC_NO_MODEL
+    raises where utils/outil.py:162 does."""
+    scores = [0, 0, 0, 0]
+    for k, st, n in zip(ran, status, inliers):
+        if int(st) == 2:
+            raise TypeError("'NoneType' object is not subscriptable")     # utils/outil.py:162
+        scores[k] = int(n) if int(st) == 0 else 0
+    return scores
+
+
+def align_pair_yfcc(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.01, It_bg=None, samples=None):
+    """One pair through evalYFCC's loop (evaluation/evalYFCC/evaluation.py:179-274) with a variant-B / C ``coarseModel``,
+    eager and steered from the host like ``align_pair_device``:
+
+      * rotation search (:191-212): the source pyramid and the four rotated targets through the trunk as one ragged batch,
+        the four masked re-matchings, ONE host read of the four match counts, then RANSAC in rotation order for the
+        rotations with at least 4 matches only (the reference returns None before RANSAC draws, so a seeded run consumes
+        the reference's sample stream); the score is the inlier count of the winning hypothesis (= ``np.sum(InlierMask)``:
+        mutual matches use each target cell once), 0 when RANSAC returns None; the first maximum wins;
+      * the hypothesis loop of ``align_pair_device`` on the winning rotation: masked re-matching per ``getCoarse``,
+        ``match12 * match21`` matchability (:32-62), 12 bytes per hypothesis to the host.
+
+    ``Is`` / ``It``: PIL images or uint8 (H, W, 3) CUDA tensors.  ``It_bg``: ``skyFromSeg`` of the unrotated target, or
+    None (no ``--segNet``).  ``samples``: optional injected (nbIter, 4) index tables, one per RANSAC call in the reference's
+    order.  Returns ``align_pair_device``'s dict plus ``angle``, ``nbInlierRot`` (the four scores) and ``It_bg`` (the
+    resized boolean background map the driver saves as ``maskBG_``)."""
+    with torch.no_grad():
+        coarseModel._set_rotated_pair(Is, It)
+        best, nbInlierRot, bg, calls = _rotation_search(coarseModel, It_bg, samples)
+        rest = None
+        if samples is not None:       # a last call with M < 4 draws nothing in the reference: any table serves it
+            rest = list(samples[calls:]) + [np.zeros((coarseModel.nbIter, coarseModel.nbPoint), dtype=np.int64)]
+        out = _hypotheses_device(coarseModel, network, maxCoarse, maskRegionTh, True, bg, rest, rewind_too_few=True)
+    w, h = coarseModel.target_size
+    out.update(angle=YFCC_ANGLES[best], nbInlierRot=nbInlierRot,
+               It_bg=(bg if bg is not None else np.ones((h, w), dtype=np.float32)).astype(bool))
+    return out
+
+
+def _rotation_search(c, It_bg, samples):
+    """evaluation.py:195-212 on the rotations ``_set_rotated_pair`` computed: selects the winning rotation.  Returns (its index,
+    the four scores, its background map (None without ``It_bg``), the number of RANSAC calls made)."""
+    bgs, found = [], []
+    for k in range(4):
+        c._select_target(k)
+        bg = yfcc_background(It_bg, k, c.rotated_target_size(k))
+        bgs.append(bg)
+        m1, m2, _, cnt = c._match_device(((1 - bg) > 0.5).astype(np.float32) if It_bg is not None else None)
+        found.append((m1, m2, cnt))
+    counts = _to_host(torch.cat([f[2] for f in found])).copy()               # the one read the draw decision needs
+    ran = rotation_draws(counts, c.nbPoint)
+    res = []
+    for n, k in enumerate(ran):
+        m1, m2, cnt = found[k]
+        _, _, mask, status = c._ransac_device(m1, m2, cnt, None if samples is None else samples[n])
+        res.append(torch.cat([status, mask[:int(counts[k])].sum(dtype=torch.int32).reshape(1)]))
+    res = _to_host(torch.cat(res)).copy().reshape(-1, 2) if res else np.zeros((0, 2), dtype=np.int32)
+    nbInlierRot = rotation_scores(ran, res[:, 0], res[:, 1])
+    best = int(np.argmax(nbInlierRot))                                          # np.argmax: the first maximum wins
+    c._select_target(best)
+    return best, nbInlierRot, (bgs[best] if It_bg is not None else None), len(ran)
+
+
+def align_pair_yfcc_host(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.01, It_bg=None):
+    """The drop-in path of evalYFCC: the driver's statements (evaluation/evalYFCC/evaluation.py:191-274) on the mirror
+    ``CoarseAlignB`` (``setSource`` / ``setTarget`` / ``getCoarse``, host-synchronised, RANSAC samples from
+    ``torch.randint`` on the CUDA generator) and ``PredFlowMask`` with ``match21``.  ``Is`` / ``It``: PIL images.  Same
+    dict as ``align_pair_yfcc`` (without ``nbMatch``); the yardstick its device path is tested and timed against."""
+    c = coarseModel
+    with torch.no_grad():
+        c.setSource(Is)
+        ItList = [It] + [It.rotate(a, expand=True) for a in YFCC_ANGLES[1:]]
+        nbInlier = []
+        for k in range(4):
+            c.setTarget(ItList[k])
+            bg = yfcc_background(It_bg, k, c.It.size)
+            bestPara, InlierMask = c.getCoarse(((1 - bg) > 0.5).astype(np.float32))
+            nbInlier.append(0 if bestPara is None else int(np.sum(InlierMask)))
+        best = int(np.argmax(nbInlier))
+        c.setTarget(ItList[best])
+        Itw, Ith = c.It.size
+        bg = yfcc_background(It_bg, best, (Itw, Ith))
+        featt = fine_features(network["netFeatCoarse"], c.ItTensor)
+        grid = torch.empty((1, Ith, Itw, 2), device="meta")                     # size carrier only
+        warper = HomographyWarper(Ith, Itw)
+        Mask = np.zeros((Ith, Itw), dtype=np.float32)
+        Hs, flows8, matches8, flows, matches = [], [], [], [], []
+        nbCoarse = 0
+        while nbCoarse <= maxCoarse:
+            fgMask = ((Mask + (1 - bg)) > 0.5).astype(np.float32)
+            bestPara, _ = c.getCoarse(fgMask)
+            if bestPara is None:
+                break
+            flowCoarse = warper.warp_grid(torch.from_numpy(bestPara).unsqueeze(0).cuda())
+            flowFine, matchFine, f8, m8 = PredFlowMask(c.IsTensor, featt, flowCoarse, grid, network, with_match21=True)
+            if (matchFine * (1 - fgMask)).mean() > maskRegionTh or nbCoarse == 0:
+                Hs.append(bestPara[None])
+                flows8.append(f8)
+                matches8.append(m8)
+                flows.append(flowFine)
+                matches.append(matchFine)
+                nbCoarse += 1
+                Mask = ((Mask + matchFine * (1 - fgMask)) >= 1.0).astype(np.float32)
+            else:
+                break
+    cat = lambda l: np.concatenate(l, axis=0) if l else np.zeros((0,))
+    return dict(H=cat(Hs), flowDown8=cat(flows8), matchDown8=cat(matches8), flow12=flows, match=matches, angle=YFCC_ANGLES[best],
+                nbInlierRot=nbInlier, It_bg=bg.astype(bool))
 
 
 def align2images(coarseModel, network, img1, img2, align_corners=False):

@@ -2,6 +2,7 @@
 that results written here are read by the reference's ``getResults.py`` and vice versa.
 
   save_pair / load_pair            : evaluation/evalHpatch/evaluation.py:244-260 (identical in evalCorr :244-260)
+  save_rotation                    : evaluation/evalYFCC/evaluation.py:270-271 (rotation.json, read by evalYFCC/getResults.py)
   getFlow_all_from_files           : evaluation/evalHpatch/getResults.py:16-63 (file lookup + np.load + composition)
   getFlow_from_files               : evaluation/evalCorr/getResults.py:78-134 / evalYFCC/getResults.py:132-190 (flow AND matchability)
   save_pair_kitti / kitti_pairs    : evaluation/evalKITTI/evaluation.py:43-47,338-344; evalKITTI/getResults.py:190-193
@@ -39,6 +40,17 @@ def save_pair(outCoarse, outFine, idx, out, It_bg=None):
     np.save(os.path.join(outCoarse, "flow_" + tag), np.asarray(out["H"], dtype=np.float32))
     np.save(os.path.join(outFine, "flow_" + tag), f8)
     return nH
+
+
+def save_rotation(outSceneFine, angle_rotation):
+    """evaluation/evalYFCC/evaluation.py:270-271: ``outSceneFine/rotation.json``, the json dump of {pair index: angle} (the
+    keys become strings: evalYFCC/getResults.py reads ``rotation[str(i)]``).  ``angle_rotation``: the ``angle`` of
+    ``pipeline.align_pair_yfcc`` per pair.  Returns the path."""
+    import json
+    path = os.path.join(outSceneFine, "rotation.json")
+    with open(path, "w") as f:
+        json.dump({k: int(v) for k, v in angle_rotation.items()}, f)
+    return path
 
 
 def find_nbH(pairID, flowList):

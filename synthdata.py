@@ -267,6 +267,14 @@ def make_pair(i, h=480, w=640):
     return src_n.astype(np.uint8), tgt.astype(np.uint8), H
 
 
+def make_rotated_pair(i, h=480, w=640, k=1):
+    """``make_pair(i, h, w)`` with the target rotated by 90 k degrees counter-clockwise (``np.rot90``, which is what
+    ``PIL.Image.rotate(90 k, expand=True)`` does): the rotation evalYFCC's target search must undo is 360 - 90 k.
+    Returns (source (h,w,3), rotated target ((h,w) or (w,h),3), H_t2s of the unrotated target)."""
+    src, tgt, H = make_pair(i, h, w)
+    return src, np.ascontiguousarray(np.rot90(tgt, k % 4)), H
+
+
 # --------------------------------------------------------------------------
 # match sets for kernel-level RANSAC cases (SURVEY.md section 8d)
 # --------------------------------------------------------------------------
