@@ -158,9 +158,9 @@ int rf_conv1x1_dual_split(const void* x1, const void* x2, int nimg, const int* h
 #define RF_OP_BLUR 2      /* model/downsample.py: reflect-pad 1 + [1 2 1]^2/16, stride */
 #define RF_OP_IM2COL 3    /* k x k x Cin patches (r, s, c order) zero-padded to Cout floats per output pixel: few-channel stems */
 #define RF_OP_POOLBLUR 4  /* MaxPool2d(2, stride 1) + blur stride 2 fused (model/model.py:71-72) */
-#define RF_OP_STEM7 5     /* engines 2 / 4 only: ResNet-50 stem fused (7x7 / stride 2 / pad 3 on the 3-channel fp32 image + bias + ReLU ->
-                             fp16 / split, 64 channels) without the im2col matrix; w_f16 = [64][192] ([2][64][192] for engine 4) in
-                             (r, s, c) order, zero padded */
+#define RF_OP_STEM7 5     /* engines 2 / 4 only: a direct stem on the 3-channel fp32 image + bias + ReLU -> fp16 / split, 64 channels,
+                             without the im2col matrix: k 7 / stride 2 / pad 3 (ResNet-50) or k 3 / stride 1 / pad 1 (FeatureExtractor);
+                             w_f16 = [64][Kpad] ([2][64][Kpad] for engine 4) in (r, s, c) order, zero padded to Kpad = 192 / 64 */
 #define RF_OP_CONV_DUAL 6  /* engine 4 only: rf_conv1x1_dual_split; src = x1 (Cin channels), src2 = x2 (Cin2 channels, stride2), w_f16 = [2][Cout][Cin + Cin2] */
 #define RF_OP_STEM3 7      /* engine 4 only: the first conv of segNet's deep stem (segNet/segModel.py:64,108) fused: 3x3 / stride 2 / pad 1 on the
                              3-channel fp32 input slot + bias + ReLU -> split, 64 channels, exact fp32 FMA; w = [27][64] ((r, s, c) rows) */
@@ -180,7 +180,7 @@ typedef struct rf_layer {
 } rf_layer_t;
 #define RF_LAYER_OUT_F32 1          /* conv: fp16 operands, fp32 output (RF_ENGINE_F16_OUT32; engine 4: RF_ENGINE_SPLIT_OUT32) */
 #define RF_LAYER_TF32 2             /* conv: fp32 input and output on the TF32 engine (e.g. a 49-channel head after an OUT_F32 layer) */
-#define RF_LAYER_STEM_POOL 4        /* RF_OP_STEM7 whose output only feeds the next layer, a 3x3 / stride 2 / pad 1 RF_OP_MAXPOOL: both run
+#define RF_LAYER_STEM_POOL 4        /* 7x7 RF_OP_STEM7 whose output only feeds the next layer, a 3x3 / stride 2 / pad 1 RF_OP_MAXPOOL: both run
                                        as one kernel that writes the max-pool's dst slot; the stem's own dst slot is never written */
 /* engine 2: slots hold fp16 except the input of an RF_OP_IM2COL (the fp32 image; row length = Cout % 64 == 0), the
  * output of an RF_LAYER_OUT_F32 conv and the input / output of an RF_LAYER_TF32 conv; pooling and blur run in fp16. */

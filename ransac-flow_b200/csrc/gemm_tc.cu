@@ -402,46 +402,77 @@ wg_kernel(const __grid_constant__ WgParams p) {
 
 
 // ------------------------------------------------------------------------------------------------------------
-// ResNet-50 front end, fused: conv 7x7 / stride 2 / pad 3 on the 3-channel fp32 image + folded BN + ReLU and, with pool = 1,
-// the 3x3 / stride 2 / pad 1 max-pool on its output -> fp16 (engine 2) or split (engine 4) NHWC.  No im2col matrix goes to
-// HBM, and with pool = 1 neither does the full-resolution stem output.
-// Persistent, 256 threads, 1 CTA per SM: the weights are TMA-loaded once per CTA and stay resident.  A work unit (step) is a
-// tile of 4 stem rows x 32 stem columns (128 pixels x 64 channels); units run down column strips (steps fastest) and CTA b
-// takes the contiguous range [U b / G, U (b + 1) / G) of them.  Per step:
-//   build    : two threads per pixel build its 147-long (r, s, c) patch from the staged 13 x 69 x 3 input window (split into
-//              (hi, lo) pairs once, at staging) as hi / lo planes in the 128-byte-swizzled K-major layout (3 K blocks of 64;
-//              147..191 are zeros); K block kb + 1 is built while the wgmmas of K block kb run;
-//   MMA      : warpgroup g = pixels 64g .. 64g + 63, wgmma over the three K blocks against the resident weights;
-//   prefetch : while the MMAs run, the next step's input window is loaded into registers (staged after the MMAs);
-//   epilogue : pool = 0: bias, ReLU, conversion and stores from the registers.  pool = 1: the stem values go to a shared tile
-//              (engine 4: split and rebuilt, i.e. the values the max-pool of a split tensor reads), then the step's 2 pooled
-//              rows x 15 pooled columns are reduced there and stored with 16-byte stores.
+// Direct stems: conv k x k / stride S / pad (k - 1) / 2 on the 3-channel fp32 image + folded BN + ReLU -> fp16 (engine 2) or
+// split (engine 4) NHWC, 64 channels, with no im2col matrix in HBM: the ResNet-50 stem (7, 2) - with pool = 1 fused with its
+// 3x3 / stride 2 / pad 1 max-pool, so that its full-resolution output never goes to HBM either - and the FeatureExtractor
+// stem (3, 1).
+// Persistent, 256 threads: the weights are TMA-loaded once per CTA and stay resident.  A work unit (step) is a tile of 4 stem
+// rows x 32 stem columns (128 pixels x 64 channels); units run down column strips (steps fastest) and CTA b takes the
+// contiguous range [U b / G, U (b + 1) / G) of them.  Per step:
+//   MMA      : warpgroup g = pixels 64g .. 64g + 63.  Per k16 step every thread gathers its own m64k16 A fragment (pixels
+//              rbase and rbase + 8, patch elements 16j + 2q + {0, 1, 8, 9}) from the staged input window, which holds each
+//              input value split once into an (hi, lo) fp16 pair, and issues the three split MMAs with A from registers
+//              against the resident weights.  The fragments are double-buffered: the gather of k16 step j + 1 runs while
+//              the MMAs of step j do.  Only the k16 steps that hold patch elements run (10 for K = 147, 2 for K = 27): the
+//              rest would multiply zero patch elements with the weights' zero rows;
+//   prefetch : while the MMAs run, the next step's input window is loaded into registers (staged after the MMAs, into the
+//              other of two window buffers);
+//   epilogue : bias, ReLU and conversion into a shared tile (the tiles rotate over NT buffers, so one __syncthreads per step
+//              orders every shared-memory hand-over).  pool = 0: the tile leaves with coalesced 16-byte stores.  pool = 1:
+//              the tile holds the stem values as the max-pool reads them (engine 4: split and rebuilt in fp32), and the
+//              step's 2 pooled rows x 15 pooled columns are reduced there and stored with 16-byte stores.
 // Pooling: pooled column q needs stem columns 2q - 1 .. 2q + 1, so the tiles of strip s start at stem column 30 s - 1 and
 // overlap the strip to their left by one column (1/16 of the stem is computed twice); pooled row p needs stem rows
-// 2p - 1 .. 2p + 1, so each step keeps its last stem row for the next step of the strip (two alternating tiles).  A CTA whose
-// range starts inside a strip first computes the step above, without pooling it.  As in the standalone max-pool, window
-// positions outside the stem image are skipped and the maximum runs over (r, s) in the same order.
+// 2p - 1 .. 2p + 1, so each step reads the last stem row of the step before it from that step's tile.  A CTA whose range
+// starts inside a strip first computes the step above, without pooling it.  As in the standalone max-pool, window positions
+// outside the stem image are skipped and the maximum runs over (r, s) in the same order.
+//
+// Window layout.  Element (r, s, c) of the patch of pixel (py, px) = m of the tile is window row S py + r, window column
+// ix = S px + s, channel c.  One 32-bit word per element ((hi, lo) pair, hi in the low half), rows LD words apart:
+//   S = 1: word 3 ix + c                                  [col 0 | col 1 | col 2 | ... ]
+//   S = 2: even columns first, then the odd ones:         [col 0 | col 2 | ... | col 68 | col 1 | col 3 | ... | col 67 ]
+//          word (ix % 2) * EVEN_W + 3 (ix / 2) + c
+// so that in both layouts the element sits at word 3 px + S py LD + off(r, s, c): one table of offsets per (k16 step, q)
+// serves every pixel.  In one gather instruction a warp reads 8 pixels (lanes / 4) at 3 words apart and 4 patch elements
+// (lanes % 4) 2 apart in k.  With the pixels 6 words apart (the plain stride-2 layout) the ResNet stem's gathers take up to 3
+// shared-memory wavefronts, 1.95 on average; the even / odd split brings that to at most 2, 1.28 on average (the
+// FeatureExtractor stem: at most 2, 1.5 on average).
 // ------------------------------------------------------------------------------------------------------------
-constexpr int ST_TW = 32, ST_TH = 4, ST_K = 7, ST_C = 3, ST_KK = 147, ST_KB = 3;
+constexpr int ST_TW = 32, ST_TH = 4, ST_C = 3;
 constexpr int ST_PW = (ST_TW - 2) / 2, ST_PH = ST_TH / 2;                // pooled columns per strip, pooled rows per step
-constexpr int ST_IN_W = ((ST_TW - 1) * 2 + ST_K) * ST_C;                  // 207 floats per staged input row
-constexpr int ST_IN_H = (ST_TH - 1) * 2 + ST_K;                           // 13 rows
-constexpr int ST_IN_LD = 208;
 constexpr int ST_THREADS = 256;
 constexpr int ST_B_PLANE = 64 * 128;                                      // one K block of 64 weight rows: 8 KB
-constexpr int ST_OFF_ALO = ST_KB * TC_A_BYTES;                            // 48 KB: lo planes of the patches
-constexpr int ST_OFF_B = 2 * ST_KB * TC_A_BYTES;                          // 96 KB
-constexpr int ST_OFF_T = ST_OFF_B + ST_KB * 2 * ST_B_PLANE;               // 144 KB: two stem tiles of 128 pixels x 64 fp32
-constexpr int ST_T_BYTES = 128 * 64 * 4;
-constexpr int ST_OFF_IN = ST_OFF_T + 2 * ST_T_BYTES;                      // 208 KB
-constexpr int ST_OFF_BAR = ST_OFF_IN + ST_IN_H * ST_IN_LD * 4;
-constexpr int ST_SMEM = ST_OFF_BAR + 64 + 1024;
-constexpr int ST_NLD = (ST_IN_H * ST_IN_W + ST_THREADS - 1) / ST_THREADS;  // window floats per thread
-static_assert(ST_SMEM <= 227 * 1024, "stem shared memory");
+constexpr int ST_T_BYTES = 128 * 64 * 4;                                  // one tile: 128 pixels x 64 fp32 (or 2 fp16 planes)
 static_assert(ST_PH * ST_PW * 8 <= ST_THREADS, "one thread per (pooled pixel, 8 channels) of a step");
 
+template <int KS, int S>
+struct StemGeo {
+    static constexpr int PAD = (KS - 1) / 2;
+    static constexpr int KK = KS * KS * ST_C;                             // patch length: 147 / 27
+    static constexpr int KSTEPS = (KK + 15) / 16;                         // k16 steps with patch elements: 10 / 2
+    static constexpr int KB = (KSTEPS + 3) / 4;                           // weight K blocks of 64 rows they use: 3 / 1
+    static constexpr int IN_H = (ST_TH - 1) * S + KS;                     // window rows: 13 / 6
+    static constexpr int IN_COLS = (ST_TW - 1) * S + KS;                  // window columns: 69 / 34
+    static constexpr int IN_W = IN_COLS * ST_C;                           // window floats per row
+    static constexpr int EVEN_W = (IN_COLS + 1) / 2 * ST_C;               // S = 2: words of the even columns
+    static constexpr int LD = S == 2 ? 208 : 104;
+    static constexpr int WIN = IN_H * LD;                                 // words per window buffer
+    static constexpr int NLD = (IN_H * IN_W + ST_THREADS - 1) / ST_THREADS;  // window floats per thread
+    static constexpr int NT = S == 2 ? 3 : 2;                             // tiles: pooling reads a step's and the one before
+    static constexpr int CTAS = S == 2 ? 1 : 2;                           // CTAs per SM
+    static constexpr int OFF_T = KB * 2 * ST_B_PLANE;
+    static constexpr int OFF_IN = OFF_T + NT * ST_T_BYTES;
+    static constexpr int OFF_K = OFF_IN + 2 * WIN * 4;                    // gather offsets: int4 [KSTEPS][4]
+    static constexpr int OFF_BAR = OFF_K + KSTEPS * 4 * 16;
+    static constexpr int SMEM = OFF_BAR + 64 + 1024;
+    static_assert(LD >= (S == 2 ? EVEN_W + IN_COLS / 2 * ST_C : IN_W), "window row");
+    static_assert(CTAS * SMEM <= 227 * 1024, "stem shared memory");
+    // window word of (row r, column ix, channel c)
+    static __device__ __forceinline__ int word(int r, int ix, int c) { return r * LD + (S == 2 ? (ix & 1) * EVEN_W + (ix >> 1) * ST_C : ix * ST_C) + c; }
+};
+
 struct alignas(64) StemParams {
-    CUtensorMap mapB;                     // weights (192, 64[, 2]) fp16, box (64, 64[, 2])
+    CUtensorMap mapB;                     // weights (64 KB, 64[, 2]) fp16, box (64, 64[, 2])
     int nimg, pool;
     int unit_start[RF_MAX_IMGS + 1];      // prefix sums of steps per image; [nimg ..] = all steps
     int steps[RF_MAX_IMGS];               // steps per strip
@@ -462,66 +493,66 @@ __device__ __forceinline__ uint32_t stem_pack_split(float v) {
     return (*reinterpret_cast<uint32_t*>(&hi) & 0xFFFFu) | (*reinterpret_cast<uint32_t*>(&lo) << 16);
 }
 
-// half a patch: the 16-byte chunks 4 * HALF .. 4 * HALF + 3 of K block kb of pixel m, hi (and lo) planes
-template <bool SPLIT, int HALF, int kb>
-__device__ __forceinline__ void stem_build_half(const uint32_t* __restrict__ base, uint8_t* sA, int m) {
+struct StemFrag { uint32_t h[4], l[4]; };     // the hi and lo planes of one m64k16 A fragment
+
+// k16 step j's fragment of the pixels at window words `base` and base + 24 (8 pixels to the right); off = that step's
+// offsets for this thread's q (-1: past the patch, a zero element)
+template <int KK, int j>
+__device__ __forceinline__ void stem_gather(StemFrag& f, const uint32_t* __restrict__ w, int base, const int4* sK, int q) {
+    const int4 o4 = sK[j * 4 + q];
+    const int o[4] = {o4.x, o4.y, o4.z, o4.w};
+    uint32_t v[2][4];
 #pragma unroll
-    for (int cc = 0; cc < 4; ++cc) {
-        const int c8 = HALF * 4 + cc;
-        uint4 oh, ol;
-        uint32_t* ph = reinterpret_cast<uint32_t*>(&oh);
-        uint32_t* pl = reinterpret_cast<uint32_t*>(&ol);
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int k0 = kb * 64 + c8 * 8 + 2 * e, k1 = k0 + 1;
-            const uint32_t a = k0 < ST_KK ? base[(k0 / 21) * ST_IN_LD + (k0 % 21)] : 0u;
-            const uint32_t b = k1 < ST_KK ? base[(k1 / 21) * ST_IN_LD + (k1 % 21)] : 0u;
-            ph[e] = __byte_perm(a, b, 0x5410);          // (hi(a), hi(b))
-            pl[e] = __byte_perm(a, b, 0x7632);          // (lo(a), lo(b))
+        for (int e = 0; e < 4; ++e) v[h][e] = (16 * (j + 1) <= KK || o[e] >= 0) ? w[base + 24 * h + o[e]] : 0u;
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            f.h[2 * e + h] = __byte_perm(v[h][2 * e], v[h][2 * e + 1], 0x5410);      // (hi(k), hi(k + 1))
+            f.l[2 * e + h] = __byte_perm(v[h][2 * e], v[h][2 * e + 1], 0x7632);      // (lo(k), lo(k + 1))
         }
-        uint8_t* dst = sA + kb * TC_A_BYTES + m * 128 + ((c8 ^ (m & 7)) << 4);
-        *reinterpret_cast<uint4*>(dst) = oh;
-        if constexpr (SPLIT) *reinterpret_cast<uint4*>(dst + ST_OFF_ALO) = ol;
-    }
 }
 
-// K block kb of a step: build it, hand it to the async proxy, issue its wgmmas (one commit group)
-template <bool SPLIT, int kb, int NACC>
-__device__ __forceinline__ void stem_kblock(float (&acc)[NACC][32], const uint32_t* base, uint8_t* sA, const uint8_t* sB, int m, int half,
-                                            int g, uint64_t* bar_b, bool first) {
-    constexpr int NPL = SPLIT ? 2 : 1;
-    if (half == 0) stem_build_half<SPLIT, 0, kb>(base, sA, m);
-    else stem_build_half<SPLIT, 1, kb>(base, sA, m);
-    fence_proxy_async();            // generic-proxy writes -> visible to the tensor core (async proxy)
-    __syncthreads();
-    if (kb == 0 && first) mbar_wait(bar_b, 0);
-    wg_fence();
-    const uint32_t a = smem_u32(sA + kb * TC_A_BYTES + g * (64 * 128)), b = smem_u32(sB + kb * NPL * ST_B_PLANE);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const uint64_t ah = wg_desc(a + 32 * k), bh = wg_desc(b + 32 * k);
+// k16 steps j .. KSTEPS - 1 (one commit group each), fragment of step j in buf[j & 1]
+template <int KK, int KSTEPS, bool SPLIT, int j, int NACC>
+__device__ __forceinline__ void stem_mma(float (&acc)[NACC][32], StemFrag (&buf)[2], const uint32_t* w, int base, const int4* sK, int q,
+                                         uint32_t sB) {
+    if constexpr (j < KSTEPS) {
+        constexpr int NPL = SPLIT ? 2 : 1;
+        StemFrag& f = buf[j & 1];
+        wg_fence();
+        const uint32_t b = sB + (j >> 2) * NPL * ST_B_PLANE + 32 * (j & 3);
+        const uint64_t bh = wg_desc(b);
         if constexpr (SPLIT) {
-            wgmma<false, 64>(acc[1], wg_desc(a + ST_OFF_ALO + 32 * k), bh);
-            wgmma<false, 64>(acc[1], ah, wg_desc(b + ST_B_PLANE + 32 * k));
+            wgmma_f16_n64_rs(acc[1], f.l, bh);
+            wgmma_f16_n64_rs(acc[1], f.h, wg_desc(b + ST_B_PLANE));
         }
-        wgmma<false, 64>(acc[0], ah, bh);
+        wgmma_f16_n64_rs(acc[0], f.h, bh);
+        wg_commit();
+        if constexpr (j + 1 < KSTEPS) {
+            wg_wait<1>();                           // the MMAs of step j - 1 have read buf[(j + 1) & 1]
+            stem_gather<KK, j + 1>(buf[(j + 1) & 1], w, base, sK, q);
+        }
+        stem_mma<KK, KSTEPS, SPLIT, j + 1>(acc, buf, w, base, sK, q, sB);
     }
-    wg_commit();
 }
 
-template <bool SPLIT>
-__global__ void __launch_bounds__(ST_THREADS, 1)
-stem7_kernel(const __grid_constant__ StemParams p) {
+template <int KS, int S, bool SPLIT>
+__global__ void __launch_bounds__(ST_THREADS, StemGeo<KS, S>::CTAS)
+stem_kernel(const __grid_constant__ StemParams p) {
+    using G = StemGeo<KS, S>;
     constexpr int NPL = SPLIT ? 2 : 1;
     constexpr int NACC = SPLIT ? 2 : 1;
-    constexpr int PIX_BYTES = SPLIT ? 256 : 128;    // one stem pixel in a shared tile: 64 fp32 (engine 2: fp16)
+    constexpr int PIX_BYTES = SPLIT ? 256 : 128;    // one stem pixel in a pooling tile: 64 fp32 (engine 2: fp16)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* sA = smem;
-    uint8_t* sB = smem + ST_OFF_B;
-    uint8_t* sT = smem + ST_OFF_T;
-    uint32_t* sIn = reinterpret_cast<uint32_t*>(smem + ST_OFF_IN);
-    uint64_t* bar_b = reinterpret_cast<uint64_t*>(smem + ST_OFF_BAR);
+    uint8_t* sB = smem;
+    uint8_t* sT = smem + G::OFF_T;
+    uint32_t* sIn = reinterpret_cast<uint32_t*>(smem + G::OFF_IN);
+    int4* sK = reinterpret_cast<int4*>(smem + G::OFF_K);
+    uint64_t* bar_b = reinterpret_cast<uint64_t*>(smem + G::OFF_BAR);
     const int t = threadIdx.x, warp = t >> 5, lane = t & 31, g = warp >> 2;
     const long long units = p.unit_start[RF_MAX_IMGS];
     const int u_begin = (int)(units * blockIdx.x / gridDim.x), u_end = (int)(units * (blockIdx.x + 1) / gridDim.x);
@@ -539,25 +570,25 @@ stem7_kernel(const __grid_constant__ StemParams p) {
         U.c0 = p.pool ? U.strip * 2 * ST_PW - 1 : U.strip * ST_TW;
         return U;
     };
-    float win[ST_NLD];
+    float win[G::NLD];
     auto load_window = [&](const Unit& U) {         // the zero-padded input window of a step, into registers
         const int H = p.H[U.img], WC = p.W[U.img] * ST_C;
         const float* src = p.x + p.in_pix[U.img] * ST_C;
-        const int iy0 = U.r0 * 2 - 3, col0 = (U.c0 * 2 - 3) * ST_C;
+        const int iy0 = U.r0 * S - G::PAD, col0 = (U.c0 * S - G::PAD) * ST_C;
 #pragma unroll
-        for (int i = 0; i < ST_NLD; ++i) {
+        for (int i = 0; i < G::NLD; ++i) {
             const int idx = t + i * ST_THREADS;
-            const int r = idx / ST_IN_W, jj = idx - r * ST_IN_W;
+            const int r = idx / G::IN_W, jj = idx - r * G::IN_W;
             const int iy = iy0 + r, col = col0 + jj;
-            win[i] = (idx < ST_IN_H * ST_IN_W && iy >= 0 && iy < H && col >= 0 && col < WC) ? __ldg(src + (long long)iy * WC + col) : 0.f;
+            win[i] = (idx < G::IN_H * G::IN_W && iy >= 0 && iy < H && col >= 0 && col < WC) ? __ldg(src + (long long)iy * WC + col) : 0.f;
         }
     };
-    auto stage_window = [&]() {                     // ... split once, into shared memory
+    auto stage_window = [&](uint32_t* dst) {        // ... split once, into a window buffer
 #pragma unroll
-        for (int i = 0; i < ST_NLD; ++i) {
+        for (int i = 0; i < G::NLD; ++i) {
             const int idx = t + i * ST_THREADS;
-            const int r = idx / ST_IN_W, jj = idx - r * ST_IN_W;
-            if (idx < ST_IN_H * ST_IN_W) sIn[r * ST_IN_LD + jj] = stem_pack_split(win[i]);
+            const int r = idx / G::IN_W, jj = idx - r * G::IN_W, ix = jj / ST_C;
+            if (idx < G::IN_H * G::IN_W) dst[G::word(r, ix, jj - ix * ST_C)] = stem_pack_split(win[i]);
         }
     };
 
@@ -565,11 +596,22 @@ stem7_kernel(const __grid_constant__ StemParams p) {
         mbar_init(bar_b, 1);
         fence_barrier_init();
     }
+    if (t < G::KSTEPS * 4) {                        // gather offsets of k16 step t / 4 for q = t % 4
+        const int j = t >> 2, q = t & 3;
+        int o[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int k = 16 * j + 2 * q + (e & 1) + 8 * (e >> 1);
+            const int r = k / (KS * ST_C), rs = k - r * KS * ST_C, s = rs / ST_C;
+            o[e] = k < G::KK ? G::word(r, s, rs - s * ST_C) : -1;
+        }
+        sK[t] = make_int4(o[0], o[1], o[2], o[3]);
+    }
     __syncthreads();
     if (t == 0) {
-        mbar_expect_tx(bar_b, ST_KB * NPL * ST_B_PLANE);
+        mbar_expect_tx(bar_b, G::KB * NPL * ST_B_PLANE);
 #pragma unroll
-        for (int kb = 0; kb < ST_KB; ++kb) {
+        for (int kb = 0; kb < G::KB; ++kb) {
             if constexpr (SPLIT) tma_load_3d(sB + kb * 2 * ST_B_PLANE, &p.mapB, bar_b, kb * 64, 0, 0);
             else tma_load_2d(sB + kb * ST_B_PLANE, &p.mapB, bar_b, kb * 64, 0);
         }
@@ -578,24 +620,26 @@ stem7_kernel(const __grid_constant__ StemParams p) {
     Unit U = decode(u);
     if (p.pool && U.j > 0) U = decode(--u);         // the step above the range: its last stem row, not pooled
     load_window(U);
-    stage_window();
+    stage_window(sIn);
     __syncthreads();
 
-    // this thread's pixel and patch half: element k = r*21 + s*3 + c of pixel (py, px) sits at sIn[2*py + r][6*px + (k % 21)]
-    const int m = t & 127, half = t >> 7;
-    const uint32_t* base = sIn + (2 * (m >> 5)) * ST_IN_LD + 6 * (m & 31);
-    // accumulator fragment: d[4j + 2h + e] = pixel rbase + 8h, channel 8j + cbase + e
-    const int rbase = 64 * g + 16 * (warp & 3) + (lane >> 2), cbase = 2 * (lane & 3);
-    int buf = 0;
+    // accumulator fragment: d[4j + 2h + e] = pixel rbase + 8h, channel 8j + cbase + e; A fragment: pixels rbase, rbase + 8
+    const int q = lane & 3;
+    const int rbase = 64 * g + 16 * (warp & 3) + (lane >> 2), cbase = 2 * q;
+    const int base = (rbase >> 5) * S * G::LD + 3 * (rbase & 31);
+    const uint32_t sB32 = smem_u32(sB);
+    int wb = 0, tb = 0;
     for (bool first = true; u < u_end; ++u, first = false) {
+        const uint32_t* w = sIn + wb * G::WIN;
         float acc[NACC][32];
 #pragma unroll
         for (int a = 0; a < NACC; ++a)
 #pragma unroll
             for (int i = 0; i < 32; ++i) acc[a][i] = 0.f;
-        stem_kblock<SPLIT, 0>(acc, base, sA, sB, m, half, g, bar_b, first);
-        stem_kblock<SPLIT, 1>(acc, base, sA, sB, m, half, g, bar_b, first);
-        stem_kblock<SPLIT, 2>(acc, base, sA, sB, m, half, g, bar_b, first);
+        StemFrag frag[2];
+        stem_gather<G::KK, 0>(frag[0], w, base, sK, q);
+        if (first) mbar_wait(bar_b, 0);
+        stem_mma<G::KK, G::KSTEPS, SPLIT, 0>(acc, frag, w, base, sK, q, sB32);
         const bool more = u + 1 < u_end;
         Unit N = U;
         if (more) {
@@ -607,13 +651,10 @@ stem7_kernel(const __grid_constant__ StemParams p) {
         for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
 
         const int img = U.img;
-        uint8_t* tile = sT + buf * ST_T_BYTES;
+        uint8_t* tile = sT + tb * ST_T_BYTES;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int mm = rbase + 8 * h;
-            const int oy = U.r0 + (mm >> 5), ox = U.c0 + (mm & 31);
-            __half* y = p.y + (p.out_pix[img] + (long long)oy * p.Wo[img] + ox) * 64;
-            const bool store = !p.pool && oy < p.Hs[img] && ox < p.Ws[img];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int n = 8 * j + cbase, i = 4 * j + 2 * h;
@@ -622,6 +663,8 @@ stem7_kernel(const __grid_constant__ StemParams p) {
                 if (p.bias) { v0 += __ldg(p.bias + n); v1 += __ldg(p.bias + n + 1); }
                 v0 = fmaxf(v0, 0.f);
                 v1 = fmaxf(v1, 0.f);
+                // pool = 0: pixel mm's 128-byte row per plane, 16-byte chunk j ^ (mm % 8); the lo plane 16 KB further
+                uint8_t* e = tile + mm * 128 + ((j ^ (mm & 7)) << 4) + cbase * 2;
                 if constexpr (SPLIT) {
                     __half2 hi, lo;
                     split2(v0, v1, hi, lo);
@@ -629,24 +672,33 @@ stem7_kernel(const __grid_constant__ StemParams p) {
                         const float2 fh = __half22float2(hi), fl = __half22float2(lo);
                         *reinterpret_cast<float2*>(tile + mm * PIX_BYTES + (((n >> 2) ^ (mm & 7)) << 4) + (n & 3) * 4) =
                             make_float2(fmaf(fl.x, 0.00048828125f, fh.x), fmaf(fl.y, 0.00048828125f, fh.y));
-                    } else if (store) {
-                        *reinterpret_cast<__half2*>(y + n) = hi;
-                        *reinterpret_cast<__half2*>(y + p.plane + n) = lo;
+                    } else {
+                        *reinterpret_cast<__half2*>(e) = hi;
+                        *reinterpret_cast<__half2*>(e + 128 * 128) = lo;
                     }
                 } else {
-                    if (p.pool) *reinterpret_cast<__half2*>(tile + mm * PIX_BYTES + ((j ^ (mm & 7)) << 4) + cbase * 2) = pack_sat(v0, v1);
-                    else if (store) *reinterpret_cast<__half2*>(y + n) = pack_sat(v0, v1);
+                    *reinterpret_cast<__half2*>(e) = pack_sat(v0, v1);
                 }
             }
         }
-        if (more) stage_window();
+        if (more) stage_window(sIn + (wb ^ 1) * G::WIN);
         __syncthreads();
 
-        if (p.pool && u >= u_begin && t < ST_PH * ST_PW * 8) {
+        if (!p.pool) {
+            // 16-byte chunks of the tile: plane, pixel, chunk; the pixels of a tile row are consecutive in the output
+            for (int i = t; i < NPL * 128 * 8; i += ST_THREADS) {
+                const int pl = i >> 10, mm = (i >> 3) & 127, ch = i & 7;
+                const int oy = U.r0 + (mm >> 5), ox = U.c0 + (mm & 31);
+                if (oy < p.Ho[img] && ox < p.Wo[img])
+                    *reinterpret_cast<uint4*>(p.y + pl * p.plane + (p.out_pix[img] + (long long)oy * p.Wo[img] + ox) * 64 + ch * 8) =
+                        *reinterpret_cast<const uint4*>(tile + pl * 128 * 128 + mm * 128 + ((ch ^ (mm & 7)) << 4));
+            }
+        } else if (u >= u_begin && t < ST_PH * ST_PW * 8) {
             // pooled pixel (oy, ox), channels 8 oct .. 8 oct + 7: stem rows 2 oy - 1 .. 2 oy + 1 are tile rows 2 pr - 1 .. 2 pr + 1
-            // (row -1: the previous step's last row, in the other tile), stem columns 2 ox - 1 .. 2 ox + 1 are tile columns 2 pc ..
-            const int oct = t & 7, q = t >> 3, pr = q / ST_PW, pc = q - pr * ST_PW;
+            // (row -1: the previous step's last row, in its tile), stem columns 2 ox - 1 .. 2 ox + 1 are tile columns 2 pc ..
+            const int oct = t & 7, qq = t >> 3, pr = qq / ST_PW, pc = qq - pr * ST_PW;
             const int oy = U.j * ST_PH + pr, ox = U.strip * ST_PW + pc;
+            const uint8_t* prev = sT + (tb == 0 ? G::NT - 1 : tb - 1) * ST_T_BYTES;
             if (oy < p.Ho[img] && ox < p.Wo[img]) {
                 float mx[8];
 #pragma unroll
@@ -657,7 +709,7 @@ stem7_kernel(const __grid_constant__ StemParams p) {
                 for (int r = 0; r < 3; ++r) {
                     const int tr = 2 * pr - 1 + r;
                     if (U.r0 + tr < 0 || U.r0 + tr >= p.Hs[img]) continue;
-                    const uint8_t* trow = tr < 0 ? sT + (buf ^ 1) * ST_T_BYTES + 3 * 32 * PIX_BYTES : tile + tr * 32 * PIX_BYTES;
+                    const uint8_t* trow = tr < 0 ? prev + 3 * 32 * PIX_BYTES : tile + tr * 32 * PIX_BYTES;
 #pragma unroll
                     for (int s = 0; s < 3; ++s) {
                         const int tc = 2 * pc + s;
@@ -688,7 +740,8 @@ stem7_kernel(const __grid_constant__ StemParams p) {
                 }
             }
         }
-        buf ^= 1;
+        wb ^= 1;
+        tb = tb + 1 == G::NT ? 0 : tb + 1;
         U = N;
     }
 }
@@ -923,12 +976,13 @@ static int conv_impl(const ImgSet& batch, const ConvParams& cp, const void* w, c
     return out32 ? launch_conv<K_SPLIT, O_F32>(p, BN, st) : launch_conv<K_SPLIT, O_SPLIT>(p, BN, st);
 }
 
-template <bool SPLIT>
+template <int KS, int S, bool SPLIT>
 static int stem_impl(const float* x, int nimg, const int* hw_host, const void* w, const float* bias, void* y, int pool, void* stream) {
-    RF_REQUIRE(x != nullptr && w != nullptr && y != nullptr, "rf_stem7: null pointer");
-    RF_REQUIRE(((uintptr_t)y % 16) == 0 && ((uintptr_t)w % 16) == 0, "rf_stem7: pointers must be 16-byte aligned");
+    using G = StemGeo<KS, S>;
+    RF_REQUIRE(x != nullptr && w != nullptr && y != nullptr, "rf_stem: null pointer");
+    RF_REQUIRE(((uintptr_t)y % 16) == 0 && ((uintptr_t)w % 16) == 0, "rf_stem: pointers must be 16-byte aligned");
     ImgSet set;
-    RF_REQUIRE(make_imgset(set, nimg, hw_host, 7, 2, 3) == 0, "rf_stem7: bad image set");
+    RF_REQUIRE(make_imgset(set, nimg, hw_host, KS, S, G::PAD) == 0, "rf_stem: bad image set");
     StemParams p;
     memset(&p, 0, sizeof(p));
     p.nimg = nimg;
@@ -948,18 +1002,19 @@ static int stem_impl(const float* x, int nimg, const int* hw_host, const void* w
         out += (long long)Ho * Wo;
     }
     for (int i = nimg; i <= RF_MAX_IMGS; ++i) p.unit_start[i] = units;
-    int rc = SPLIT ? get_map(&p.mapB, w, 192ull, 64ull, 2, 64, 64, 2, 1, 2) : get_map(&p.mapB, w, 192ull, 64ull, 0, 64, 64, 0, 1, 2);
+    constexpr unsigned long long K = G::KB * 64ull;             // the packed weights' row length: 192 / 64
+    int rc = SPLIT ? get_map(&p.mapB, w, K, 64ull, 2, 64, 64, 2, 1, 2) : get_map(&p.mapB, w, K, 64ull, 0, 64, 64, 0, 1, 2);
     if (rc) return rc;
     p.plane = out * 64;
     p.x = x; p.bias = bias; p.y = static_cast<__half*>(y);
     static bool attr[64] = {false};
     const int dev = current_device();
     if (!attr[dev]) {
-        RF_CUDA(cudaFuncSetAttribute(stem7_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM));
+        RF_CUDA(cudaFuncSetAttribute(stem_kernel<KS, S, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM));
         attr[dev] = true;
     }
-    const int grid = units < num_sms() ? units : num_sms();
-    stem7_kernel<SPLIT><<<grid, ST_THREADS, ST_SMEM, as_stream(stream)>>>(p);
+    const int resident = G::CTAS * num_sms();
+    stem_kernel<KS, S, SPLIT><<<units < resident ? units : resident, ST_THREADS, G::SMEM, as_stream(stream)>>>(p);
     RF_LAUNCHED();
     return 0;
 }
@@ -1028,10 +1083,17 @@ extern "C" int rf_conv1x1_dual_split(const void* x1, const void* x2, int nimg, c
     return conv_impl(set, p, w_split, as_stream(stream), K_SPLIT, false, &dual);
 }
 
-// fused ResNet-50 stem (pool: and its 3x3 / stride 2 / pad 1 max-pool).  x fp32 [sum HW][3], bias fp32 [64]; fp16 (engine 2):
-// w [64][192] ((r, s, c) order, zero padded), y fp16 [sum HoWo][64]; split (engine 4): w [2][64][192], y split [2][sum HoWo][64]
-int rf_stem7(ActFormat f, const float* x, int nimg, const int* hw_host, const void* w, const float* bias, int pool, void* y, void* stream) {
-    return f == ACT_SPLIT ? stem_impl<true>(x, nimg, hw_host, w, bias, y, pool, stream) : stem_impl<false>(x, nimg, hw_host, w, bias, y, pool, stream);
+// direct stems, 3 -> 64 channels + bias + ReLU: the ResNet-50 stem (k 7, stride 2, pad 3; pool: and its 3x3 / stride 2 / pad 1
+// max-pool) and the FeatureExtractor stem (k 3, stride 1, pad 1).  x fp32 [sum HW][3], bias fp32 [64]; fp16 (engine 2):
+// w [64][Kpad] ((r, s, c) order, zero padded to Kpad = 192 / 64), y fp16 [sum HoWo][64]; split (engine 4): w [2][64][Kpad],
+// y split [2][sum HoWo][64]
+int rf_stem(ActFormat f, const float* x, int nimg, const int* hw_host, int k, int stride, const void* w, const float* bias, int pool, void* y,
+            void* stream) {
+    const bool split = f == ACT_SPLIT;
+    if (k == 7 && stride == 2)
+        return split ? stem_impl<7, 2, true>(x, nimg, hw_host, w, bias, y, pool, stream) : stem_impl<7, 2, false>(x, nimg, hw_host, w, bias, y, pool, stream);
+    RF_REQUIRE(k == 3 && stride == 1 && !pool, "rf_stem: the 7x7 / stride 2 stem (optionally pooled) or the 3x3 / stride 1 stem");
+    return split ? stem_impl<3, 1, true>(x, nimg, hw_host, w, bias, y, 0, stream) : stem_impl<3, 1, false>(x, nimg, hw_host, w, bias, y, 0, stream);
 }
 
 size_t rf_corr_tc_workspace(int NA, int NB, int C) { return 2ull * ((size_t)NA + NB) * C * sizeof(float) + 1024; }

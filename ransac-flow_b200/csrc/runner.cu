@@ -9,7 +9,8 @@ int rf_maxpool(ActFormat f, const void* x, int nimg, const int* hw_host, int C, 
 int rf_blur(ActFormat f, const void* x, int nimg, const int* hw_host, int C, int stride, void* y, void* stream);
 int rf_poolblur(ActFormat f, const void* x, int nimg, const int* hw_host, int C, void* y, void* stream);
 int rf_im2col(ActFormat f, const float* x, int nimg, const int* hw_host, int C, int k, int stride, int pad, int Kpad, void* y, void* stream);
-int rf_stem7(ActFormat f, const float* x, int nimg, const int* hw_host, const void* w, const float* bias, int pool, void* y, void* stream);
+int rf_stem(ActFormat f, const float* x, int nimg, const int* hw_host, int k, int stride, const void* w, const float* bias, int pool, void* y,
+            void* stream);
 int rf_stem3(const float* x, int nimg, const int* hw_host, const float* w, const float* bias, void* y, void* stream);
 int rf_conv2d_nhwc_dil(const float* x, int nimg, const int* hw_host, int Cin, const float* w, const float* w_tc, const float* bias,
                        const float* residual, int Cout, int R, int S, int stride, int pad, int dil, int relu, int engine, float* y, void* stream);
@@ -62,14 +63,15 @@ extern "C" int rf_run_layers(const rf_layer_t* L, int n, void* const* slots, int
             break;
         case RF_OP_STEM7: {
             RF_REQUIRE(f == ACT_F16 || f == ACT_SPLIT, "rf_run_layers: RF_OP_STEM7 needs engine 2 or 4");
-            RF_REQUIRE(l.src == L[0].src && l.Cin == 3 && l.Cout == 64 && k == 7 && stride == 2 && pad == 3 && l.relu,
-                       "rf_run_layers: RF_OP_STEM7 is the ResNet-50 stem on the fp32 input slot");
+            RF_REQUIRE(l.src == L[0].src && l.Cin == 3 && l.Cout == 64 && ((k == 7 && stride == 2 && pad == 3) || (k == 3 && stride == 1 && pad == 1)) && l.relu,
+                       "rf_run_layers: RF_OP_STEM7 is the ResNet-50 stem (7x7 / 2 / pad 3) or the FeatureExtractor stem (3x3 / 1 / pad 1) on the fp32 input slot");
             const bool pool = (l.flags & RF_LAYER_STEM_POOL) != 0;
+            RF_REQUIRE(!pool || k == 7, "rf_run_layers: RF_LAYER_STEM_POOL pools the 7x7 stem");
             const rf_layer_t* mp = pool && li + 1 < n ? &L[li + 1] : nullptr;
             RF_REQUIRE(!pool || (mp != nullptr && mp->op == RF_OP_MAXPOOL && mp->src == l.dst && mp->Cin == 64 && mp->k == 3 && mp->stride == 2 &&
                                  mp->pad == 1 && mp->dst >= 0 && mp->dst < RF_MAX_SLOTS && mp->dst != l.src),
                        "rf_run_layers: RF_LAYER_STEM_POOL needs the next layer to be a 3x3 / stride 2 / pad 1 max-pool of the stem's output");
-            rc = rf_stem7(f, x, nimg, shw, l.w_f16, l.bias, pool, pool ? slots[mp->dst] : y, stream);
+            rc = rf_stem(f, x, nimg, shw, k, stride, l.w_f16, l.bias, pool, pool ? slots[mp->dst] : y, stream);
             if (rc) return rc;
             if (pool) {         // the stem's own slot is never written: the pair's output is the max-pool's
                 for (int i = 0; i < nimg; ++i)

@@ -202,7 +202,10 @@ class FeatureExtractor(_Engine):
     def _fold_build(self, f16=False):
         """The whole network as one layer program (model/model.py:106-114 do_forward)."""
         P = LayerProgram(3)
-        x = P.stem(0, self.conv1.weight, self.bn1, 1, 1, 64 if f16 else 32)          # conv1 + bn1 + relu (im2col + 1x1; 64-wide rows for fp16 / split)
+        if f16:
+            x = P.stem7_fused(0, self.conv1.weight, self.bn1)                        # conv1 + bn1 + relu, patches gathered on chip
+        else:
+            x = P.stem(0, self.conv1.weight, self.bn1, 1, 1)                         # conv1 + bn1 + relu as im2col + 1x1
         x = P.poolblur(x)                                                            # MaxPool2d(2, 1) + anti-aliased stride 2, fused
         for layer in (self.layer1, self.layer2, self.layer3):
             for b in layer:

@@ -101,16 +101,19 @@ class LayerProgram:
         return self.conv(x, FoldedConv(w, bn, 1, pad=0, device=dev), relu=True)
 
     def stem7_fused(self, src, weight, bn):
-        """fp16 engine only: the ResNet-50 stem (7x7 / 2 / pad 3, 3 -> 64, BN, ReLU) in one kernel that builds the patches
-        in shared memory (no im2col matrix in HBM).  Same packed weights as ``stem(kalign=64)``."""
+        """fp16 / split engines only: a 3 -> 64 stem conv + BN + ReLU in one kernel that gathers its patches from the fp32 image
+        staged in shared memory (no im2col matrix in HBM): the ResNet-50 stem (7 x 7 / 2 / pad 3) or the FeatureExtractor stem
+        (3 x 3 / 1 / pad 1), by the weight's size.  Same packed weights as ``stem(kalign=64)``."""
         from .model import FoldedConv
         cout, cin, k, _ = weight.shape
-        assert (cout, cin, k) == (64, 3, 7) and self.chan[src] == 3
+        assert (cout, cin) == (64, 3) and k in (7, 3) and self.chan[src] == 3
+        stride, pad = (2, 3) if k == 7 else (1, 1)
+        kpad = (k * k * cin + 63) // 64 * 64
         dev = self.device or weight.device
         w = weight.detach().float().cpu().permute(0, 2, 3, 1).reshape(cout, k * k * cin)
-        w = torch.nn.functional.pad(w, (0, 192 - k * k * cin)).reshape(cout, 192, 1, 1)
+        w = torch.nn.functional.pad(w, (0, kpad - k * k * cin)).reshape(cout, kpad, 1, 1)
         fc = FoldedConv(w, bn, 1, pad=0, device=dev)
-        self.ops.append((RF_OP_STEM7, src, -1, 3, 64, 7, 2, 3, 1, fc))
+        self.ops.append((RF_OP_STEM7, src, -1, 3, 64, k, stride, pad, 1, fc))
         self._keep.append(fc)
         self.chan.append(64)
         self.f16_only = True
@@ -168,7 +171,7 @@ class LayerProgram:
         stem_pool = set()
         for i, o in enumerate(self.ops[:-1]):
             q = self.ops[i + 1]
-            if (f16 or split) and o[0] == RF_OP_STEM7 and q[0] == RF_OP_MAXPOOL and q[1] == i + 1 and tuple(q[5:8]) == (3, 2, 1) \
+            if (f16 or split) and o[0] == RF_OP_STEM7 and o[5] == 7 and q[0] == RF_OP_MAXPOOL and q[1] == i + 1 and tuple(q[5:8]) == (3, 2, 1) \
                     and last_use[i + 1] == i + 1:
                 stem_pool.add(i)
                 elems[i + 1] = 0

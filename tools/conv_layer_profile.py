@@ -6,9 +6,10 @@
 One eager pair (bench.py's weights, synthdata pair 0, 480x640) records every layer program it runs and the input it runs
 on: the ResNet-50 trunk on the 8-image ragged batch (7 pyramid scales + the target), the FeatureExtractor, NetFlowCoarse and
 NetMatchability.  Each program is then warmed up and run N times under torch.profiler with CUDA activities; every op of a
-program is exactly one kernel launch, except a stem fused with the max-pool after it (RF_LAYER_STEM_POOL): one kernel for the
-two ops, timed on the stem row, with the max-pool row marked fused and the pair's own floor (the image in, the pooled output
-out) printed beside it.  The kernels zip with `program.ops` in launch order.
+program is exactly one kernel launch - the direct stems (`stem7`: the trunk's 7x7 / 2 and the FeatureExtractor's 3x3 / 1, the
+fp32 image in, the stem output out) included - except a stem fused with the max-pool after it (RF_LAYER_STEM_POOL): one
+kernel for the two ops, timed on the stem row, with the max-pool row marked fused and the pair's own floor (the image in, the
+pooled output out) printed beside it.  The kernels zip with `program.ops` in launch order.
 
 Per layer: kernel, shape, tiles x N tiles, K blocks (KI), median time, algorithmic GFLOP and the executed TFLOP/s (3 MMAs per
 MAC on the split engine), algorithmic HBM bytes and GB/s, and which data-sheet floor bounds the layer and what share of it
@@ -97,7 +98,7 @@ def layer_model(ops, hw, dual=None, out_f32=()):
             tiles = pixel_tiles(ohw, flat)
             t_flop = MMAS_PER_MAC * flop / (PEAK_TFLOPS * 1e12)
             t_byte = nbytes / (PEAK_GBS * 1e9)
-            r.update(K=K, KI=(K // 64) if op != OP_STEM7 else 3, tiles=tiles, ntiles=(cout + bn - 1) // bn, bn=bn, residual=res is not None and res >= 0,
+            r.update(K=K, KI=(K + 63) // 64, tiles=tiles, ntiles=(cout + bn - 1) // bn, bn=bn, residual=res is not None and res >= 0,
                      gflop=flop / 1e9, bytes=nbytes, floor_ms=1e3 * max(t_flop, t_byte), bound="tensor" if t_flop >= t_byte else "hbm")
         rows.append(r)
     return rows
