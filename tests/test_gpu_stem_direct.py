@@ -2,14 +2,17 @@
 and the FeatureExtractor stem (3x3 / 1 / pad 1) in one kernel that gathers each thread's wgmma A fragments from the staged
 input window.  It issues the same three split MMAs per k16 step on the same operand values as the kernels before it (the
 ResNet stem's patch tile in shared memory; for the FeatureExtractor, im2col + a 1x1 convolution) and skips only k16 steps
-whose products are all zero, so every output keeps the bits of those kernels: SHA-256 digests recorded with them."""
+whose products are all zero, so every output keeps the bits of those kernels: SHA-256 digests recorded with them.  A digest
+says that bits changed, not that they are wrong: the numerical reference of both stems is tests/test_gpu_stem_geometry.py, and
+the digests are re-recorded after a deliberate change of arithmetic only once that file passes."""
 import hashlib
 import importlib.util
 import os
 
-import numpy as np
 import pytest
 import torch
+
+from stem_ref import stem_args
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -25,18 +28,6 @@ def _profile_tool():
     return mod
 
 
-def _stem_args(seed, k):
-    g = torch.Generator().manual_seed(seed)
-    weight = torch.randn(64, 3, k, k, generator=g) / np.sqrt(3 * k * k)
-    bn = torch.nn.BatchNorm2d(64).eval()
-    with torch.no_grad():
-        bn.weight.copy_(torch.rand(64, generator=g) + 0.5)
-        bn.bias.copy_(torch.randn(64, generator=g) * 0.3)
-        bn.running_mean.copy_(torch.randn(64, generator=g) * 0.2)
-        bn.running_var.copy_(torch.rand(64, generator=g) + 0.5)
-    return weight, bn
-
-
 def _images(sizes, seed):
     g = torch.Generator().manual_seed(seed)
     return torch.cat([torch.randn(h * w, 3, generator=g) for h, w in sizes]).cuda()
@@ -50,14 +41,14 @@ def _digest(y):
 def resnet_stem_pool(seed=1):
     from ransac_flow_b200.program import LayerProgram
     P = LayerProgram(3, device="cuda")
-    P.maxpool(P.stem7_fused(0, *_stem_args(seed, 7)), 3, 2, 1)
+    P.maxpool(P.stem7_fused(0, *stem_args(seed, 7)), 3, 2, 1)
     return P
 
 
 def fe_stem(seed=3):
     from ransac_flow_b200.program import LayerProgram
     P = LayerProgram(3, device="cuda")
-    P.stem7_fused(0, *_stem_args(seed, 3))
+    P.stem7_fused(0, *stem_args(seed, 3))
     return P
 
 

@@ -8,6 +8,8 @@ import numpy as np
 import pytest
 import torch
 
+from stem_ref import stem_args
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -18,22 +20,10 @@ def _profile_tool():
     return mod
 
 
-def _stem_args(seed):
-    g = torch.Generator().manual_seed(seed)
-    weight = torch.randn(64, 3, 7, 7, generator=g) / np.sqrt(147)
-    bn = torch.nn.BatchNorm2d(64).eval()
-    with torch.no_grad():
-        bn.weight.copy_(torch.rand(64, generator=g) + 0.5)
-        bn.bias.copy_(torch.randn(64, generator=g) * 0.3)
-        bn.running_mean.copy_(torch.randn(64, generator=g) * 0.2)
-        bn.running_var.copy_(torch.rand(64, generator=g) + 0.5)
-    return weight, bn
-
-
 def _programs(seed, device="cuda"):
     """(fused stem + max-pool, stem only, max-pool only) with the same weights."""
     from ransac_flow_b200.program import LayerProgram
-    weight, bn = _stem_args(seed)
+    weight, bn = stem_args(seed, 7)
     fused = LayerProgram(3, device=device)
     fused.maxpool(fused.stem7_fused(0, weight, bn), 3, 2, 1)
     stem = LayerProgram(3, device=device)

@@ -7,51 +7,13 @@ import numpy as np
 import pytest
 import torch
 
+import stem_ref as S
 import wgmma_ref as R
 
 pytestmark = pytest.mark.gpu
 
 
 # ------------------------------------------------------------------ stem (RF_OP_STEM7) on engines 2 and 4
-def stem_program(rf, seed):
-    from ransac_flow_b200.program import LayerProgram
-    g = torch.Generator().manual_seed(seed)
-    weight = torch.randn(64, 3, 7, 7, generator=g) / np.sqrt(147)
-    bn = torch.nn.BatchNorm2d(64).eval()
-    with torch.no_grad():
-        bn.weight.copy_(torch.rand(64, generator=g) + 0.5)
-        bn.bias.copy_(torch.randn(64, generator=g) * 0.3)
-        bn.running_mean.copy_(torch.randn(64, generator=g) * 0.2)
-        bn.running_var.copy_(torch.rand(64, generator=g) + 0.5)
-    P = LayerProgram(3, device="cuda")
-    P.stem7_fused(0, weight, bn)
-    return P, P.ops[0][9]
-
-
-def stem_run(rf, P, xs, engine):
-    """Runs the stem program twice, the second time into its output buffer filled with NaN; returns that output (a view)."""
-    x = rf.ops.Ragged(R.nhwc(xs).cuda(), [(t.shape[2], t.shape[3]) for t in xs])
-    out, ohw = P.run(x, engine)
-    out.fill_(float("nan"))
-    out, ohw = P.run(x, engine)
-    torch.cuda.synchronize()
-    return out, ohw
-
-
-def stem_check(rf, P, fc, xs, engine, out, ohw, what):
-    kind = "split" if engine == 4 else "f16"
-    _, xq = R.operand(R.nhwc(xs), kind)
-    w = R.from_split(fc.w_split) if engine == 4 else fc.w_f16.double()
-    wq = w[:, :147].reshape(64, 7, 7, 3).permute(0, 3, 1, 2).cuda()
-    got = R.images(R.from_split(out) if engine == 4 else out.double(), ohw)
-    worst = 0.0
-    for i, xi in enumerate(R.images(xq.cuda(), [(t.shape[2], t.shape[3]) for t in xs])):
-        ref, absref = R.conv_ref(xi, wq, fc.bias, None, 2, 3, relu=True)
-        worst = max(worst, R.check(got[i], ref, absref, R.R_SPLIT if engine == 4 else R.R_F16, R.ACC[kind], R.ATOL[kind],
-                                   "%s image %d" % (what, i)))
-    return worst
-
-
 STEM_SIZES = [[(1, 1)], [(1, 45)], [(38, 1)], [(17, 35), (3, 5), (9, 33)], [(480, 640)],
               [(5 + 9 * i, 7 + 13 * i) for i in range(16)]]
 
@@ -62,27 +24,27 @@ def test_stem7_layer_vs_fp64(rf, engine, sizes):
     """7x7 / stride 2 / pad 3 + folded BN + ReLU of the fused stem against fp64 of its operands (fp16 / split input and
     weights): split-grade on engine 4, fp16 rounding on engine 2.  Sizes: single pixels and rows / columns, outputs that are
     not multiples of the 16 x 8 tile, the 480 x 640 pair size and a sixteen-image batch."""
-    P, fc = stem_program(rf, 7)
+    P, fc = S.stem_program(*S.stem_args(7, 7))
     g = torch.Generator().manual_seed(len(sizes) * 31 + sizes[0][1])
     xs = [torch.randn(1, 3, h, w, generator=g) for h, w in sizes]
-    out, ohw = stem_run(rf, P, xs, engine)
-    worst = stem_check(rf, P, fc, xs, engine, out, ohw, "stem engine %d" % engine)
+    out, ohw = S.run_nan(rf, P, xs, engine)
+    worst = S.check_stem(fc, 7, xs, engine, out, ohw, "stem engine %d" % engine)
     print("stem engine %d %s: worst error / allowance %.3g" % (engine, sizes[:2], worst))
 
 
 @pytest.mark.parametrize("engine", [2, 4])
 def test_stem7_sixteen_images_equal_images_alone(rf, engine):
-    P, _ = stem_program(rf, 8)
+    P, _ = S.stem_program(*S.stem_args(8, 7))
     g = torch.Generator().manual_seed(3)
     sizes = STEM_SIZES[-1]
     xs = [torch.randn(1, 3, h, w, generator=g) for h, w in sizes]
-    batch, ohw = stem_run(rf, P, xs, engine)
+    batch, ohw = S.run_nan(rf, P, xs, engine)
     batch = batch.clone()
-    again, _ = stem_run(rf, P, xs, engine)
+    again, _ = S.run_nan(rf, P, xs, engine)
     assert torch.equal(batch.view(torch.int16), again.view(torch.int16))
     o = np.cumsum([0] + [h * w for h, w in ohw])
     for i in range(16):
-        alone, _ = stem_run(rf, P, [xs[i]], engine)
+        alone, _ = S.run_nan(rf, P, [xs[i]], engine)
         part = batch[:, o[i]:o[i + 1]] if engine == 4 else batch[o[i]:o[i + 1]]
         assert torch.equal(part.view(torch.int16), alone.view(torch.int16)), i
     with pytest.raises(rf._lib.RFError):
