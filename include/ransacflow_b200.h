@@ -297,6 +297,59 @@ size_t rf_fill_nearest_matched_workspace(int H, int W);
 int rf_fill_nearest_matched(const float* flow, const uint8_t* matched, int H, int W, float* flow_out, int* index_out,
                             void* ws, size_t ws_bytes, void* stream);
 
+/* -------------------------------------------------------------- YFCC pose --
+ * The relative-pose metric of evaluation/evalYFCC/getResults.py:53-111 (matches_from_flow, norm_kp, opencv_decompose) in
+ * fp64 on the device.  The point count stays on the device; the three calls share one record the host reads at the end. */
+#define RF_POSE_OK 0          /* E (and, after rf_recover_pose, R / t) valid                                     */
+#define RF_POSE_TOO_FEW 1     /* fewer than 5 matches: the driver's pts1.shape[0] >= 5 test fails (no model)     */
+#define RF_POSE_NO_MODEL 2    /* findEssentialMat finds no E with 5 or more inliers                             */
+#define RF_POSE_NO_POSE 3     /* every recoverPose count is 0: the driver's loop keeps no (R, t)                 */
+typedef struct rf_pose_record {
+    int status;                     /* RF_POSE_* */
+    int n_points;                   /* N */
+    int niters;                     /* RANSAC iteration budget at the end (RANSACUpdateNumIters) */
+    int best_iter, best_cand;       /* (iteration, candidate) of the best E; -1 when none */
+    int ransac_count;               /* its inlier count */
+    int n_E;                        /* stacked candidates in E: 1, or every solution of the single minimal problem when N == 5 */
+    int pose_count;                 /* the driver's num_inlier */
+    int pose_cand, pose_index;      /* the winning candidate and its pose (0..3: (R1, t), (R2, t), (R1, -t), (R2, -t)) */
+    int pose_counts[40];            /* [candidate][pose] cheirality counts */
+    double E[90];                   /* [n_E][3][3] row-major, unit Frobenius norm */
+    double poses[480];              /* [candidate][pose][3][4] = [R | t] of decomposeEssentialMat */
+    double R[9], t[3];
+} rf_pose_record_t;
+/* matches_from_flow (:53-71) + norm_kp (:29-50): flow [H][W][2] fp32 (flowGlobal), mask [H][W] u8 (non-zero = matched), the target
+ * grid np.rot90(meshgrid(arange(wB), arange(hB)), k) (H x W after the rotation, else an error), (wA, hA) the source size,
+ * norm1_host / norm2_host = (cx, cy, fx, fy) of each image.  pts1 = ((f + 1) * (wA - 1) / 2 in fp32 - c) / f_ in fp64,
+ * pts2 = (grid - c) / f_ in fp64, [H*W][2] capacity, in numpy's boolean-index (row-major) order; the count goes to *N_out. */
+size_t rf_yfcc_matches_workspace(int H, int W);
+int rf_yfcc_matches(const float* flow, const uint8_t* mask, int H, int W, int k, int wB, int hB, int wA, int hA,
+                    const double* norm1_host, const double* norm2_host, double* pts1_out, double* pts2_out, int* N_out,
+                    void* ws, size_t ws_bytes, void* stream);
+/* cv2.findEssentialMat(pts1, pts2, method=RANSAC, threshold) (focal 1, pp (0, 0), prob 0.999, maxIters 1000): cv::RNG((uint64)-1)
+ * subsets, every real five-point solution of each (ascending root), OpenCV's Sampson error cast to fp32 against (float)(t * t),
+ * and RANSACPointSetRegistrator::run's sequential best / iteration-budget update, scored 64 iterations per launch (a launch past
+ * the budget exits at once: a fixed launch sequence, graph-capturable).  pts [capacity][2], N = *N_dev <= capacity.
+ * Writes rec (status, E, counts) and mask_out[N] (the best E's inliers; all ones when N == 5). */
+size_t rf_essential_ransac_workspace(int capacity);
+int rf_essential_ransac(const double* pts1, const double* pts2, int capacity, const int* N_dev, double threshold,
+                        rf_pose_record_t* rec, uint8_t* mask_out, void* ws, size_t ws_bytes, void* stream);
+/* cv2.recoverPose(E, pts1, pts2, mask=mask_in) for each stacked E of rec (distance threshold 50), with the driver's loop
+ * (:96-104): cv2 writes each call's mask into mask_in, so candidate c + 1 starts from candidate c's output, and the first
+ * candidate with the strictly largest count wins.  Writes rec (R, t, pose_count, status) and mask_out[N] (the winner's mask).
+ * The first 8 * capacity bytes of ws hold the per-point cheirality bits: bit 4 c + p = pose p of candidate c passes. */
+size_t rf_recover_pose_workspace(int capacity);
+int rf_recover_pose(const double* pts1, const double* pts2, int capacity, const uint8_t* mask_in, rf_pose_record_t* rec,
+                    uint8_t* mask_out, void* ws, size_t ws_bytes, void* stream);
+/* The stages of rf_essential_ransac alone (for tests): the [1000][5] int32 subset table of N = *N_dev points; the five-point
+ * solutions E_out [nsamples][10][9] / nsol_out [nsamples] of the subsets idx [nsamples][5]; the Sampson inlier counts of nmodels
+ * (<= 640) models E [nmodels][9] over N points, with the fp32 errors in err_out [nmodels][N] (nullable). */
+int rf_essential_samples(const int* N_dev, int* idx_out, void* stream);
+int rf_essential_five_point(const double* pts1, const double* pts2, const int* idx, int nsamples, double* E_out, int* nsol_out,
+                            void* stream);
+int rf_essential_score(const double* pts1, const double* pts2, int N, const double* E, int nmodels, double threshold,
+                       int* counts_out, float* err_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

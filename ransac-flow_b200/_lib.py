@@ -58,6 +58,15 @@ SIGNATURES = {
     "rf_fill_nearest_matched": (i32, [vp, vp, i32, i32, vp, vp, vp, sz, vp]),
     "rf_remove_small_cc_workspace": (sz, [i32, i32]),
     "rf_remove_small_cc": (i32, [vp, i32, i32, i32, f32, C.c_double, vp, sz, vp]),
+    "rf_yfcc_matches_workspace": (sz, [i32, i32]),
+    "rf_yfcc_matches": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, sz, vp]),
+    "rf_essential_ransac_workspace": (sz, [i32]),
+    "rf_essential_ransac": (i32, [vp, vp, i32, vp, C.c_double, vp, vp, vp, sz, vp]),
+    "rf_recover_pose_workspace": (sz, [i32]),
+    "rf_recover_pose": (i32, [vp, vp, i32, vp, vp, vp, vp, sz, vp]),
+    "rf_essential_samples": (i32, [vp, vp, vp]),
+    "rf_essential_five_point": (i32, [vp, vp, vp, i32, vp, vp, vp]),
+    "rf_essential_score": (i32, [vp, vp, i32, vp, i32, C.c_double, vp, vp, vp]),
 }
 
 

@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libransacflow_b200.so")
-SOURCES = ["api.cu", "ransac.cu", "gemm_simt.cu", "gemm_tc.cu", "elementwise.cu", "runner.cu"]
+SOURCES = ["api.cu", "ransac.cu", "pose.cu", "gemm_simt.cu", "gemm_tc.cu", "elementwise.cu", "runner.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -325,6 +325,125 @@ def build_matches(idx1, idx2, count, W1, H1, W2, H2, valid16=None):
     return m1, m2, kept, cnt
 
 
+# --------------------------------------------------------------------------- YFCC pose
+POSE_OK, POSE_TOO_FEW, POSE_NO_MODEL, POSE_NO_POSE = 0, 1, 2, 3
+
+
+class PoseRecord(C.Structure):
+    """Mirror of rf_pose_record_t (include/ransacflow_b200.h)."""
+    _fields_ = [("status", C.c_int), ("n_points", C.c_int), ("niters", C.c_int), ("best_iter", C.c_int), ("best_cand", C.c_int),
+                ("ransac_count", C.c_int), ("n_E", C.c_int), ("pose_count", C.c_int), ("pose_cand", C.c_int), ("pose_index", C.c_int),
+                ("pose_counts", C.c_int * 40), ("E", C.c_double * 90), ("poses", C.c_double * 480), ("R", C.c_double * 9),
+                ("t", C.c_double * 3)]
+
+
+def pose_record(device):
+    """A device buffer for one rf_pose_record_t."""
+    return torch.zeros(C.sizeof(PoseRecord), device=device, dtype=torch.uint8)
+
+
+def read_pose_record(rec):
+    """The record as a dict of host values / numpy arrays (one device-to-host copy)."""
+    r = PoseRecord.from_buffer_copy(rec.cpu().numpy().tobytes())
+    nE = max(r.n_E, 0)
+    return dict(status=r.status, n_points=r.n_points, niters=r.niters, best=(r.best_iter, r.best_cand), ransac_count=r.ransac_count,
+                n_E=r.n_E, pose_count=r.pose_count, pose=(r.pose_cand, r.pose_index),
+                pose_counts=np.array(r.pose_counts, dtype=np.int64).reshape(10, 4)[:nE],
+                E=np.array(r.E).reshape(10, 3, 3)[:nE], poses=np.array(r.poses).reshape(10, 4, 3, 4)[:nE],
+                R=np.array(r.R).reshape(3, 3), t=np.array(r.t).reshape(3, 1))
+
+
+def record_E(rec):
+    """The E field of a record buffer as a writable fp64 view [10][9] (tests supply their own E through it)."""
+    off = PoseRecord.E.offset
+    return rec[off:off + 90 * 8].view(torch.float64).view(10, 9)
+
+
+def yfcc_matches(flow, mask, angle, sizeA, sizeB, norm1, norm2):
+    """evaluation/evalYFCC/getResults.py:53-71 matches_from_flow + :29-50 norm_kp on the device: flow (H,W,2) fp32, mask (H,W)
+    (non-zero = matched) -> (pts1, pts2 [H*W][2] fp64 capacity, N [1] int32 on the device).  ``norm1`` / ``norm2`` are norm_kp's
+    (cx, cy, fx, fy) of each image.  A mask whose shape is not the rotated target grid's raises IndexError, as numpy does."""
+    need_cuda(flow, mask)
+    wA, hA = int(sizeA[0]), int(sizeA[1])
+    wB, hB = int(sizeB[0]), int(sizeB[1])
+    k = (int(angle) // 90) % 4
+    H, W = int(mask.shape[0]), int(mask.shape[1])
+    if mask.dim() != 2 or (H, W) != ((hB, wB) if k % 2 == 0 else (wB, hB)):
+        raise IndexError("boolean index did not match indexed array: mask %s vs rotated grid %s"
+                         % (tuple(mask.shape), (hB, wB) if k % 2 == 0 else (wB, hB)))
+    assert tuple(flow.shape) == (H, W, 2), flow.shape
+    flow = flow.float().contiguous()
+    mask = (mask != 0).to(torch.uint8).contiguous() if mask.dtype != torch.uint8 else mask.contiguous()
+    dev = flow.device
+    cap = max(H * W, 1)
+    pts1 = torch.empty((cap, 2), device=dev, dtype=torch.float64)
+    pts2 = torch.empty((cap, 2), device=dev, dtype=torch.float64)
+    N = torch.empty(1, device=dev, dtype=torch.int32)
+    wsz = lib.rf_yfcc_matches_workspace(H, W)
+    ws = torch.empty(max(wsz, 1), device=dev, dtype=torch.uint8)
+    n1 = (C.c_double * 4)(*[float(v) for v in norm1])
+    n2 = (C.c_double * 4)(*[float(v) for v in norm2])
+    check(lib.rf_yfcc_matches(ptr(flow), ptr(mask), H, W, k, wB, hB, wA, hA, n1, n2, ptr(pts1), ptr(pts2), ptr(N), ptr(ws), wsz,
+                              stream()))
+    return pts1, pts2, N
+
+
+def essential_ransac(pts1, pts2, N, threshold=0.0005, rec=None):
+    """cv2.findEssentialMat(pts1[:N], pts2[:N], method=cv2.RANSAC, threshold) on the device (N: [1] int32 device count):
+    -> (record buffer, mask [capacity] u8).  Read the record with ``read_pose_record``."""
+    need_cuda(pts1, pts2, N)
+    dev = pts1.device
+    cap = int(pts1.shape[0])
+    rec = pose_record(dev) if rec is None else rec
+    mask = torch.zeros(max(cap, 1), device=dev, dtype=torch.uint8)
+    wsz = lib.rf_essential_ransac_workspace(cap)
+    ws = torch.empty(wsz, device=dev, dtype=torch.uint8)
+    check(lib.rf_essential_ransac(ptr(pts1), ptr(pts2), cap, ptr(N), float(threshold), ptr(rec), ptr(mask), ptr(ws), wsz, stream()))
+    return rec, mask
+
+
+def recover_pose(pts1, pts2, mask, rec):
+    """cv2.recoverPose(E, pts1, pts2, mask=mask) over the stacked E of ``rec`` with evalYFCC's loop (getResults.py:96-104):
+    fills R, t and the count in the record; -> (mask_out [capacity] u8, cheirality bits [capacity] int64)."""
+    need_cuda(pts1, pts2, mask, rec)
+    dev = pts1.device
+    cap = int(pts1.shape[0])
+    out = torch.zeros(max(cap, 1), device=dev, dtype=torch.uint8)
+    wsz = lib.rf_recover_pose_workspace(cap)
+    ws = torch.zeros(wsz, device=dev, dtype=torch.uint8)
+    check(lib.rf_recover_pose(ptr(pts1), ptr(pts2), cap, ptr(mask), ptr(rec), ptr(out), ptr(ws), wsz, stream()))
+    return out, ws[:8 * cap].view(torch.int64)
+
+
+def essential_samples(N):
+    """The [1000][5] subset table of cv2.findEssentialMat's RANSAC for N = N[0] (device int32) points."""
+    need_cuda(N)
+    idx = torch.zeros((1000, 5), device=N.device, dtype=torch.int32)
+    check(lib.rf_essential_samples(ptr(N), ptr(idx), stream()))
+    return idx
+
+
+def essential_five_point(pts1, pts2, idx):
+    """Five-point solutions of the subsets idx [S][5]: (E [S][10][9] fp64, count [S] int32)."""
+    need_cuda(pts1, pts2, idx)
+    S = int(idx.shape[0])
+    E = torch.full((max(S, 1), 10, 9), float("nan"), device=pts1.device, dtype=torch.float64)
+    n = torch.full((max(S, 1),), -1, device=pts1.device, dtype=torch.int32)
+    check(lib.rf_essential_five_point(ptr(pts1), ptr(pts2), ptr(idx.int().contiguous()), S, ptr(E), ptr(n), stream()))
+    return E[:S], n[:S]
+
+
+def essential_score(pts1, pts2, E, threshold=0.0005, want_err=False):
+    """Sampson inlier counts of models E [M][9] (M <= 640) over all rows of pts1 / pts2 (and the fp32 errors [M][N])."""
+    need_cuda(pts1, pts2, E)
+    N, M = int(pts1.shape[0]), int(E.shape[0])
+    counts = torch.zeros(max(M, 1), device=E.device, dtype=torch.int32)
+    err = torch.full((M, N), float("nan"), device=E.device, dtype=torch.float32) if want_err else None
+    check(lib.rf_essential_score(ptr(pts1.contiguous()), ptr(pts2.contiguous()), N, ptr(E.contiguous()), M, float(threshold),
+                                 ptr(counts), ptr(err), stream()))
+    return counts[:M], err
+
+
 # --------------------------------------------------------------------------- warp
 def warp_grid(H, h, w):
     need_cuda(H)

@@ -821,6 +821,13 @@ def getFlow_corr(flow, param, match, th=0.95, multiH=True):
     """evaluation/evalCorr/getResults.py:78-134 ``getFlow`` (= evalYFCC/getResults.py:150-190 ``_getFlow``) after its np.load
     calls: flow (nH,2,h8,w8), param (nH,3,3), match (nH,2,h8,w8) -> (flowGlobal (1,8h8,8w8,2), matchGlobal (1,8h8,8w8,1)), CUDA:
     x8 upsampling, ``match12 * grid_sample(match21) * inside`` from the fused composition kernel, then ``merge_first_wins``."""
+    flowGlobal, matchGlobal, _ = getFlow_corr_binary(flow, param, match, th, multiH)
+    return flowGlobal, matchGlobal
+
+
+def getFlow_corr_binary(flow, param, match, th=0.95, multiH=True):
+    """``getFlow_corr`` plus the merge's binary map (1,8h8,8w8,1) bool, which evalYFCC's ``_getFlow`` returns instead of the
+    matchability (evalYFCC/getResults.py:178-187)."""
     flow = torch.as_tensor(flow, dtype=torch.float32).cuda()
     param = torch.as_tensor(param, dtype=torch.float32).cuda()
     match = torch.as_tensor(match, dtype=torch.float32).cuda()
@@ -833,8 +840,7 @@ def getFlow_corr(flow, param, match, th=0.95, multiH=True):
         ms.append(m)
     f = torch.clamp(torch.cat(fl, dim=0), min=-1, max=1)
     m = torch.cat(ms, dim=0).permute(0, 2, 3, 1)
-    flowGlobal, matchGlobal, _ = merge_first_wins(f, m, th, multiH)
-    return flowGlobal, matchGlobal
+    return merge_first_wins(f, m, th, multiH)
 
 
 def getFlow_all(flow, param, match, outH, outW, th=0.95, multiH=True, with_match21=False):

@@ -19,7 +19,7 @@ import os
 import numpy as np
 import torch
 
-from . import pipeline
+from . import ops, pipeline
 
 
 # --------------------------------------------------------------------------- evalHpatch / evalCorr / evalYFCC
@@ -92,6 +92,102 @@ def getFlow_from_files(pairID, finePath, flowList, coarsePath, maskPath, multiH,
         return [], []
     flow, param, match = t
     return pipeline.getFlow_corr(flow, param, match, th=th, multiH=multiH)
+
+
+# --------------------------------------------------------------------------- evalYFCC pose
+def getFlow_yfcc_from_files(pairID, finePath, flowList, coarsePath, maskPath, multiH, th):
+    """evaluation/evalYFCC/getResults.py:132-190 ``getFlow``: (flowGlobal (H,W,2) fp32, match_binary (H,W) bool) CUDA, the
+    first-hypothesis-wins binary map multiplied by ``maskPath/maskBG_{pairID}_{nH}H.npy``; ([], []) when the pair has no files."""
+    if flowList is None:
+        flowList = os.listdir(finePath)
+    t = load_pair(pairID, finePath, coarsePath, flowList)
+    if t is None:
+        return [], []
+    flow, param, match = t
+    bg = np.load(os.path.join(maskPath, "maskBG_{}_{}H.npy".format(pairID, find_nbH(pairID, flowList))))
+    flowGlobal, _, mb = pipeline.getFlow_corr_binary(flow, param, match, th=th, multiH=multiH)
+    mb = mb.squeeze() * torch.as_tensor(np.asarray(bg), device=mb.device).bool()
+    return flowGlobal.squeeze(), mb
+
+
+def yfcc_pose(flowGlobal, match_binary, size_A, size_B, angle, K_A, K_B, org_A, org_B, ransac=True, threshold=0.0005):
+    """getResults.py:318-325 on the device: matches_from_flow + norm_kp + opencv_decompose (cv2.findEssentialMat(RANSAC) and
+    cv2.recoverPose over the stacked candidates), every stage on the current stream; the host reads one record at the end.
+    ``size_*`` = resized_shapes[id] (w, h), ``org_*`` = org_imsizes[id] (w, h).  Returns ((R, t) or None, match count)."""
+    if not ransac:
+        raise NotImplementedError("yfcc_pose: the non-RANSAC branch (cv2.findFundamentalMat(FM_8POINT) fed to recoverPose) "
+                                  "is not implemented")
+    flowGlobal = torch.as_tensor(flowGlobal).cuda()
+    match_binary = torch.as_tensor(match_binary).cuda()
+    n1 = _norm_params(org_A, size_A, np.asarray(K_A, dtype=np.float64))
+    n2 = _norm_params(org_B, size_B, np.asarray(K_B, dtype=np.float64))
+    pts1, pts2, N = ops.yfcc_matches(flowGlobal, match_binary, angle, size_A, size_B, n1, n2)
+    rec, mask = ops.essential_ransac(pts1, pts2, N, threshold)
+    ops.recover_pose(pts1, pts2, mask, rec)
+    r = ops.read_pose_record(rec)
+    if r["status"] != ops.POSE_OK or r["pose_count"] <= 0:
+        return None, r["n_points"]
+    return (r["R"], r["t"]), r["n_points"]
+
+
+def _norm_params(org_size, new_size, K):
+    """norm_kp's (cx, cy, fx, fy) (getResults.py:29-50), in its statement order."""
+    w, h = org_size
+    w_n, h_n = new_size
+    cx = (w - 1.0) * 0.5
+    cy = (h - 1.0) * 0.5
+    cx += K[0, 2]
+    cy += K[1, 2]
+    fx = K[0, 0]
+    fy = K[1, 1]
+    cx *= (w_n / w)
+    cy *= (h_n / h)
+    fx *= (w_n / w)
+    fy *= (h_n / h)
+    return float(cx), float(cy), float(fx), float(fy)
+
+
+def evaluate_R_t(R_gt, t_gt, R_pred, t_pred):
+    """getResults.py:114-129: (rotation error, translation-direction error) in degrees (host numpy on 3 x 3s)."""
+    t_gt = np.asarray(t_gt).flatten()
+    t_pred = np.asarray(t_pred).flatten()
+    R = np.asarray(R_gt) @ np.asarray(R_pred).T
+    err_q = np.arccos((np.trace(R) - 1) / 2) * 180 / np.pi
+    t_pred = t_pred / (np.linalg.norm(t_pred))
+    t_gt = t_gt / (np.linalg.norm(t_gt))
+    err_t = np.arccos(t_gt[None, :] @ t_pred[:, None]).item() * 180 / np.pi
+    return err_q, err_t
+
+
+def pose_accuracy(errors):
+    """getResults.py:335-347: {'Acc@5', 'Acc@10', 'Acc@15', 'Acc@20'}, the fraction of pose errors below each threshold."""
+    e = np.array(errors)
+    return {"Acc@%d" % th: np.sum(e < th) / float(len(e)) for th in (5, 10, 15, 20)}
+
+
+def yfcc_pose_errors(pairs_ids, finePath, coarsePath, maskPath, rotation, R_list, T_list, K_list, org_imsizes, resized_shapes,
+                     multiH=True, th=0.95, ransac=True, threshold=0.0005, flowList=None):
+    """The per-pair loop of getResults.py:298-331 for one scene: the max of the rotation and translation errors per pair, 180 for
+    a pair with no files, no matches or no model.  ``R_list`` / ``T_list`` / ``K_list`` / ``org_imsizes`` are what the driver
+    reads from its calibration files (``T_list[i]`` as the driver's ``np.array(calib['T']).T``), ``resized_shapes`` its
+    getResizedSize per image, ``rotation`` the loaded rotation.json."""
+    if flowList is None:
+        flowList = [item for item in os.listdir(finePath) if "flow" in item]
+    res = []
+    for i, (idA, idB) in enumerate(pairs_ids):
+        flow, match = getFlow_yfcc_from_files(i, finePath, flowList, coarsePath, maskPath, multiH, th)
+        if len(flow) == 0:
+            res.append(180)
+            continue
+        r = R_list[idB] @ R_list[idA].T
+        t = T_list[idB] - r @ T_list[idA]
+        decomposed, n = yfcc_pose(flow, match, resized_shapes[idA], resized_shapes[idB], rotation[str(i)], K_list[idA], K_list[idB],
+                                  org_imsizes[idA], org_imsizes[idB], ransac=ransac, threshold=threshold)
+        if n == 0 or decomposed is None:
+            res.append(180)
+        else:
+            res.append(max(evaluate_R_t(r, t, decomposed[0], decomposed[1])))
+    return res
 
 
 # --------------------------------------------------------------------------- evalKITTI
