@@ -302,19 +302,21 @@ int rf_fill_nearest_matched(const float* flow, const uint8_t* matched, int H, in
  * fp64 on the device.  The point count stays on the device; the three calls share one record the host reads at the end. */
 #define RF_POSE_OK 0          /* E (and, after rf_recover_pose, R / t) valid                                     */
 #define RF_POSE_TOO_FEW 1     /* fewer than 5 matches: the driver's pts1.shape[0] >= 5 test fails (no model)     */
-#define RF_POSE_NO_MODEL 2    /* findEssentialMat finds no E with 5 or more inliers                             */
+#define RF_POSE_NO_MODEL 2    /* findEssentialMat finds no E with 5 or more inliers; findFundamentalMat no F     */
 #define RF_POSE_NO_POSE 3     /* every recoverPose count is 0: the driver's loop keeps no (R, t)                 */
 typedef struct rf_pose_record {
     int status;                     /* RF_POSE_* */
     int n_points;                   /* N */
-    int niters;                     /* RANSAC iteration budget at the end (RANSACUpdateNumIters) */
-    int best_iter, best_cand;       /* (iteration, candidate) of the best E; -1 when none */
-    int ransac_count;               /* its inlier count */
-    int n_E;                        /* stacked candidates in E: 1, or every solution of the single minimal problem when N == 5 */
+    int niters;                     /* RANSAC iteration budget at the end (RANSACUpdateNumIters); 0 from rf_fundamental_8point */
+    int best_iter, best_cand;       /* (iteration, candidate) of the best E; -1 when none, and from rf_fundamental_8point */
+    int ransac_count;               /* its inlier count; -1 from rf_fundamental_8point (its mask is all ones) */
+    int n_E;                        /* stacked candidates in E: 1, or every solution of the single minimal problem when N == 5
+                                       (rf_essential_ransac) or N == 7 (rf_fundamental_8point: 1..3) */
     int pose_count;                 /* the driver's num_inlier */
     int pose_cand, pose_index;      /* the winning candidate and its pose (0..3: (R1, t), (R2, t), (R1, -t), (R2, -t)) */
     int pose_counts[40];            /* [candidate][pose] cheirality counts */
-    double E[90];                   /* [n_E][3][3] row-major, unit Frobenius norm */
+    double E[90];                   /* [n_E][3][3] row-major: E with unit Frobenius norm (rf_essential_ransac), or F as
+                                       cv2.findFundamentalMat returns it, F22 = 1 unless |F22| <= FLT_EPSILON (rf_fundamental_8point) */
     double poses[480];              /* [candidate][pose][3][4] = [R | t] of decomposeEssentialMat */
     double R[9], t[3];
 } rf_pose_record_t;
@@ -349,6 +351,21 @@ int rf_essential_five_point(const double* pts1, const double* pts2, const int* i
                             void* stream);
 int rf_essential_score(const double* pts1, const double* pts2, int N, const double* E, int nmodels, double threshold,
                        int* counts_out, float* err_out, void* stream);
+/* cv2.findFundamentalMat(pts1, pts2, method=FM_8POINT), the driver's non-RANSAC branch (:84-87), with the points cast to fp32
+ * first as cv2 does: N < 5 RF_POSE_TOO_FEW; 5 <= N < 7 RF_POSE_NO_MODEL; N == 7 the seven-point solver (n_E = 1..3 stacked
+ * candidates in cv2's order); N >= 8 the eight-point solver (n_E = 1); a degenerate normalisation or eigen-spectrum, or no real
+ * root, RF_POSE_NO_MODEL.  mask_out[N] is all ones whenever N >= 7.  Three grid-wide fp64 reductions (centroids, mean
+ * distances, the 45 moments of A = sum r r^T) write per-CTA partials that are summed in a fixed order (no atomics: the same
+ * bits on every run), then one warp solves the 9 x 9 eigenproblem.  A fixed launch sequence sized from capacity, N = *N_dev
+ * <= capacity on the device: graph-capturable.  rf_recover_pose then runs on rec as it does after rf_essential_ransac. */
+size_t rf_fundamental_8point_workspace(int capacity);
+int rf_fundamental_8point(const double* pts1, const double* pts2, int capacity, const int* N_dev, rf_pose_record_t* rec,
+                          uint8_t* mask_out, void* ws, size_t ws_bytes, void* stream);
+/* The reductions of rf_fundamental_8point alone (for tests), N = *N_dev >= 1: out[51] = (m1c.x, m1c.y, m2c.x, m2c.y, scale1,
+ * scale2, A[45]) with scale = sqrt(2) / mean distance and A's upper triangle row by row (A00, A01, ..., A08, A11, ..., A88).
+ * ws as rf_fundamental_8point_workspace(capacity). */
+int rf_fundamental_moments(const double* pts1, const double* pts2, int capacity, const int* N_dev, double* out, void* ws,
+                           size_t ws_bytes, void* stream);
 
 #ifdef __cplusplus
 }

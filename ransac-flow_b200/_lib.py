@@ -67,6 +67,9 @@ SIGNATURES = {
     "rf_essential_samples": (i32, [vp, vp, vp]),
     "rf_essential_five_point": (i32, [vp, vp, vp, i32, vp, vp, vp]),
     "rf_essential_score": (i32, [vp, vp, i32, vp, i32, C.c_double, vp, vp, vp]),
+    "rf_fundamental_8point_workspace": (sz, [i32]),
+    "rf_fundamental_8point": (i32, [vp, vp, i32, vp, vp, vp, vp, sz, vp]),
+    "rf_fundamental_moments": (i32, [vp, vp, i32, vp, vp, vp, sz, vp]),
 }
 
 

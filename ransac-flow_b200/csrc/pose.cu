@@ -801,6 +801,405 @@ __global__ void pose_mask_kernel(const uint8_t* __restrict__ mask_in, int capaci
     mask_out[i] = (rec->status == RF_POSE_OK && p >= 0) ? (uint8_t)(mask_in[i] != 0 && ((bits[i] >> p) & 1ull)) : 0;
 }
 
+// ------------------------------------------------------------------------------------------------ findFundamentalMat
+// cv2.findFundamentalMat(FM_8POINT): run8Point (N >= 8) / run7Point (N == 7) on the points cast to fp32.  Three passes over
+// the points (centroids, mean distances, the 45 moments); each CTA writes its partial sums, and every consumer sums the
+// partials of the CTAs that held points in the same fixed order, so the result does not depend on scheduling.
+constexpr int FM_THREADS = 256;
+constexpr int FM_MAXGRID = 512;
+constexpr int FM_STATS = 51;             // m1c (2), m2c (2), scale1, scale2, A's upper triangle (45)
+
+static inline int fm_grid(int capacity) {
+    const int g = (capacity + FM_THREADS - 1) / FM_THREADS;
+    return g < 1 ? 1 : (g > FM_MAXGRID ? FM_MAXGRID : g);
+}
+
+struct FmWs {
+    double* p1;   // [grid][4]  sum of (x1, y1, x2, y2)
+    double* p2;   // [grid][2]  sum of the distances to the centroids
+    double* p3;   // [grid][45] sum of r r^T
+};
+static FmWs fm_carve(void* ws, int grid) {
+    unsigned char* p = static_cast<unsigned char*>(ws);
+    FmWs w;
+    w.p1 = reinterpret_cast<double*>(p);
+    p += align256((size_t)grid * 4 * sizeof(double));
+    w.p2 = reinterpret_cast<double*>(p);
+    p += align256((size_t)grid * 2 * sizeof(double));
+    w.p3 = reinterpret_cast<double*>(p);
+    return w;
+}
+
+// findFundamentalMat's convertTo(CV_32F), back in fp64 for run8Point's arithmetic
+__device__ __forceinline__ void fm_load(const double* __restrict__ pts1, const double* __restrict__ pts2, long long i, double& x1,
+                                        double& y1, double& x2, double& y2) {
+    x1 = (double)__double2float_rn(pts1[2 * i]);
+    y1 = (double)__double2float_rn(pts1[2 * i + 1]);
+    x2 = (double)__double2float_rn(pts2[2 * i]);
+    y2 = (double)__double2float_rn(pts2[2 * i + 1]);
+}
+
+// the CTA's sums of v[K] into out[K]: xor-butterfly within each warp, then the warps in order
+template <int K>
+__device__ __forceinline__ void fm_block_sum(double (&v)[K], double* __restrict__ out) {
+    __shared__ double s[FM_THREADS / 32][K];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        double x = v[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+        if (lane == 0) s[warp][k] = x;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < K; k += blockDim.x) {
+        double x = 0.0;
+        for (int w = 0; w < FM_THREADS / 32; ++w) x += s[w][k];
+        out[k] = x;
+    }
+}
+
+// sum over the first `active` CTAs' partials part[g][K] (component k) in one warp: lanes stride over g, then an xor
+// butterfly; every lane, and every CTA that calls it, gets the same bits
+__device__ __forceinline__ double fm_warp_total(const double* __restrict__ part, int K, int k, int active) {
+    double x = 0.0;
+    for (int g = threadIdx.x & 31; g < active; g += 32) x += part[(size_t)g * K + k];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    return x;
+}
+
+__device__ __forceinline__ int fm_active(int N, int grid) {
+    const int a = (N + FM_THREADS - 1) / FM_THREADS;
+    return a < grid ? a : grid;
+}
+
+// centroids (cv: m1c += Point2d(m1[i]); m1c *= 1. / count) from the pass-1 partials, by warp 0 of the calling CTA
+__device__ __forceinline__ void fm_centroids(const FmWs& w, int N, int grid, double* __restrict__ c) {
+    const int active = fm_active(N, grid);
+    const double t = 1.0 / N;
+    for (int k = 0; k < 4; ++k) {
+        const double s = fm_warp_total(w.p1, 4, k, active);
+        if (threadIdx.x == 0) c[k] = s * t;
+    }
+}
+
+// scale = sqrt(2) / mean distance; a mean below FLT_EPSILON marks a degenerate set (returned as scale 0)
+__device__ __forceinline__ void fm_scales(const FmWs& w, int N, int grid, double* __restrict__ sc) {
+    const int active = fm_active(N, grid);
+    const double t = 1.0 / N;
+    for (int k = 0; k < 2; ++k) {
+        const double m = fm_warp_total(w.p2, 2, k, active) * t;
+        if (threadIdx.x == 0) sc[k] = m < 1.1920928955078125e-07 ? 0.0 : 1.4142135623730951 / m;
+    }
+}
+
+// pass 1: centroid sums; also writes the all-ones mask of findFundamentalMat when N >= 7
+__global__ void __launch_bounds__(FM_THREADS) fm_centroid_kernel(const double* __restrict__ pts1, const double* __restrict__ pts2,
+                                                                 const int* __restrict__ N_dev, FmWs w, uint8_t* __restrict__ mask_out) {
+    const int N = *N_dev;
+    if ((long long)blockIdx.x * FM_THREADS >= N) return;
+    double v[4] = {0.0, 0.0, 0.0, 0.0};
+    for (long long i = (long long)blockIdx.x * FM_THREADS + threadIdx.x; i < N; i += (long long)gridDim.x * FM_THREADS) {
+        double x1, y1, x2, y2;
+        fm_load(pts1, pts2, i, x1, y1, x2, y2);
+        v[0] += x1; v[1] += y1; v[2] += x2; v[3] += y2;
+        if (mask_out && N >= 7) mask_out[i] = 1;
+    }
+    fm_block_sum<4>(v, w.p1 + (size_t)blockIdx.x * 4);
+}
+
+// pass 2: sums of the distances to the centroids
+__global__ void __launch_bounds__(FM_THREADS) fm_distance_kernel(const double* __restrict__ pts1, const double* __restrict__ pts2,
+                                                                 const int* __restrict__ N_dev, FmWs w) {
+    __shared__ double s_c[4];
+    const int N = *N_dev;
+    if ((long long)blockIdx.x * FM_THREADS >= N) return;
+    if (threadIdx.x < 32) fm_centroids(w, N, gridDim.x, s_c);
+    __syncthreads();
+    const double c0 = s_c[0], c1 = s_c[1], c2 = s_c[2], c3 = s_c[3];
+    double v[2] = {0.0, 0.0};
+    for (long long i = (long long)blockIdx.x * FM_THREADS + threadIdx.x; i < N; i += (long long)gridDim.x * FM_THREADS) {
+        double x1, y1, x2, y2;
+        fm_load(pts1, pts2, i, x1, y1, x2, y2);
+        const double a = x1 - c0, b = y1 - c1, d = x2 - c2, e = y2 - c3;
+        v[0] += sqrt(a * a + b * b);
+        v[1] += sqrt(d * d + e * e);
+    }
+    fm_block_sum<2>(v, w.p2 + (size_t)blockIdx.x * 2);
+}
+
+// r = (x2 x1, x2 y1, x2, y2 x1, y2 y1, y2, x1, y1, 1) of a normalised point pair
+__device__ __forceinline__ void fm_row(double x1, double y1, double x2, double y2, const double* c, const double* sc, double (&r)[9]) {
+    const double u1 = (x1 - c[0]) * sc[0], v1 = (y1 - c[1]) * sc[0];
+    const double u2 = (x2 - c[2]) * sc[1], v2 = (y2 - c[3]) * sc[1];
+    r[0] = u2 * u1; r[1] = u2 * v1; r[2] = u2;
+    r[3] = v2 * u1; r[4] = v2 * v1; r[5] = v2;
+    r[6] = u1; r[7] = v1; r[8] = 1.0;
+}
+
+// pass 3: the 45 distinct sums of r r^T
+__global__ void __launch_bounds__(FM_THREADS, 1) fm_moment_kernel(const double* __restrict__ pts1, const double* __restrict__ pts2,
+                                                               const int* __restrict__ N_dev, FmWs w) {
+    __shared__ double s_c[4], s_sc[2];
+    const int N = *N_dev;
+    if ((long long)blockIdx.x * FM_THREADS >= N) return;
+    if (threadIdx.x < 32) {
+        fm_centroids(w, N, gridDim.x, s_c);
+        fm_scales(w, N, gridDim.x, s_sc);
+    }
+    __syncthreads();
+    const double c[4] = {s_c[0], s_c[1], s_c[2], s_c[3]}, sc[2] = {s_sc[0], s_sc[1]};
+    double acc[45];
+#pragma unroll
+    for (int k = 0; k < 45; ++k) acc[k] = 0.0;
+    for (long long i = (long long)blockIdx.x * FM_THREADS + threadIdx.x; i < N; i += (long long)gridDim.x * FM_THREADS) {
+        double x1, y1, x2, y2, r[9];
+        fm_load(pts1, pts2, i, x1, y1, x2, y2);
+        fm_row(x1, y1, x2, y2, c, sc, r);
+        int k = 0;
+#pragma unroll
+        for (int a = 0; a < 9; ++a)
+#pragma unroll
+            for (int b = a; b < 9; ++b) acc[k++] += r[a] * r[b];
+    }
+    fm_block_sum<45>(acc, w.p3 + (size_t)blockIdx.x * 45);
+}
+
+// the statistics run8Point works from, by one warp: out[FM_STATS] as rf_fundamental_moments documents
+__device__ void fm_stats(const FmWs& w, int N, int grid, double* __restrict__ out) {
+    fm_centroids(w, N, grid, out);
+    fm_scales(w, N, grid, out + 4);
+    const int active = fm_active(N, grid);
+    for (int k = 0; k < 45; ++k) {
+        const double s = fm_warp_total(w.p3, 45, k, active);
+        if (threadIdx.x == 0) out[6 + k] = s;
+    }
+}
+
+__global__ void fm_stats_kernel(const int* __restrict__ N_dev, FmWs w, int grid, double* __restrict__ out) {
+    const int N = *N_dev;
+    if (N >= 1) fm_stats(w, N, grid, out);
+}
+
+// the eigen-decomposition of the symmetric 9 x 9 A by one warp: one-sided Jacobi (the SVD of A, whose right vectors are A's
+// eigenvectors) with lane j < 9 holding column j of A and of V, the nine columns paired round-robin (9 rounds of four
+// disjoint pairs per sweep).  On return lam = v_j . a_j, the signed eigenvalue of lane j, and v = its eigenvector.
+__device__ void fm_eigen9(double (&a)[9], double (&v)[9], double& lam) {
+    const int j = threadIdx.x & 31;
+    for (int sweep = 0; sweep < 40; ++sweep) {
+        bool rotated = false;
+        for (int round = 0; round < 9; ++round) {
+            const int p = j < 9 ? (2 * round - j + 18) % 9 : j;   // partner; p == j: idle this round
+            double ap[9], vp[9];
+#pragma unroll
+            for (int r = 0; r < 9; ++r) {
+                ap[r] = __shfl_sync(0xffffffffu, a[r], p);
+                vp[r] = __shfl_sync(0xffffffffu, v[r], p);
+            }
+            if (p == j) continue;
+            const bool lo = j < p;                                  // this lane holds column i of the pair (i < k)
+            double ni = 0.0, nk = 0.0, g = 0.0;
+#pragma unroll
+            for (int r = 0; r < 9; ++r) {
+                const double ai = lo ? a[r] : ap[r], ak = lo ? ap[r] : a[r];
+                ni += ai * ai; nk += ak * ak; g += ai * ak;
+            }
+            if (g == 0.0 || fabs(g) <= 2.220446049250313e-16 * sqrt(ni * nk)) continue;
+            rotated = true;
+            const double zeta = (nk - ni) / (2.0 * g);
+            const double t = copysign(1.0, zeta) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+            const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
+#pragma unroll
+            for (int r = 0; r < 9; ++r) {
+                // column i -> c a_i - s a_k, column k -> s a_i + c a_k
+                a[r] = lo ? c * a[r] - s * ap[r] : s * ap[r] + c * a[r];
+                v[r] = lo ? c * v[r] - s * vp[r] : s * vp[r] + c * v[r];
+            }
+        }
+        if (!__any_sync(0xffffffffu, rotated)) break;
+    }
+    lam = 0.0;
+#pragma unroll
+    for (int r = 0; r < 9; ++r) lam += a[r] * v[r];
+}
+
+// F = T2^T F0 T1 with T = [[s, 0, -s cx], [0, s, -s cy], [0, 0, 1]], then F *= 1 / F22 when |F22| > FLT_EPSILON
+__device__ void fm_denormalise(const double (&F0)[3][3], const double* c, const double* sc, double* out) {
+    const double T1[3][3] = {{sc[0], 0.0, -sc[0] * c[0]}, {0.0, sc[0], -sc[0] * c[1]}, {0.0, 0.0, 1.0}};
+    const double T2[3][3] = {{sc[1], 0.0, -sc[1] * c[2]}, {0.0, sc[1], -sc[1] * c[3]}, {0.0, 0.0, 1.0}};
+    double TF[3][3], F[3][3];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) TF[i][j] = T2[0][i] * F0[0][j] + T2[1][i] * F0[1][j] + T2[2][i] * F0[2][j];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) F[i][j] = TF[i][0] * T1[0][j] + TF[i][1] * T1[1][j] + TF[i][2] * T1[2][j];
+    const double f = fabs(F[2][2]) > 1.1920928955078125e-07 ? 1.0 / F[2][2] : 1.0;
+    for (int k = 0; k < 9; ++k) out[k] = F[k / 3][k % 3] * f;
+}
+
+// cv::solveCubic for c0 x^3 + c1 x^2 + c2 x + c3, c0 != 0: the real roots in its order (trigonometric case: the
+// smallest, the largest, the middle one)
+__device__ int fm_solve_cubic(const double* c, double* x) {
+    const double a1 = c[1] / c[0], a2 = c[2] / c[0], a3 = c[3] / c[0];
+    const double Q = (a1 * a1 - 3 * a2) * (1. / 9);
+    const double R = (2 * a1 * a1 * a1 - 9 * a1 * a2 + 27 * a3) * (1. / 54);
+    const double Qcubed = Q * Q * Q;
+    const double d = Qcubed - R * R;
+    if (d > 0) {
+        const double theta = acos(R / sqrt(Qcubed));
+        const double t0 = -2 * sqrt(Q), t1 = theta * (1. / 3), t2 = a1 * (1. / 3);
+        const double pi = 3.141592653589793;
+        x[0] = t0 * cos(t1) - t2;
+        x[1] = t0 * cos(t1 + (2. * pi / 3)) - t2;
+        x[2] = t0 * cos(t1 - (2. * pi / 3)) - t2;
+        return 3;
+    }
+    double e = cbrt(sqrt(-d) + fabs(R));
+    if (R > 0) e = -e;
+    x[0] = (e + Q / e) - a1 * (1. / 3);
+    return 1;
+}
+
+// run7Point on lane 0: the 7 x 9 system's null space in the basis OpenCV's SVD completes it with (two sign vectors of
+// cv::RNG(0x12345678) scaled by 1/9, each orthogonalised twice against the row space and the one before it), then the cubic
+// det(l f1 + (1 - l) f2) = 0 and one F per real root.  Returns the candidate count (0: no model).
+__device__ int fm_seven_point(const double* __restrict__ pts1, const double* __restrict__ pts2, const double* c, const double* sc,
+                              double* __restrict__ Fout) {
+    __shared__ double q[9][9];    // rows 0..6: an orthonormal basis of the row space; rows 7, 8: f1, f2
+    for (int i = 0; i < 7; ++i) {
+        double x1, y1, x2, y2, r[9];
+        fm_load(pts1, pts2, i, x1, y1, x2, y2);
+        fm_row(x1, y1, x2, y2, c, sc, r);
+        for (int k = 0; k < 9; ++k) q[i][k] = r[k];
+    }
+    uint64_t state = 0x12345678ull;
+    for (int i = 0; i < 9; ++i) {
+        if (i >= 7)
+            for (int k = 0; k < 9; ++k) {
+                state = (uint64_t)(uint32_t)state * 4164903690ull + (state >> 32);
+                q[i][k] = ((uint32_t)state & 256u) ? 1.0 / 9 : -1.0 / 9;
+            }
+        // Gram-Schmidt, twice, against the rows before it
+        for (int pass = 0; pass < 2; ++pass)
+            for (int j = 0; j < i; ++j) {
+                double d = 0.0;
+                for (int k = 0; k < 9; ++k) d += q[i][k] * q[j][k];
+                for (int k = 0; k < 9; ++k) q[i][k] -= d * q[j][k];
+            }
+        double n = 0.0;
+        for (int k = 0; k < 9; ++k) n += q[i][k] * q[i][k];
+        const double inv = n > 0.0 ? 1.0 / sqrt(n) : 0.0;
+        for (int k = 0; k < 9; ++k) q[i][k] *= inv;
+    }
+    double f1[9], f2[9];
+    for (int k = 0; k < 9; ++k) { f2[k] = q[8][k]; f1[k] = q[7][k] - f2[k]; }
+    double cf[4];
+    {
+        double t0 = f2[4] * f2[8] - f2[5] * f2[7], t1 = f2[3] * f2[8] - f2[5] * f2[6], t2 = f2[3] * f2[7] - f2[4] * f2[6];
+        cf[3] = f2[0] * t0 - f2[1] * t1 + f2[2] * t2;
+        cf[2] = f1[0] * t0 - f1[1] * t1 + f1[2] * t2 - f1[3] * (f2[1] * f2[8] - f2[2] * f2[7]) + f1[4] * (f2[0] * f2[8] - f2[2] * f2[6]) -
+                f1[5] * (f2[0] * f2[7] - f2[1] * f2[6]) + f1[6] * (f2[1] * f2[5] - f2[2] * f2[4]) -
+                f1[7] * (f2[0] * f2[5] - f2[2] * f2[3]) + f1[8] * (f2[0] * f2[4] - f2[1] * f2[3]);
+        t0 = f1[4] * f1[8] - f1[5] * f1[7]; t1 = f1[3] * f1[8] - f1[5] * f1[6]; t2 = f1[3] * f1[7] - f1[4] * f1[6];
+        cf[1] = f2[0] * t0 - f2[1] * t1 + f2[2] * t2 - f2[3] * (f1[1] * f1[8] - f1[2] * f1[7]) + f2[4] * (f1[0] * f1[8] - f1[2] * f1[6]) -
+                f2[5] * (f1[0] * f1[7] - f1[1] * f1[6]) + f2[6] * (f1[1] * f1[5] - f1[2] * f1[4]) -
+                f2[7] * (f1[0] * f1[5] - f1[2] * f1[3]) + f2[8] * (f1[0] * f1[4] - f1[1] * f1[3]);
+        cf[0] = f1[0] * t0 - f1[1] * t1 + f1[2] * t2;
+    }
+    if (cf[0] == 0.0) return 0;
+    double roots[3];
+    const int n = fm_solve_cubic(cf, roots);
+    for (int k = 0; k < n; ++k) {
+        double lambda = roots[k], mu = 1.0;
+        const double s = f1[8] * roots[k] + f2[8];
+        double F0[3][3];
+        if (fabs(s) > 2.220446049250313e-16) {
+            mu = 1.0 / s;
+            lambda *= mu;
+            F0[2][2] = 1.0;
+        } else {
+            F0[2][2] = 0.0;
+        }
+        for (int i = 0; i < 8; ++i) F0[i / 3][i % 3] = f1[i] * lambda + f2[i] * mu;
+        fm_denormalise(F0, c, sc, Fout + 9 * k);
+    }
+    return n;
+}
+
+// the dense tail, one warp: statuses, run8Point's eigenvector and rank-2 step, or run7Point; fills the record
+__global__ void __launch_bounds__(32) fm_solve_kernel(const double* __restrict__ pts1, const double* __restrict__ pts2,
+                                                      const int* __restrict__ N_dev, FmWs w, int grid, rf_pose_record_t* __restrict__ rec) {
+    __shared__ double s_st[FM_STATS];
+    const int N = *N_dev, lane = threadIdx.x;
+    if (lane == 0) {
+        rec->n_points = N;
+        rec->niters = 0;
+        rec->best_iter = rec->best_cand = -1;
+        rec->ransac_count = -1;
+        rec->n_E = 0;
+        rec->pose_count = 0;
+        rec->pose_cand = rec->pose_index = -1;
+        for (int k = 0; k < 4 * ESS_MAXSOL; ++k) rec->pose_counts[k] = 0;
+        rec->status = N < 5 ? RF_POSE_TOO_FEW : RF_POSE_NO_MODEL;
+    }
+    if (N < 7) return;
+    fm_stats(w, N, grid, s_st);
+    __syncwarp();
+    const double* c = s_st;
+    const double* sc = s_st + 4;
+    if (sc[0] == 0.0 || sc[1] == 0.0) return;                      // a mean distance below FLT_EPSILON
+    if (N == 7) {
+        if (lane == 0) {
+            const int n = fm_seven_point(pts1, pts2, c, sc, rec->E);
+            rec->n_E = n;
+            rec->status = n > 0 ? RF_POSE_OK : RF_POSE_NO_MODEL;
+        }
+        return;
+    }
+    // lane j < 9: column j of A (= row j), column j of V = e_j
+    double a[9], v[9], lam;
+#pragma unroll
+    for (int r = 0; r < 9; ++r) {
+        const int i = min(lane, r), k = max(lane, r);
+        a[r] = lane < 9 ? s_st[6 + i * 9 - i * (i - 1) / 2 + (k - i)] : 0.0;
+        v[r] = r == lane ? 1.0 : 0.0;
+    }
+    fm_eigen9(a, v, lam);
+    // cv::eigen's descending order; the first eight must all be at least DBL_EPSILON in magnitude
+    double l[9];
+#pragma unroll
+    for (int j = 0; j < 9; ++j) l[j] = __shfl_sync(0xffffffffu, lam, j);
+    int order[9] = {0, 1, 2, 3, 4, 5, 6, 7, 8};
+    for (int i = 0; i < 9; ++i)
+        for (int j = i + 1; j < 9; ++j)
+            if (l[order[j]] > l[order[i]]) { const int t = order[i]; order[i] = order[j]; order[j] = t; }
+    bool degenerate = false;
+    for (int i = 0; i < 8; ++i) degenerate |= fabs(l[order[i]]) < 2.220446049250313e-16;
+    const int smallest = order[8];
+    double f0[9];
+#pragma unroll
+    for (int r = 0; r < 9; ++r) f0[r] = __shfl_sync(0xffffffffu, v[r], smallest);
+    if (lane != 0 || degenerate) return;
+    // rank 2: F0 = U diag(w0, w1, 0) V^T from its 3 x 3 SVD
+    double A3[3][3], V3[3][3], F0[3][3];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) A3[i][j] = f0[3 * i + j];
+    jacobi_svd<3>(A3, V3);
+    double sg[3];
+    for (int j = 0; j < 3; ++j) sg[j] = A3[0][j] * A3[0][j] + A3[1][j] * A3[1][j] + A3[2][j] * A3[2][j];
+    const int drop = (sg[0] <= sg[1] && sg[0] <= sg[2]) ? 0 : (sg[1] <= sg[2] ? 1 : 2);
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+            double x = 0.0;
+            for (int k = 0; k < 3; ++k)
+                if (k != drop) x += A3[i][k] * V3[j][k];
+            F0[i][j] = x;
+        }
+    fm_denormalise(F0, c, sc, rec->E);
+    rec->n_E = 1;
+    rec->status = RF_POSE_OK;
+}
+
 }  // namespace rf
 
 using namespace rf;
@@ -947,6 +1346,47 @@ extern "C" int rf_recover_pose(const double* pts1, const double* pts2, int capac
     pose_select_kernel<<<1, 256, 0, st>>>(mask_in, capacity, rec, bits, chain, mask_out);
     RF_LAUNCHED();
     pose_mask_kernel<<<grid, 256, 0, st>>>(mask_in, capacity, rec, bits, mask_out);
+    RF_LAUNCHED();
+    return 0;
+}
+
+extern "C" size_t rf_fundamental_8point_workspace(int capacity) {
+    const size_t g = (size_t)fm_grid(capacity);
+    return align256(g * 4 * sizeof(double)) + align256(g * 2 * sizeof(double)) + align256(g * 45 * sizeof(double));
+}
+
+// the three reduction passes; CTAs past N exit at once
+static void fm_passes(const double* pts1, const double* pts2, const int* N_dev, const FmWs& w, int grid, uint8_t* mask_out,
+                      cudaStream_t st) {
+    fm_centroid_kernel<<<grid, FM_THREADS, 0, st>>>(pts1, pts2, N_dev, w, mask_out);
+    fm_distance_kernel<<<grid, FM_THREADS, 0, st>>>(pts1, pts2, N_dev, w);
+    fm_moment_kernel<<<grid, FM_THREADS, 0, st>>>(pts1, pts2, N_dev, w);
+}
+
+extern "C" int rf_fundamental_8point(const double* pts1, const double* pts2, int capacity, const int* N_dev, rf_pose_record_t* rec,
+                                     uint8_t* mask_out, void* ws, size_t ws_bytes, void* stream) {
+    RF_REQUIRE(capacity >= 0 && N_dev != nullptr && rec != nullptr && mask_out != nullptr, "rf_fundamental_8point: bad arguments");
+    RF_REQUIRE(ws != nullptr && ws_bytes >= rf_fundamental_8point_workspace(capacity), "rf_fundamental_8point: workspace too small");
+    cudaStream_t st = as_stream(stream);
+    const int grid = fm_grid(capacity);
+    const FmWs w = fm_carve(ws, grid);
+    fm_passes(pts1, pts2, N_dev, w, grid, mask_out, st);
+    RF_LAUNCHED();
+    fm_solve_kernel<<<1, 32, 0, st>>>(pts1, pts2, N_dev, w, grid, rec);
+    RF_LAUNCHED();
+    return 0;
+}
+
+extern "C" int rf_fundamental_moments(const double* pts1, const double* pts2, int capacity, const int* N_dev, double* out, void* ws,
+                                      size_t ws_bytes, void* stream) {
+    RF_REQUIRE(capacity >= 0 && N_dev != nullptr && out != nullptr, "rf_fundamental_moments: bad arguments");
+    RF_REQUIRE(ws != nullptr && ws_bytes >= rf_fundamental_8point_workspace(capacity), "rf_fundamental_moments: workspace too small");
+    cudaStream_t st = as_stream(stream);
+    const int grid = fm_grid(capacity);
+    const FmWs w = fm_carve(ws, grid);
+    fm_passes(pts1, pts2, N_dev, w, grid, nullptr, st);
+    RF_LAUNCHED();
+    fm_stats_kernel<<<1, 32, 0, st>>>(N_dev, w, grid, out);
     RF_LAUNCHED();
     return 0;
 }

@@ -444,6 +444,33 @@ def essential_score(pts1, pts2, E, threshold=0.0005, want_err=False):
     return counts[:M], err
 
 
+def fundamental_8point(pts1, pts2, N, rec=None):
+    """cv2.findFundamentalMat(pts1[:N], pts2[:N], method=cv2.FM_8POINT) on the device (N: [1] int32 device count), the points
+    cast to fp32 first as cv2 does: -> (record buffer, mask [capacity] u8, all ones over the first N rows when N >= 7).  The
+    record's E holds F (1 candidate, or 1..3 when N == 7); ``recover_pose`` runs on it as on essential_ransac's record."""
+    need_cuda(pts1, pts2, N)
+    dev = pts1.device
+    cap = int(pts1.shape[0])
+    rec = pose_record(dev) if rec is None else rec
+    mask = torch.zeros(max(cap, 1), device=dev, dtype=torch.uint8)
+    wsz = lib.rf_fundamental_8point_workspace(cap)
+    ws = torch.empty(wsz, device=dev, dtype=torch.uint8)
+    check(lib.rf_fundamental_8point(ptr(pts1), ptr(pts2), cap, ptr(N), ptr(rec), ptr(mask), ptr(ws), wsz, stream()))
+    return rec, mask
+
+
+def fundamental_moments(pts1, pts2, N):
+    """The reductions of fundamental_8point alone (N = N[0] >= 1): [51] fp64 = (m1c, m2c, scale1, scale2, A's upper triangle
+    row by row) over the first N rows."""
+    need_cuda(pts1, pts2, N)
+    cap = int(pts1.shape[0])
+    out = torch.full((51,), float("nan"), device=pts1.device, dtype=torch.float64)
+    wsz = lib.rf_fundamental_8point_workspace(cap)
+    ws = torch.empty(wsz, device=pts1.device, dtype=torch.uint8)
+    check(lib.rf_fundamental_moments(ptr(pts1), ptr(pts2), cap, ptr(N), ptr(out), ptr(ws), wsz, stream()))
+    return out
+
+
 # --------------------------------------------------------------------------- warp
 def warp_grid(H, h, w):
     need_cuda(H)

@@ -130,6 +130,45 @@ def yfcc_pose(flowGlobal, match_binary, size_A, size_B, angle, K_A, K_B, org_A, 
     return (r["R"], r["t"]), r["n_points"]
 
 
+def yfcc_pose_8point(flowGlobal, match_binary, size_A, size_B, angle, K_A, K_B, org_A, org_B):
+    """``yfcc_pose`` on the driver's non-RANSAC branch (getResults.py without --ransac): cv2.findFundamentalMat(FM_8POINT) and
+    cv2.recoverPose over its stacked candidates, every stage on the current stream; the host reads one record at the end.
+    Returns ((R, t) or None, match count)."""
+    flowGlobal = torch.as_tensor(flowGlobal).cuda()
+    match_binary = torch.as_tensor(match_binary).cuda()
+    n1 = _norm_params(org_A, size_A, np.asarray(K_A, dtype=np.float64))
+    n2 = _norm_params(org_B, size_B, np.asarray(K_B, dtype=np.float64))
+    pts1, pts2, N = ops.yfcc_matches(flowGlobal, match_binary, angle, size_A, size_B, n1, n2)
+    rec, mask = ops.fundamental_8point(pts1, pts2, N)
+    ops.recover_pose(pts1, pts2, mask, rec)
+    r = ops.read_pose_record(rec)
+    if r["status"] != ops.POSE_OK or r["pose_count"] <= 0:
+        return None, r["n_points"]
+    return (r["R"], r["t"]), r["n_points"]
+
+
+def opencv_decompose(pts1, pts2, ransac, threshold=0.0005):
+    """getResults.py:75-111 on the device, both branches: ransac=True cv2.findEssentialMat(RANSAC, threshold), ransac=False
+    cv2.findFundamentalMat(FM_8POINT), then cv2.recoverPose over the stacked candidates.  pts1 / pts2: (N, 2) normalised points
+    (numpy or torch).  Returns ((R, t) or None, mask_final) as the driver does; mask_final is the winning candidate's recoverPose
+    mask, (N, 1) uint8 on the device, or None.  (The driver's own mask_final aliases the array cv2 writes in place, so with
+    stacked candidates it ends as the last candidate's mask; the driver never reads it.)  The host reads one record."""
+    dev = torch.device("cuda", torch.cuda.current_device())
+    P1 = torch.as_tensor(np.asarray(pts1) if not torch.is_tensor(pts1) else pts1).to(dev, torch.float64).reshape(-1, 2).contiguous()
+    P2 = torch.as_tensor(np.asarray(pts2) if not torch.is_tensor(pts2) else pts2).to(dev, torch.float64).reshape(-1, 2).contiguous()
+    N = int(P1.shape[0])
+    Nd = torch.tensor([N], dtype=torch.int32, device=dev)
+    if ransac:
+        rec, mask = ops.essential_ransac(P1, P2, Nd, threshold)
+    else:
+        rec, mask = ops.fundamental_8point(P1, P2, Nd)
+    out, _ = ops.recover_pose(P1, P2, mask, rec)
+    r = ops.read_pose_record(rec)
+    if r["status"] != ops.POSE_OK or r["pose_count"] <= 0:
+        return None, None
+    return (r["R"], r["t"]), out[:N].view(N, 1)
+
+
 def _norm_params(org_size, new_size, K):
     """norm_kp's (cx, cy, fx, fy) (getResults.py:29-50), in its statement order."""
     w, h = org_size
@@ -171,6 +210,23 @@ def yfcc_pose_errors(pairs_ids, finePath, coarsePath, maskPath, rotation, R_list
     a pair with no files, no matches or no model.  ``R_list`` / ``T_list`` / ``K_list`` / ``org_imsizes`` are what the driver
     reads from its calibration files (``T_list[i]`` as the driver's ``np.array(calib['T']).T``), ``resized_shapes`` its
     getResizedSize per image, ``rotation`` the loaded rotation.json."""
+    def pose(*args):
+        return yfcc_pose(*args, ransac=ransac, threshold=threshold)
+    return _pose_errors(pose, pairs_ids, finePath, coarsePath, maskPath, rotation, R_list, T_list, K_list, org_imsizes,
+                        resized_shapes, multiH, th, flowList)
+
+
+def yfcc_pose_errors_8point(pairs_ids, finePath, coarsePath, maskPath, rotation, R_list, T_list, K_list, org_imsizes,
+                            resized_shapes, multiH=True, th=0.95, flowList=None):
+    """``yfcc_pose_errors`` on the driver's non-RANSAC branch (getResults.py run without --ransac), through
+    ``yfcc_pose_8point``."""
+    return _pose_errors(yfcc_pose_8point, pairs_ids, finePath, coarsePath, maskPath, rotation, R_list, T_list, K_list, org_imsizes,
+                        resized_shapes, multiH, th, flowList)
+
+
+def _pose_errors(pose, pairs_ids, finePath, coarsePath, maskPath, rotation, R_list, T_list, K_list, org_imsizes, resized_shapes,
+                 multiH, th, flowList):
+    """The per-pair loop of getResults.py:298-331 with ``pose`` = the pose estimate of one pair."""
     if flowList is None:
         flowList = [item for item in os.listdir(finePath) if "flow" in item]
     res = []
@@ -181,8 +237,8 @@ def yfcc_pose_errors(pairs_ids, finePath, coarsePath, maskPath, rotation, R_list
             continue
         r = R_list[idB] @ R_list[idA].T
         t = T_list[idB] - r @ T_list[idA]
-        decomposed, n = yfcc_pose(flow, match, resized_shapes[idA], resized_shapes[idB], rotation[str(i)], K_list[idA], K_list[idB],
-                                  org_imsizes[idA], org_imsizes[idB], ransac=ransac, threshold=threshold)
+        decomposed, n = pose(flow, match, resized_shapes[idA], resized_shapes[idB], rotation[str(i)], K_list[idA], K_list[idB],
+                             org_imsizes[idA], org_imsizes[idB])
         if n == 0 or decomposed is None:
             res.append(180)
         else:

@@ -4,7 +4,11 @@ calls as ``results.yfcc_pose`` (match buffers of H * W rows, N on the device), w
 runs after warm-up).  Reports the RANSAC iterations used, the models scored, and fp64 Sampson evaluations per second; times
 cv2.findEssentialMat + cv2.recoverPose on the same points when cv2 is importable.
 
-    python tools/yfcc_pose_profile.py [--reps 10] [--out results.json]
+    python tools/yfcc_pose_profile.py [--reps 10] [--out results.json] [--method ransac|8point]
+
+``--method 8point`` times the non-RANSAC branch instead (results.yfcc_pose_8point's calls): the three moment passes and the
+one-warp tail of rf_fundamental_8point alone, and the whole matches + findFundamentalMat + recoverPose path, next to
+cv2.findFundamentalMat + cv2.recoverPose when cv2 is importable.
 """
 import argparse
 import json
@@ -57,6 +61,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--out", default=None, help="also write the rows as JSON here")
+    ap.add_argument("--method", default="ransac", choices=["ransac", "8point"])
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device")
@@ -68,6 +73,8 @@ def main():
     except ImportError:
         cv2 = None
     rows = []
+    if args.method == "8point":
+        return profile_8point(args, ops, q, cv2)
     for N in (10000, 100000, 300000):
         for outlier in (0.1, 0.5):
             flow, mask, norm = flow_inputs(N, outlier, seed=N + int(outlier * 10))
@@ -114,6 +121,70 @@ def main():
             rows.append(row)
             print(json.dumps(row), flush=True)
     res = dict(gpu=q, rows=rows)
+    if args.out:
+        with open(args.out, "w") as f:
+            json.dump(res, f, indent=1)
+    print(q)
+
+
+def cuda_median(fn, reps):
+    for _ in range(3):
+        fn()
+    torch.cuda.synchronize()
+    times = []
+    for _ in range(reps):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        b.synchronize()
+        times.append(a.elapsed_time(b))
+    return float(np.median(times))
+
+
+def profile_8point(args, ops, q, cv2):
+    lib, ptr = rf._lib.lib, rf._lib.ptr
+    rows = []
+    size = (W_IMG, H_IMG)
+    for N in (10000, 100000, 300000):
+        flow, mask, norm = flow_inputs(N, 0.3, seed=N + 3)
+        pts1, pts2, Nd = ops.yfcc_matches(flow, mask, 0, size, size, norm, norm)
+        cap = int(pts1.shape[0])
+        rec = ops.pose_record(pts1.device)
+        m = torch.zeros(cap, device=pts1.device, dtype=torch.uint8)
+        wsz = lib.rf_fundamental_8point_workspace(cap)
+        ws = torch.empty(wsz, device=pts1.device, dtype=torch.uint8)
+        out = torch.empty(51, device=pts1.device, dtype=torch.float64)
+        st = rf._lib.stream()
+
+        def fundamental():
+            rf._lib.check(lib.rf_fundamental_8point(ptr(pts1), ptr(pts2), cap, ptr(Nd), ptr(rec), ptr(m), ptr(ws), wsz, st))
+
+        def moments():
+            rf._lib.check(lib.rf_fundamental_moments(ptr(pts1), ptr(pts2), cap, ptr(Nd), ptr(out), ptr(ws), wsz, st))
+
+        def whole():
+            p1, p2, n = ops.yfcc_matches(flow, mask, 0, size, size, norm, norm)
+            r, mk = ops.fundamental_8point(p1, p2, n)
+            ops.recover_pose(p1, p2, mk, r)
+            return r
+
+        t_f, t_m, t_all = cuda_median(fundamental, args.reps), cuda_median(moments, args.reps), cuda_median(whole, args.reps)
+        r = ops.read_pose_record(whole())
+        assert int(Nd) == N and r["status"] == ops.POSE_OK
+        row = dict(N=N, outlier=0.3, fundamental_8point_ms=t_f, moment_passes_ms=t_m, tail_ms_estimate=t_f - t_m,
+                   yfcc_pose_8point_path_ms=t_all, pose_count=r["pose_count"])
+        if cv2 is not None:
+            p1, p2 = pts1[:N].cpu().numpy(), pts2[:N].cpu().numpy()
+            t0 = time.perf_counter()
+            F, mc = cv2.findFundamentalMat(p1, p2, method=cv2.FM_8POINT)
+            t1 = time.perf_counter()
+            cv2.recoverPose(F[:3], p1, p2, mask=mc)
+            t2 = time.perf_counter()
+            row.update(cv2_findFundamentalMat_s=t1 - t0, cv2_recoverPose_s=t2 - t1)
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+    res = dict(gpu=q, method="8point", rows=rows)
     if args.out:
         with open(args.out, "w") as f:
             json.dump(res, f, indent=1)
