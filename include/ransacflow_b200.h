@@ -332,13 +332,17 @@ int rf_yfcc_matches(const float* flow, const uint8_t* mask, int H, int W, int k,
  * subsets, every real five-point solution of each (ascending root), OpenCV's Sampson error cast to fp32 against (float)(t * t),
  * and RANSACPointSetRegistrator::run's sequential best / iteration-budget update, scored 64 iterations per launch (a launch past
  * the budget exits at once: a fixed launch sequence, graph-capturable).  pts [capacity][2], N = *N_dev <= capacity.
- * Writes rec (status, E, counts) and mask_out[N] (the best E's inliers; all ones when N == 5). */
+ * Writes rec (status, E, counts) and mask_out[N] (the best E's inliers; all ones when N == 5).
+ * ws holds four segments, each starting at a multiple of 256 bytes after the one before it: idx [1000][5] int32 (the subset
+ * table; untouched when N < 5, row 0 only when N == 5), candE [1000][10][9] fp64 (the solutions of each subset), ncand [1000]
+ * int32 (their count), counts [1000][10] int32 (Sampson inlier counts; zero for launches past the budget). */
 size_t rf_essential_ransac_workspace(int capacity);
 int rf_essential_ransac(const double* pts1, const double* pts2, int capacity, const int* N_dev, double threshold,
                         rf_pose_record_t* rec, uint8_t* mask_out, void* ws, size_t ws_bytes, void* stream);
 /* cv2.recoverPose(E, pts1, pts2, mask=mask_in) for each stacked E of rec (distance threshold 50), with the driver's loop
  * (:96-104): cv2 writes each call's mask into mask_in, so candidate c + 1 starts from candidate c's output, and the first
- * candidate with the strictly largest count wins.  Writes rec (R, t, pose_count, status) and mask_out[N] (the winner's mask).
+ * candidate with the strictly largest count wins.  Writes rec (R, t, pose_count, status) and mask_out[N] whatever the status:
+ * the winner's mask, or zeros when no candidate wins (RF_POSE_NO_POSE) or rec holds no E (RF_POSE_TOO_FEW, RF_POSE_NO_MODEL).
  * The first 8 * capacity bytes of ws hold the per-point cheirality bits: bit 4 c + p = pose p of candidate c passes. */
 size_t rf_recover_pose_workspace(int capacity);
 int rf_recover_pose(const double* pts1, const double* pts2, int capacity, const uint8_t* mask_in, rf_pose_record_t* rec,

@@ -791,10 +791,11 @@ __global__ void pose_select_kernel(const uint8_t* __restrict__ mask_in, int capa
     }
 }
 
-// single-candidate mask: the chosen pose's bits ANDed with the input mask
+// single-candidate mask: the chosen pose's bits ANDed with the input mask.  Every other outcome that pose_select_kernel
+// left unwritten (no stacked candidate won, or no E to start from) gets zeros: what cv2's mask= array holds when every count is 0
 __global__ void pose_mask_kernel(const uint8_t* __restrict__ mask_in, int capacity, const rf_pose_record_t* __restrict__ rec,
                                  const unsigned long long* __restrict__ bits, uint8_t* __restrict__ mask_out) {
-    if (rec->n_E != 1) return;
+    if (rec->n_E > 1 && rec->status == RF_POSE_OK) return;   // the winner's chained mask, written by pose_select_kernel
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= rec->n_points || i >= capacity) return;
     const int p = rec->pose_index;

@@ -100,7 +100,8 @@ def test_end_to_end_against_oracle(rf, s):
         assert len(A) == len(B) and all(np.abs(B - e).max(axis=1).min() < 1e-9 for e in A)
         assert mask.all()
         return
-    # the replay: the oracle's sequential rule on the device's own candidates and counts gives the device's best and budget
+    # the device's best and budget against the oracle's own run; the replay of the device's own candidates and counts, launch
+    # by launch, is test_gpu_pose_stages.py's test_ransac_stages_bit_exact
     E_dev = PO.canonical(rec["E"].reshape(-1, 9))[0]
     same = np.abs(E_dev - r["E"][0]).max() < 1e-7
     if not same:
