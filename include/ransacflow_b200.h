@@ -233,6 +233,14 @@ int rf_lanczos_coeffs_host(int in_size, int out_size, int* bounds_host, int* kk_
 /* The same tables for PIL's BILINEAR filter (triangle, support 1): Image.resize(size, BILINEAR) through rf_resample_u8, the
  * resize of segNet/segData.py:7-17,71 (called from :53-76 getImg). */
 int rf_bilinear_coeffs_host(int in_size, int out_size, int* bounds_host, int* kk_host, int kk_capacity, int* ksize_out);
+/* The byte-scaling step of SciPy 1.2's imresize on a float32 map, as the drivers' `imresize(It_bg, (h, w)) < 128` runs it
+ * (evaluation/evalHpatch/evaluation.py:180, evalCorr:187, evalYFCC:200/212, evalKITTI:248), after np.rot90 of the map:
+ * out (uint8, [W][H] for odd rot, else [H][W]) = scipy.misc.bytescale(np.rot90(map [H][W], rot)), i.e. in fp32
+ * clip((x - cmin) * (255 / span), 0, 255) + 0.5 truncated, span = cmax - cmin or 1 when the map is constant.  cmin / cmax are
+ * reduced on the device (two launches, no host read, graph-capturable, deterministic); NaN-free maps.  The PIL BILINEAR
+ * resize that follows is rf_resample_u8 with channels = 1 and the rf_bilinear_coeffs_host tables. */
+size_t rf_bytescale_mask_u8_workspace(int H, int W);
+int rf_bytescale_mask_u8(const float* map, int H, int W, int rot, uint8_t* out, void* ws, size_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------ segNet --
  * The decoder of the ADE20K scene-parsing network (segNet/segModel.py:218-264 PPMDeepsup, inference) and the multi-scale vote of

@@ -46,6 +46,8 @@ SIGNATURES = {
     "rf_resample_u8": (i32, [vp, i32, i32, i32, i32, vp, vp, i32, i32, vp, vp]),
     "rf_lanczos_coeffs_host": (i32, [i32, i32, vp, vp, i32, vp]),
     "rf_bilinear_coeffs_host": (i32, [i32, i32, vp, vp, i32, vp]),
+    "rf_bytescale_mask_u8_workspace": (sz, [i32, i32]),
+    "rf_bytescale_mask_u8": (i32, [vp, i32, i32, i32, vp, vp, sz, vp]),
     "rf_adaptive_avgpool_split": (i32, [vp, i32, vp, i32, vp, i32, vp, vp]),
     "rf_ppm_concat_split": (i32, [vp, i32, vp, i32, vp, vp, i32, i32, vp, vp]),
     "rf_seg_vote": (i32, [vp, i32, vp, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp, vp]),

@@ -1604,3 +1604,101 @@ extern "C" int rf_fill_nearest_matched(const float* flow, const uint8_t* matched
     RF_LAUNCHED();
     return 0;
 }
+
+// scipy.misc.bytescale(np.rot90(map, rot)) as SciPy 1.2's imresize computes it on a float32 map (the drivers'
+// `imresize(It_bg, (h, w)) < 128` before its PIL resize).  Two launches, no host read, so the call can be captured in a CUDA
+// graph: (1) every CTA reduces a strided slice of the map to its (min, max); (2) every CTA reduces those partials in one fixed
+// order (min / max are exact, so any order gives the same bits) and byte-scales its output pixels in fp32:
+//   span = cmax - cmin (1 when 0); scale = 255 / span; v = clip((x - cmin) * scale, 0, 255) + 0.5; out = (uint8)v.
+// NaN-free maps only (fminf / fmaxf drop a NaN where numpy propagates it).
+#define RF_BYTESCALE_PARTS 256
+#define RF_BYTESCALE_THREADS 256
+
+static __device__ __forceinline__ float2 minmax_block(float lo, float hi, float2* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+        hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) red[warp] = make_float2(lo, hi);
+    __syncthreads();
+    if (warp == 0) {
+        float2 v = lane < (RF_BYTESCALE_THREADS >> 5) ? red[lane] : make_float2(INFINITY, -INFINITY);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            v.x = fminf(v.x, __shfl_xor_sync(0xffffffffu, v.x, o));
+            v.y = fmaxf(v.y, __shfl_xor_sync(0xffffffffu, v.y, o));
+        }
+        if (lane == 0) red[0] = v;
+    }
+    __syncthreads();
+    return red[0];
+}
+
+__global__ void __launch_bounds__(RF_BYTESCALE_THREADS) bytescale_minmax_kernel(const float* __restrict__ x, long long n, float2* __restrict__ part) {
+    __shared__ float2 red[RF_BYTESCALE_THREADS / 32];
+    float lo = INFINITY, hi = -INFINITY;
+    for (long long i = (long long)blockIdx.x * RF_BYTESCALE_THREADS + threadIdx.x; i < n; i += (long long)gridDim.x * RF_BYTESCALE_THREADS) {
+        const float v = __ldg(x + i);
+        lo = fminf(lo, v);
+        hi = fmaxf(hi, v);
+    }
+    const float2 r = minmax_block(lo, hi, red);
+    if (threadIdx.x == 0) part[blockIdx.x] = r;
+}
+
+// out [Ho][Wo] = bytescale(np.rot90(x [H][W], rot)); rot 1: out[i][j] = x[j][W-1-i], 2: x[H-1-i][W-1-j], 3: x[H-1-j][i]
+__global__ void __launch_bounds__(RF_BYTESCALE_THREADS) bytescale_rot_kernel(const float* __restrict__ x, int H, int W, int rot,
+                                                                            const float2* __restrict__ part, int nparts, uint8_t* __restrict__ out) {
+    __shared__ float2 red[RF_BYTESCALE_THREADS / 32];
+    float lo = INFINITY, hi = -INFINITY;
+    for (int p = threadIdx.x; p < nparts; p += RF_BYTESCALE_THREADS) {
+        const float2 v = part[p];
+        lo = fminf(lo, v.x);
+        hi = fmaxf(hi, v.y);
+    }
+    const float2 mm = minmax_block(lo, hi, red);
+    const float cmin = mm.x;
+    const float span = __fsub_rn(mm.y, mm.x);
+    const float scale = span == 0.f ? 255.f : __fdiv_rn(255.f, span);
+    const int Ho = (rot & 1) ? W : H, Wo = (rot & 1) ? H : W;
+    const long long n = (long long)Ho * Wo;
+    for (long long o = (long long)blockIdx.x * RF_BYTESCALE_THREADS + threadIdx.x; o < n; o += (long long)gridDim.x * RF_BYTESCALE_THREADS) {
+        const int i = (int)(o / Wo), j = (int)(o - (long long)i * Wo);
+        int r, c;
+        switch (rot) {
+            case 1: r = j; c = W - 1 - i; break;
+            case 2: r = H - 1 - i; c = W - 1 - j; break;
+            case 3: r = H - 1 - j; c = i; break;
+            default: r = i; c = j; break;
+        }
+        float v = __fmul_rn(__fsub_rn(__ldg(x + (long long)r * W + c), cmin), scale);
+        v = fminf(fmaxf(v, 0.f), 255.f);
+        out[o] = (uint8_t)(int)__fadd_rn(v, 0.5f);
+    }
+}
+
+extern "C" size_t rf_bytescale_mask_u8_workspace(int H, int W) {
+    (void)H;
+    (void)W;
+    return RF_BYTESCALE_PARTS * sizeof(float2) + 256;
+}
+
+extern "C" int rf_bytescale_mask_u8(const float* map, int H, int W, int rot, uint8_t* out, void* ws, size_t ws_bytes, void* stream) {
+    RF_REQUIRE(map != nullptr && out != nullptr && H >= 1 && W >= 1 && rot >= 0 && rot <= 3,
+               "rf_bytescale_mask_u8: need a non-empty map, an output and 0 <= rot <= 3");
+    RF_REQUIRE(ws != nullptr && ws_bytes >= rf_bytescale_mask_u8_workspace(H, W), "rf_bytescale_mask_u8: workspace too small");
+    const long long n = (long long)H * W;
+    float2* part = reinterpret_cast<float2*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
+    long long want = (n + 4 * RF_BYTESCALE_THREADS - 1) / (4 * RF_BYTESCALE_THREADS);       // >= 4 elements per thread
+    const int nparts = (int)(want < 1 ? 1 : (want > RF_BYTESCALE_PARTS ? RF_BYTESCALE_PARTS : want));
+    cudaStream_t st = as_stream(stream);
+    bytescale_minmax_kernel<<<nparts, RF_BYTESCALE_THREADS, 0, st>>>(map, n, part);
+    RF_LAUNCHED();
+    long long blocks = (n + RF_BYTESCALE_THREADS - 1) / RF_BYTESCALE_THREADS;
+    if (blocks > 1024) blocks = 1024;
+    bytescale_rot_kernel<<<(unsigned)blocks, RF_BYTESCALE_THREADS, 0, st>>>(map, H, W, rot, part, nparts, out);
+    RF_LAUNCHED();
+    return 0;
+}

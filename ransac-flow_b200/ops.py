@@ -603,3 +603,39 @@ def _resize_u8(img, out_w, out_h, fn):
         check(lib.rf_resample_u8(ptr(cur), H, W, ch, 0, ptr(b), ptr(k), ks, out_h, ptr(nxt), stream()))
         cur = nxt
     return cur
+
+
+# --------------------------------------------------------------------------- the drivers' background-mask resize
+def bytescale_mask_u8(m, rot=0):
+    """``scipy.misc.bytescale(np.rot90(m, rot))`` of a float32 (H, W) CUDA map, as SciPy 1.2's ``imresize`` (``dropin.imresize``)
+    byte-scales it: uint8 (H, W), or (W, H) for an odd ``rot``.  Min and max are reduced on the device (graph-capturable)."""
+    need_cuda(m)
+    assert m.dim() == 2 and m.dtype == torch.float32, (m.dim(), m.dtype)
+    m = m.contiguous()
+    H, W = int(m.shape[0]), int(m.shape[1])
+    k = int(rot) % 4
+    out = torch.empty((W, H) if k % 2 else (H, W), device=m.device, dtype=torch.uint8)
+    wsz = lib.rf_bytescale_mask_u8_workspace(H, W)
+    ws = torch.empty(wsz, device=m.device, dtype=torch.uint8)
+    check(lib.rf_bytescale_mask_u8(ptr(m), H, W, k, ptr(out), ptr(ws), wsz, stream()))
+    return out
+
+
+def imresize_keep(m, h, w, rot=0):
+    """``imresize(np.rot90(m, rot), (h, w)) < 128`` as a bool (h, w) CUDA tensor (True = kept, not background).  ``m``: a float32
+    (H, W) map, CUDA or host (copied to the current device)."""
+    if not torch.is_tensor(m):
+        m = torch.from_numpy(np.ascontiguousarray(m, dtype=np.float32))
+    if not m.is_cuda:
+        m = m.to(device=torch.device("cuda", torch.cuda.current_device()), dtype=torch.float32)
+    u8 = bytescale_mask_u8(m, rot)
+    r = _resize_u8(u8.view(u8.shape[0], u8.shape[1], 1), int(w), int(h), "rf_bilinear_coeffs_host")     # PIL BILINEAR, mode L
+    return (r < 128).view(int(h), int(w))
+
+
+def imresize_mask(m, h, w, rot=0):
+    """``(dropin.imresize(np.rot90(m, rot), (h, w)) < 128).astype(np.float32)`` on the device: a float32 (h, w) CUDA tensor,
+    1 = kept.  The background map of evaluation/evalHpatch/evaluation.py:180, evalCorr:187, evalYFCC:200/212, evalKITTI:248:
+    byte-scaling (``rf_bytescale_mask_u8``), then PIL's BILINEAR passes (``rf_resample_u8``, skipped where a side keeps its
+    size), then the comparison.  No host read: it can be captured in a CUDA graph once its resampling tables exist."""
+    return imresize_keep(m, h, w, rot).float()

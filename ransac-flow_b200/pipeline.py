@@ -173,6 +173,9 @@ class GraphedAligner:
     def _programs(self):
         """Every LayerProgram whose cached activation buffers a captured graph of this aligner points into."""
         progs = [p for p in (self.coarse.net.program, self.coarse.net._program_f16, self.coarse.net._program_split) if p is not None]
+        seg = getattr(self.coarse, "segNet", None)
+        if seg is not None:                     # segNet's encoder and head programs (used by the graphs of a segNet aligner)
+            progs += [seg.encoder, seg.head]
         for m in self.net.values():
             progs += list(getattr(m, "_fold", {}).values())
         return progs
@@ -209,14 +212,14 @@ class GraphedAligner:
             g.register_generator_state(self.generator)
         n0 = _lib.launch_count()
         with torch.cuda.graph(g):
-            packed, flow12, size, f8shape = self._device(s_in, t_in)
+            packed, flow12, size, f8shape, *aux = self._device(s_in, t_in)
         # the compiled program entries (activation buffers) this graph's kernels point into: every entry whose image-set
         # signature the warm-up / capture of THIS input size touched
         touched = {(id(p), k) for p in self._programs() for k in p._compiled if k in p.__dict__.get("_touched", ())}
         for p in self._programs():
             p.__dict__["_touched"] = set()
         return dict(n_kernels=_lib.launch_count() - n0, graph=g, s_in=s_in, t_in=t_in, packed=packed, flow12=flow12, size=size, f8shape=f8shape,
-                    prog_keys=touched)
+                    prog_keys=touched, bg=aux[0] if aux else None)
 
     def prepare(self, Is, It):
         """Capture (once) the graph for this pair of input sizes; returns its record."""
@@ -247,6 +250,10 @@ class GraphedAligner:
         if "host" not in c:
             c["host"] = torch.empty(c["packed"].numel(), dtype=c["packed"].dtype).pin_memory()
         c["host"].copy_(c["packed"].reshape(-1), non_blocking=True)
+        if c["bg"] is not None:                                # the background map: a uint8 buffer of its own
+            if "host_bg" not in c:
+                c["host_bg"] = torch.empty(c["bg"].numel(), dtype=torch.uint8).pin_memory()
+            c["host_bg"].copy_(c["bg"].reshape(-1), non_blocking=True)
         done = torch.cuda.Event()
         done.record()
         return (c, done)
@@ -258,14 +265,28 @@ class GraphedAligner:
         c, done = ticket
         done.synchronize()
         f12 = c["flow12"]
-        return self._unpack(c["host"].numpy().copy(), (f12.clone() if copy else f12) if f12 is not None else None, c["size"], c["f8shape"])
+        out = self._unpack(c["host"].numpy().copy(), (f12.clone() if copy else f12) if f12 is not None else None, c["size"], c["f8shape"])
+        if c["bg"] is not None:
+            out["It_bg"] = c["host_bg"].numpy().reshape(c["size"]).astype(bool)
+        return out
 
     def __call__(self, Is, It, copy=True):
         """Is, It: uint8 (H, W, 3) torch tensors (CUDA, or pinned host for an asynchronous H2D) or numpy arrays."""
         return self.fetch(self.enqueue(Is, It), copy)
 
 
-def _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_match21, samples=None):
+def _sky_background(coarseModel, It):
+    """evaluation/evalCorr/evaluation.py:184-189 on the device: segNet's mask of the original target ``It`` (a path, PIL image or
+    uint8 (H, W, 3) CUDA tensor), resized to the resized target like ``imresize(It_bg, (h, w)) < 128``.  Returns the bool
+    (h, w) CUDA map (True = kept).  Nothing is read back to the host."""
+    seg = getattr(coarseModel, "segNet", None)
+    if seg is None:
+        raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
+    Itw, Ith = coarseModel.target_size
+    return ops.imresize_keep(seg.run(It)[0], Ith, Itw)
+
+
+def _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_match21, samples=None, segNet=False):
     """The multi-hypothesis loop of evaluation/evalCorr/evaluation.py:211-243 with NO host control at all: every one of the
     ``maxCoarse + 1`` iterations is queued unconditionally; what the reference decides on the host - stop at the first failed
     RANSAC (:215-216), stop at the first hypothesis whose new-region matchability mean is below ``maskRegionTh`` (:226), update
@@ -273,17 +294,25 @@ def _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_ma
     after the first dead one when it unpacks.  Accepted hypotheses are computed from exactly the state the reference's loop
     would have had; dead ones are wasted work (none when every hypothesis is accepted, the common case at maxCoarse = 10).
     One packed result tensor: per hypothesis [alive, status, nbMatch, nbInlier, H(9), flowDown8, matchDown8] - the tensors
-    the drivers save (evaluation.py:244-260); the full-resolution maps stay on the device and are not returned."""
+    the drivers save (evaluation.py:244-260); the full-resolution maps stay on the device and are not returned.
+    ``segNet`` (the drivers' ``--segNet``): the background map of the target (``_sky_background``) masks every hypothesis,
+    the first included (:211-243 with ``It_bg``); it is returned as a fifth item, a uint8 (h, w) CUDA map (1 = kept)."""
     box = {}
     coarseModel.setPair(Is, It)
     Itw, Ith = coarseModel.target_size
     dev = coarseModel.ItTensor.device
+    keep = _sky_background(coarseModel, It) if segNet else None
+    bg = keep.float() if segNet else None
     Mask = torch.zeros((Ith, Itw), device=dev)
     alive = torch.ones((), device=dev, dtype=torch.bool)
     recs, featt, f8shape = [], None, None
     for k in range(maxCoarse + 1):
-        fgMask = (Mask > 0.5).float()                                    # It_bg = 1 everywhere: (Mask + (1 - It_bg)) > 0.5
-        Hd, nb, mask, status, cnt = coarseModel.getCoarse_device(fgMask if k > 0 else None, None if samples is None else samples[k])
+        if bg is None:
+            fgMask = (Mask > 0.5).float()                                # It_bg = 1 everywhere: (Mask + (1 - It_bg)) > 0.5
+        else:
+            fgMask = ((Mask + (1 - bg)) > 0.5).float()
+        Hd, nb, mask, status, cnt = coarseModel.getCoarse_device(fgMask if k > 0 or bg is not None else None,
+                                                                 None if samples is None else samples[k])
         flowCoarse = ops.warp_grid(Hd.view(1, 3, 3), Ith, Itw)
         flow12, match, f8, mboth = PredFlowMask_device(coarseModel.IsTensor, featt, flowCoarse, (Ith, Itw), network, with_match21,
                                                        ItTensor=coarseModel.ItTensor, feat_box=box)
@@ -292,10 +321,13 @@ def _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_ma
         newreg = (match[0, 0] * (1 - fgMask)).mean()
         ok = (status[0] == 0) & ((newreg > maskRegionTh) if k > 0 else torch.ones((), device=dev, dtype=torch.bool))
         alive = alive & ok
-        matchFine = match[0, 0] if k == 0 else match[0, 0] * (1 - fgMask)
+        # (evaluation.py:235 masks from the first hypothesis on; without a background the first mask is all zeros)
+        matchFine = match[0, 0] if (k == 0 and bg is None) else match[0, 0] * (1 - fgMask)
         Mask = torch.where(alive, ((Mask + matchFine) >= 1.0).float(), Mask)
         recs.append(torch.cat([alive.float().reshape(1), status.float(), cnt.float(), nb.float(), Hd, f8.reshape(-1), mboth.reshape(-1)]))
         f8shape = tuple(f8.shape)
+    if segNet:
+        return torch.cat(recs), None, (Ith, Itw), f8shape, keep.view(torch.uint8)
     return torch.cat(recs), None, (Ith, Itw), f8shape
 
 
@@ -315,11 +347,16 @@ def _unpack_multi(host, size, f8shape, nhyp):
                 flow12=[], match=[], nbMatch=[int(v) for v in host[:n, 2]], nbInlier=[int(v) for v in host[:n, 3]])
 
 
-def align_pair_multi(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.01, with_match21=True, samples=None):
+def align_pair_multi(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.01, with_match21=True, samples=None, segNet=False):
     """``align_pair_device`` without any host round trip inside the loop (see ``_multi_device``): one pinned D2H at the end.
-    Returns H / flowDown8 / matchDown8 / nbMatch / nbInlier of the accepted hypotheses (what the drivers save)."""
-    packed, _, size, f8shape = _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_match21, samples)
-    return _unpack_multi(_to_host(packed).copy(), size, f8shape, maxCoarse + 1)
+    Returns H / flowDown8 / matchDown8 / nbMatch / nbInlier of the accepted hypotheses (what the drivers save).  ``segNet``:
+    the sky of the target is masked as the drivers' ``--segNet`` masks it (the ``coarseModel`` needs ``segNet=True``), and the
+    result has ``It_bg``, the (h, w) bool background map the drivers save as ``maskBG_*``."""
+    packed, _, size, f8shape, *aux = _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_match21, samples, segNet)
+    out = _unpack_multi(_to_host(packed).copy(), size, f8shape, maxCoarse + 1)
+    if segNet:
+        out["It_bg"] = _to_host(aux[0]).reshape(size).astype(bool)
+    return out
 
 
 class GraphedMultiAligner(GraphedAligner):
@@ -327,12 +364,16 @@ class GraphedMultiAligner(GraphedAligner):
     acceptance test, mask update)) as ONE CUDA graph per input size: ~0.6 k kernels per pair at maxCoarse = 10 with no host
     work between them.  BASELINE config 4 (evalCorr / evalYFCC semantics) is measured through it."""
 
-    def __init__(self, coarseModel, network, maxCoarse=10, maskRegionTh=0.01, with_match21=True, warmup=2, max_graphs=4):
+    def __init__(self, coarseModel, network, maxCoarse=10, maskRegionTh=0.01, with_match21=True, warmup=2, max_graphs=4, segNet=False):
+        """``segNet`` (the drivers' ``--segNet``): segNet and the background-map resize run inside the graph, every hypothesis
+        is masked with the background, and ``fetch`` also returns ``It_bg`` (``align_pair_multi(segNet=True)``)."""
+        if segNet and getattr(coarseModel, "segNet", None) is None:
+            raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
         super().__init__(coarseModel, network, with_match21=with_match21, warmup=warmup, max_graphs=max_graphs)
-        self.maxCoarse, self.maskRegionTh = maxCoarse, maskRegionTh
+        self.maxCoarse, self.maskRegionTh, self.segNet = maxCoarse, maskRegionTh, bool(segNet)
 
     def _device(self, s_in, t_in):
-        return _multi_device(self.coarse, self.net, s_in, t_in, self.maxCoarse, self.maskRegionTh, self.m21)
+        return _multi_device(self.coarse, self.net, s_in, t_in, self.maxCoarse, self.maskRegionTh, self.m21, segNet=self.segNet)
 
     def _unpack(self, host, flow12, size, f8shape):
         return _unpack_multi(host, size, f8shape, self.maxCoarse + 1)
@@ -526,11 +567,14 @@ YFCC_ANGLES = (0, 90, 180, 270)
 def yfcc_background(It_bg, k, size):
     """evaluation/evalYFCC/evaluation.py:193 / :200 / :212 for rotation ``k``: the segNet map of the unrotated target (or
     None: all ones) rotated by ``np.rot90``, resized by SciPy 1.2's ``imresize`` (byte-scaling) to ``size`` = (w, h),
-    ``< 128``.  float32 (h, w), 1 = kept (not sky)."""
+    ``< 128``.  float32 (h, w), 1 = kept (not sky): a CUDA tensor when ``It_bg`` is one (``ops.imresize_mask``, no host
+    copy), else a numpy array."""
     from .dropin import imresize
     w, h = size
     if It_bg is None:                      # imresize of a constant map byte-scales to 0: every cell < 128
         return np.ones((h, w), dtype=np.float32)
+    if torch.is_tensor(It_bg):
+        return ops.imresize_mask(It_bg, h, w, rot=k)
     return (imresize(np.rot90(np.asarray(It_bg, dtype=np.float32), k), (h, w)) < 128).astype(np.float32)
 
 
@@ -564,8 +608,8 @@ def align_pair_yfcc(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.0
       * the hypothesis loop of ``align_pair_device`` on the winning rotation: masked re-matching per ``getCoarse``,
         ``match12 * match21`` matchability (:32-62), 12 bytes per hypothesis to the host.
 
-    ``Is`` / ``It``: PIL images or uint8 (H, W, 3) CUDA tensors.  ``It_bg``: ``skyFromSeg`` of the unrotated target, or
-    None (no ``--segNet``).  ``samples``: optional injected (nbIter, 4) index tables, one per RANSAC call in the reference's
+    ``Is`` / ``It``: PIL images or uint8 (H, W, 3) CUDA tensors.  ``It_bg``: ``skyFromSeg`` of the unrotated target (a host
+    array, or the float32 CUDA mask of ``SegNet.run``, which then never leaves the device), or None (no ``--segNet``).  ``samples``: optional injected (nbIter, 4) index tables, one per RANSAC call in the reference's
     order.  Returns ``align_pair_device``'s dict plus ``angle``, ``nbInlierRot`` (the four scores) and ``It_bg`` (the
     resized boolean background map the driver saves as ``maskBG_``)."""
     with torch.no_grad():
@@ -576,6 +620,8 @@ def align_pair_yfcc(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.0
             rest = list(samples[calls:]) + [np.zeros((coarseModel.nbIter, coarseModel.nbPoint), dtype=np.int64)]
         out = _hypotheses_device(coarseModel, network, maxCoarse, maskRegionTh, True, bg, rest, rewind_too_few=True)
     w, h = coarseModel.target_size
+    if torch.is_tensor(bg):
+        bg = bg.cpu().numpy()
     out.update(angle=YFCC_ANGLES[best], nbInlierRot=nbInlierRot,
                It_bg=(bg if bg is not None else np.ones((h, w), dtype=np.float32)).astype(bool))
     return out
@@ -589,7 +635,13 @@ def _rotation_search(c, It_bg, samples):
         c._select_target(k)
         bg = yfcc_background(It_bg, k, c.rotated_target_size(k))
         bgs.append(bg)
-        m1, m2, _, cnt = c._match_device(((1 - bg) > 0.5).astype(np.float32) if It_bg is not None else None)
+        if It_bg is None:
+            Mt = None
+        elif torch.is_tensor(bg):
+            Mt = ((1 - bg) > 0.5).float()
+        else:
+            Mt = ((1 - bg) > 0.5).astype(np.float32)
+        m1, m2, _, cnt = c._match_device(Mt)
         found.append((m1, m2, cnt))
     counts = _to_host(torch.cat([f[2] for f in found])).copy()               # the one read the draw decision needs
     ran = rotation_draws(counts, c.nbPoint)
@@ -717,13 +769,16 @@ def remove_small_cc(matchFine, match_th, cc_th):
     return ops.remove_small_cc(m, match_th, cc_th).cpu().numpy()
 
 
-def align_pair_kitti(coarseModel, network, Is, It, fineSize=650, cc_th=0.01, maskRegionTh=0.005, maxH=None):
-    """One pair through evaluation/evalKITTI/evaluation.py:216-344 (no segNet, no file output): per hypothesis the coarse
+def align_pair_kitti(coarseModel, network, Is, It, fineSize=650, cc_th=0.01, maskRegionTh=0.005, maxH=None, It_bg=None):
+    """One pair through evaluation/evalKITTI/evaluation.py:216-344 (no file output): per hypothesis the coarse
     homography from ``coarseModel`` (variant A at ``coarseSize``), the first fine level on the half-size target, the
     second level on the ``fineSize`` target sampled on the ORIGINAL image's grid, small connected components of the
     matchability removed on the device, and the reference's mask update on the host.  ``Is`` / ``It``: PIL images.
-    ``maxH`` caps the reference's ``while True``.  Returns the four arrays the script saves (H (nH,3,3) 'Homograpy',
-    flow_d2 'Finetune_D2', mask 'Finetune_Mask', flow 'Finetune') plus the per-hypothesis full-resolution maps."""
+    ``maxH`` caps the reference's ``while True``.  ``It_bg``: with ``--segNet``, the raw ``skyFromSeg`` map of the target (host
+    array or CUDA tensor, :245-250), resized to the original size by ``ops.imresize_mask`` (byte-scaling; both PIL passes are
+    skipped); it masks every hypothesis and is returned as ``It_bg`` (bool, for ``results.save_pair_kitti``).  Returns the four
+    arrays the script saves (H (nH,3,3) 'Homograpy', flow_d2 'Finetune_D2', mask 'Finetune_Mask', flow 'Finetune') plus the
+    per-hypothesis full-resolution maps."""
     from . import outil
     strideNet = 8
     to_t = lambda I: coarseModel._to_tensor01(coarseModel._to_device_u8(I))          # transforms.ToTensor()(I)[None].cuda()
@@ -734,7 +789,11 @@ def align_pair_kitti(coarseModel, network, Is, It, fineSize=650, cc_th=0.01, mas
     (w_r, h_r), tensor_resize = It_resize.size, to_t(It_resize)
     (w_d2, h_d2), tensor_d2 = It_d2.size, to_t(It_d2)
     coarseModel.setPair(Is, It)
-    It_bg = np.ones((h_org, w_org), dtype=np.float32)
+    given = It_bg is not None
+    if given:                    # :248 (the reference's It_bg_tensor at the d2 size, :247, is never used)
+        It_bg = ops.imresize_mask(It_bg, h_org, w_org).cpu().numpy()
+    else:
+        It_bg = np.ones((h_org, w_org), dtype=np.float32)
     Mask = np.zeros((h_org, w_org), dtype=np.float32)
     Hs, D2, Msk, Fin, maps = [], [], [], [], []
     nbCoarse = 0
@@ -766,7 +825,10 @@ def align_pair_kitti(coarseModel, network, Is, It, fineSize=650, cc_th=0.01, mas
         else:
             break
     cat = lambda l: np.concatenate(l, axis=0) if l else np.zeros((0,))
-    return dict(H=cat(Hs), flow_d2=cat(D2), mask=cat(Msk), flow=cat(Fin), maps=maps, size=(h_org, w_org))
+    out = dict(H=cat(Hs), flow_d2=cat(D2), mask=cat(Msk), flow=cat(Fin), maps=maps, size=(h_org, w_org))
+    if given:
+        out["It_bg"] = It_bg.astype(bool)
+    return out
 
 
 def getFlow_all_kitti(param, flowd2, flow, match, outH, outW, th=1.0, cc_th=0.01, multiH=True, interpolate=False):

@@ -207,10 +207,17 @@ class SegNet:
         return mask, cls, scores
 
     def run(self, img, want_class=False, want_scores=False):
-        """The whole of getSky on the device: (mask, class map, scores) as in ``vote``."""
-        img = self.load(img)
-        W, H = img.size
-        u8 = torch.from_numpy(np.array(img, dtype=np.uint8)).to(self.device)
+        """The whole of getSky on the device: (mask, class map, scores) as in ``vote``.  ``img``: a path, a PIL image, or a uint8
+        (H, W, 3) CUDA tensor (RGB; nothing is read back, so the call can be captured in a CUDA graph)."""
+        if torch.is_tensor(img):
+            ops.need_cuda(img)
+            assert img.dtype == torch.uint8 and img.dim() == 3 and img.shape[2] == 3, (img.dtype, tuple(img.shape))
+            u8 = img
+            H, W = int(img.shape[0]), int(img.shape[1])
+        else:
+            img = self.load(img)
+            W, H = img.size
+            u8 = torch.from_numpy(np.array(img, dtype=np.uint8)).to(self.device)
         distinct, order = self.plan(H, W)
         with torch.no_grad():
             logits = self.conv_last(self.ppm(self.encode(self.resize(u8, distinct))))
