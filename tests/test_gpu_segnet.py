@@ -69,6 +69,18 @@ def test_dilated_conv_partial_n_tile(rf, d):
     dilated_check(rf, [(3, 5), (17, 40)], 64, 200, d, False, True, 7 + d)
 
 
+# segNet's own widths on its conv4 / conv5 maps (38 x 50 and 47 x 63 of a 480 x 640 image, 19 x 63 of a 376 x 1241 one) and on
+# a single pixel: 256 channels at dil 2 (4 K blocks of 64 per tap, 2 N tiles), 512 at dil 4 (8 K blocks, 4 N tiles), and the
+# first blocks of layer3 (dil 1) and layer4 (dil 2)
+SEGNET_MAPS = [(38, 50), (47, 63), (19, 63), (1, 1)]
+SEGNET_DILATED = [(256, 2, False), (256, 2, True), (512, 4, False), (512, 4, True), (256, 1, False), (512, 2, False)]
+
+
+@pytest.mark.parametrize("c,d,res", SEGNET_DILATED, ids=["c%d-d%d%s" % (c, d, "-res" if r else "") for c, d, r in SEGNET_DILATED])
+def test_dilated_conv_segnet_widths(rf, c, d, res):
+    dilated_check(rf, SEGNET_MAPS, c, c, d, res, True, 100 + c + 10 * d + res)
+
+
 def test_dilation_refused_outside_engine_4(rf):
     from ransac_flow_b200.model import FoldedConv
     from ransac_flow_b200.program import LayerProgram
