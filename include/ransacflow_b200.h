@@ -296,6 +296,19 @@ int rf_compose_fine_ex(const float* flowDown8, const float* match12, const float
  * area fraction count / (H*W) is <= cc_th gets its matchability zeroed; cc_th == 0 leaves the map untouched. */
 size_t rf_remove_small_cc_workspace(int H, int W);
 int rf_remove_small_cc(float* match, int N, int H, int W, float match_th, double cc_th, void* ws, size_t ws_bytes, void* stream);
+/* One hypothesis of evalKITTI's loop after remove_small_cc (evaluation/evalKITTI/evaluation.py:316-326), with the host's
+ * decisions kept on the device.  match, bg [H][W] fp32 (bg: 1 = kept); Mask, fgMask [H][W] fp32 {0, 1}, in / out; status
+ * (int32, RF_RANSAC_*) and alive (int32 flag, in / out) are device scalars.
+ *   count = #{p : match[p] > 0.9999f && fgMask[p] == 0}      (exact: both factors of the reference's product are 0 / 1)
+ *   alive = alive && status == 0 && (first || count >= cmin)
+ * and where alive holds, in fp32 as numpy evaluates it: Mask = ((Mask + match * (1 - fgMask)) > 0.9999f), then
+ * fgMask = ((Mask + (1 - bg)) > 0.5f).  Where it does not, Mask and fgMask are left untouched.  cmin is the smallest count the
+ * reference's float32 test `mean > maskRegionTh` accepts for an H*W map (found on the host).  rec (nullable, int32 [2]) receives
+ * {alive, count}.  Two launches (per-CTA partial counts, then a fixed-order reduction in every CTA + the update), no host read,
+ * no atomics: graph-capturable and deterministic. */
+size_t rf_kitti_region_step_workspace(int H, int W);
+int rf_kitti_region_step(const float* match, float* Mask, const float* bg, float* fgMask, int H, int W, const int* status, int* alive,
+                         int first, int cmin, int* rec, void* ws, size_t ws_bytes, void* stream);
 
 /* interpolate_flow_match, evaluation/evalKITTI/getResults.py:87-93: flow_out[p] = flow[nearest matched pixel of p]
  * (exact Euclidean distance; a matched pixel keeps its own flow).  flow / flow_out [H][W][2] (distinct buffers), matched

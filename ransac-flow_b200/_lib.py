@@ -60,6 +60,8 @@ SIGNATURES = {
     "rf_fill_nearest_matched": (i32, [vp, vp, i32, i32, vp, vp, vp, sz, vp]),
     "rf_remove_small_cc_workspace": (sz, [i32, i32]),
     "rf_remove_small_cc": (i32, [vp, i32, i32, i32, f32, C.c_double, vp, sz, vp]),
+    "rf_kitti_region_step_workspace": (sz, [i32, i32]),
+    "rf_kitti_region_step": (i32, [vp, vp, vp, vp, i32, i32, vp, vp, i32, i32, vp, vp, sz, vp]),
     "rf_yfcc_matches_workspace": (sz, [i32, i32]),
     "rf_yfcc_matches": (i32, [vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, sz, vp]),
     "rf_essential_ransac_workspace": (sz, [i32]),

@@ -1702,3 +1702,100 @@ extern "C" int rf_bytescale_mask_u8(const float* map, int H, int W, int rot, uin
     RF_LAUNCHED();
     return 0;
 }
+
+// One hypothesis of evalKITTI's loop after remove_small_cc (evaluation/evalKITTI/evaluation.py:316-326), with the host's
+// decisions turned into a device flag.  Two launches, no host read, no atomics, so the step can be captured in a CUDA graph and
+// gives the same bits every run:
+//   (1) every CTA counts the pixels of a strided slice with match > 0.9999 and fgMask == 0 (both factors of the reference's
+//       `(matchFine > 0.9999) * (1 - fgMask)` are 0 / 1, so the count is exact); block 0 also snapshots the incoming flag;
+//   (2) every CTA sums those partials in one fixed order, decides ok = status == 0 && (first || count >= cmin) and
+//       alive = alive_in && ok, and where alive holds rewrites its pixels in fp32 exactly as numpy evaluates them:
+//       Mask = ((Mask + match * (1 - fgMask)) > 0.9999), then fgMask = ((Mask + (1 - bg)) > 0.5).
+// Launch 2 reads the snapshot, never the flag it writes.  A dead hypothesis leaves Mask and fgMask untouched (its match may be
+// the NaN of a failed RANSAC's H = 0).
+#define RF_KITTI_PARTS 256
+#define RF_KITTI_THREADS 256
+
+static __device__ __forceinline__ int sum_block(int v, int* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    if (warp == 0) {
+        v = lane < (RF_KITTI_THREADS >> 5) ? red[lane] : 0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) red[0] = v;
+    }
+    __syncthreads();
+    return red[0];
+}
+
+__global__ void __launch_bounds__(RF_KITTI_THREADS) kitti_region_count_kernel(const float* __restrict__ match, const float* __restrict__ fg,
+                                                                             int n, const int* __restrict__ alive, int* __restrict__ part,
+                                                                             int* __restrict__ alive_prev) {
+    __shared__ int red[RF_KITTI_THREADS / 32];
+    int c = 0;
+    for (int i = blockIdx.x * RF_KITTI_THREADS + threadIdx.x; i < n; i += gridDim.x * RF_KITTI_THREADS)
+        c += (__ldg(match + i) > 0.9999f && __ldg(fg + i) == 0.f) ? 1 : 0;
+    c = sum_block(c, red);
+    if (threadIdx.x == 0) {
+        part[blockIdx.x] = c;
+        if (blockIdx.x == 0) *alive_prev = *alive;
+    }
+}
+
+__global__ void __launch_bounds__(RF_KITTI_THREADS) kitti_region_update_kernel(const float* __restrict__ match, float* __restrict__ Mask,
+                                                                              const float* __restrict__ bg, float* __restrict__ fg, int n,
+                                                                              const int* __restrict__ status, const int* __restrict__ alive_prev,
+                                                                              const int* __restrict__ part, int nparts, int first, int cmin,
+                                                                              int* __restrict__ alive, int* __restrict__ rec) {
+    __shared__ int red[RF_KITTI_THREADS / 32];
+    int c = 0;
+    for (int p = threadIdx.x; p < nparts; p += RF_KITTI_THREADS) c += part[p];
+    const int count = sum_block(c, red);
+    const bool live = *alive_prev != 0 && *status == 0 && (first || count >= cmin);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        *alive = live ? 1 : 0;
+        if (rec != nullptr) {
+            rec[0] = live ? 1 : 0;
+            rec[1] = count;
+        }
+    }
+    if (!live) return;
+    for (int i = blockIdx.x * RF_KITTI_THREADS + threadIdx.x; i < n; i += gridDim.x * RF_KITTI_THREADS) {
+        const float f = fg[i];
+        const float m = __fadd_rn(Mask[i], __fmul_rn(__ldg(match + i), __fsub_rn(1.f, f))) > 0.9999f ? 1.f : 0.f;
+        Mask[i] = m;
+        fg[i] = __fadd_rn(m, __fsub_rn(1.f, __ldg(bg + i))) > 0.5f ? 1.f : 0.f;
+    }
+}
+
+extern "C" size_t rf_kitti_region_step_workspace(int H, int W) {
+    (void)H;
+    (void)W;
+    return RF_KITTI_PARTS * sizeof(int) + 2 * 256;
+}
+
+extern "C" int rf_kitti_region_step(const float* match, float* Mask, const float* bg, float* fgMask, int H, int W, const int* status,
+                                    int* alive, int first, int cmin, int* rec, void* ws, size_t ws_bytes, void* stream) {
+    RF_REQUIRE(match != nullptr && Mask != nullptr && bg != nullptr && fgMask != nullptr && status != nullptr && alive != nullptr &&
+               H >= 1 && W >= 1, "rf_kitti_region_step: need non-empty maps, a status and an alive flag");
+    RF_REQUIRE((long long)H * W < (1ll << 31), "rf_kitti_region_step: map too large");
+    RF_REQUIRE(ws != nullptr && ws_bytes >= rf_kitti_region_step_workspace(H, W), "rf_kitti_region_step: workspace too small");
+    const int n = H * W;
+    int* part = reinterpret_cast<int*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255);
+    int* alive_prev = part + RF_KITTI_PARTS;
+    const int want = (n + 4 * RF_KITTI_THREADS - 1) / (4 * RF_KITTI_THREADS);       // >= 4 pixels per thread
+    const int nparts = want < 1 ? 1 : (want > RF_KITTI_PARTS ? RF_KITTI_PARTS : want);
+    cudaStream_t st = as_stream(stream);
+    kitti_region_count_kernel<<<nparts, RF_KITTI_THREADS, 0, st>>>(match, fgMask, n, alive, part, alive_prev);
+    RF_LAUNCHED();
+    int blocks = (n + RF_KITTI_THREADS - 1) / RF_KITTI_THREADS;
+    if (blocks > 1024) blocks = 1024;
+    kitti_region_update_kernel<<<blocks, RF_KITTI_THREADS, 0, st>>>(match, Mask, bg, fgMask, n, status, alive_prev, part, nparts, first,
+                                                                   cmin, alive, rec);
+    RF_LAUNCHED();
+    return 0;
+}

@@ -545,6 +545,28 @@ def remove_small_cc(match, match_th, cc_th):
     return match
 
 
+def kitti_region_step(match, Mask, bg, fgMask, status, alive, first, cmin, rec=None):
+    """One hypothesis of evaluation/evalKITTI/evaluation.py:316-326 on the device (``rf_kitti_region_step``): ``match``, ``bg``
+    (H, W) fp32; ``Mask`` / ``fgMask`` (H, W) fp32 updated in place where the hypothesis is accepted; ``status`` the RANSAC
+    status (int32 [1]); ``alive`` an int32 [1] flag, updated in place; ``cmin`` from ``pipeline.kitti_region_cmin``.  Returns
+    ``rec`` (int32 [2] = {alive, count}; allocated when None).  Nothing is read back: graph-capturable."""
+    need_cuda(match, Mask, bg, fgMask, status, alive, rec)
+    H, W = int(match.shape[-2]), int(match.shape[-1])
+    for name, t in (("match", match), ("Mask", Mask), ("bg", bg), ("fgMask", fgMask)):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != H * W:
+            raise ValueError("kitti_region_step: %s must be a contiguous fp32 (%d, %d) map" % (name, H, W))
+    for name, t in (("status", status), ("alive", alive)):
+        if t.dtype != torch.int32 or t.numel() != 1:
+            raise ValueError("kitti_region_step: %s must be one int32" % name)
+    if rec is None:
+        rec = torch.empty(2, device=match.device, dtype=torch.int32)
+    wsz = lib.rf_kitti_region_step_workspace(H, W)
+    ws = torch.empty(wsz, device=match.device, dtype=torch.uint8)
+    check(lib.rf_kitti_region_step(ptr(match), ptr(Mask), ptr(bg), ptr(fgMask), H, W, ptr(status), ptr(alive), int(bool(first)), int(cmin),
+                                   ptr(rec), ptr(ws), wsz, stream()))
+    return rec
+
+
 def fill_nearest_matched(flow, matched, want_index=False):
     """evaluation/evalKITTI/getResults.py:87-93 on the device: flow (1,H,W,2) fp32, matched (H,W) / (1,H,W,1) bool ->
     flow with every unmatched pixel replaced by the flow of its nearest matched pixel (exact EDT) [, (H,W,2) int32 indices]."""

@@ -735,15 +735,22 @@ def align2images(coarseModel, network, img1, img2, align_corners=False):
 # ------------------------------------------------------------------------------------------------------------------
 # KITTI: two-level fine flow (evaluation/evalKITTI/evaluation.py) and its recomposition (evalKITTI/getResults.py)
 # ------------------------------------------------------------------------------------------------------------------
-def PredFlowMask_kitti_device(IsSample, ItSample, flowCoarse, size, network, align_corners=False):
+def PredFlowMask_kitti_device(IsSample, ItSample, flowCoarse, size, network, align_corners=False, featt=None, feat_box=None):
     """evaluation/evalKITTI/evaluation.py:49-81 without the device->host copy: both images' fine features are computed
     here (one ragged batch of two images), the matchability is always ``match12 * grid_sample(match21) * inside``, and
     ``flowCoarse`` (1,Hc,Wc,2) may live on another grid than the ``size`` = (H, W) outputs (the second level, :296-302).
-    Returns CUDA tensors (flow12 (1,H,W,2), match (1,1,H,W), flowDown8 (1,2,h8,w8), matchDown8 (1,2,h8,w8))."""
+    Returns CUDA tensors (flow12 (1,H,W,2), match (1,1,H,W), flowDown8 (1,2,h8,w8), matchDown8 (1,2,h8,w8)).
+    ``featt`` (a Ragged): the target's fine features from an earlier batch, so only the source goes through the
+    FeatureExtractor; ``feat_box`` (a dict) receives the target's features of this batch under "featt"."""
     with torch.no_grad():
-        f = fine_features(network["netFeatCoarse"], torch.cat([IsSample, ItSample], dim=0))
-        n = f.data.shape[0] // 2
-        fs, ft = Ragged(f.data[:n], f.hw[:1]), Ragged(f.data[n:], f.hw[1:])
+        if featt is None:
+            f = fine_features(network["netFeatCoarse"], torch.cat([IsSample, ItSample], dim=0))
+            n = f.data.shape[0] // 2
+            fs, ft = Ragged(f.data[:n], f.hw[:1]), Ragged(f.data[n:], f.hw[1:])
+            if feat_box is not None:
+                feat_box["featt"] = ft
+        else:
+            fs, ft = fine_features(network["netFeatCoarse"], IsSample), featt
         k, ld, tc = network["netCorr"].kernelSize, network["netFlowCoarse"].CORR_LD, model.fine_engine()
         if tc == ops.ENGINE_SPLIT:
             corr12, both = ops.corr_neigh_pair_split(ft, fs, k, ld)
@@ -829,6 +836,183 @@ def align_pair_kitti(coarseModel, network, Is, It, fineSize=650, cc_th=0.01, mas
     if given:
         out["It_bg"] = It_bg.astype(bool)
     return out
+
+
+def fine_sizes(w, h, strideNet, minSize):
+    """The (w, h) ``outil.resizeImg(I, strideNet, minSize)`` resizes a w x h image to (utils/outil.py:6-19), from the size
+    alone: the same float divisions and Python ``round`` (half to even)."""
+    ratio = min(w / minSize, h / minSize)
+    return round(w / ratio / strideNet) * strideNet, round(h / ratio / strideNet) * strideNet
+
+
+_cmin_cache = {}
+
+
+def kitti_region_cmin(n, maskRegionTh):
+    """The smallest count c for which evalKITTI's acceptance test (evaluation.py:316), numpy's own
+    ``((m > 0.9999) * (1 - fgMask)).mean() > maskRegionTh``, holds for an n-pixel map with c new matched pixels; n + 1 when no
+    count does.  Found by bisection on that very expression (float32 mean, numpy's comparison rule), so the kernel only compares
+    integers.  The mean depends on c alone while its partial sums are exact, i.e. for n < 2**24.  Cached per (n, maskRegionTh)."""
+    n = int(n)
+    key = (n, float(maskRegionTh))
+    if key not in _cmin_cache:
+        assert 0 < n < 2 ** 24, "kitti_region_cmin: the float32 mean is exact only below 2**24 pixels"
+        fg = np.zeros(n, dtype=np.float32)
+
+        def accepted(c):
+            m = np.zeros(n, dtype=np.float32)
+            m[:c] = 1
+            return bool(((m > 0.9999) * (1 - fg)).mean() > maskRegionTh)
+
+        lo, hi = 0, n + 1                      # accepted(hi) is taken as true; find the first true in [lo, hi]
+        while lo < hi:
+            mid = (lo + hi) // 2
+            if accepted(mid):
+                hi = mid
+            else:
+                lo = mid + 1
+        _cmin_cache[key] = lo
+    return _cmin_cache[key]
+
+
+def _kitti_device(coarseModel, network, Is_u8, It_u8, fineSize, cc_th, maskRegionTh, maxH, segNet=False, samples=None):
+    """evaluation/evalKITTI/evaluation.py:216-336 for one pair with NO host control: everything is queued on the current stream
+    and nothing is read back, so the whole pair can be captured in one CUDA graph.
+      * the two fine-level targets are resized by the device LANCZOS (``outil.resizeImg`` to ``fineSize`` and ``fineSize // 2``);
+      * the target's fine features are computed once per level, in the first hypothesis' two-image batch (``feat_box``);
+      * ``maxH`` iterations run unconditionally: getCoarse (masked by fgMask), the two warp grids, the d2 level, its composition
+        to the resized grid, the org level, ``remove_small_cc`` and ``ops.kitti_region_step``, which turns the reference's
+        acceptance test and mask update (:316-326) into a device ``alive`` flag.  Hypotheses after the first dead one are
+        computed but dropped by the host when it unpacks.
+    ``Is_u8`` / ``It_u8``: uint8 (H, W, 3) CUDA images.  ``segNet``: the background of :245-250 is segNet's map of the target,
+    byte-scaled to the original size (``ops.imresize_mask``).  Returns (packed records, per-hypothesis (flow (1,H,W,2),
+    match (H,W)) CUDA maps, (h_org, w_org), (flow_d2 shape, flow shape)[, the uint8 (h_org, w_org) background map]); one record
+    per hypothesis: [alive, status, nbMatch, nbInlier, H(9), Finetune_D2, Finetune_Mask, Finetune]."""
+    with torch.no_grad():
+        h_org, w_org = int(It_u8.shape[0]), int(It_u8.shape[1])
+        w_r, h_r = fine_sizes(w_org, h_org, 8, fineSize)
+        w_d2, h_d2 = fine_sizes(w_org, h_org, 8, fineSize // 2)
+        to_t = coarseModel._to_tensor01
+        tensor_s = to_t(Is_u8)
+        tensor_resize = to_t(ops.resize_lanczos_u8(It_u8, w_r, h_r))
+        tensor_d2 = to_t(ops.resize_lanczos_u8(It_u8, w_d2, h_d2))
+        coarseModel.setPair(Is_u8, It_u8)
+        dev = It_u8.device
+        if segNet:
+            seg = getattr(coarseModel, "segNet", None)
+            if seg is None:
+                raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
+            bg = ops.imresize_mask(seg.run(It_u8)[0], h_org, w_org)              # :248
+        else:
+            bg = torch.ones((h_org, w_org), device=dev)
+        Mask = torch.zeros((h_org, w_org), device=dev)
+        fgMask = ((Mask + (1 - bg)) > 0.5).float()
+        alive = torch.ones(1, device=dev, dtype=torch.int32)
+        cmin = kitti_region_cmin(h_org * w_org, maskRegionTh)
+        box_d2, box_r = {}, {}
+        recs, maps, shapes = [], [], None
+        for k in range(maxH):
+            Hd, nb, _, status, cnt = coarseModel.getCoarse_device(fgMask, None if samples is None else samples[k])
+            bp = Hd.view(1, 3, 3)
+            homography_d2 = ops.warp_grid(bp, h_d2, w_d2)
+            homography_resize = ops.warp_grid(bp, h_r, w_r)
+            IsSample_d2 = ops.grid_sample(tensor_s, homography_d2)
+            _, _, flowFine_d2, _ = PredFlowMask_kitti_device(IsSample_d2, tensor_d2, homography_d2, (h_d2, w_d2), network,
+                                                             featt=box_d2.get("featt"), feat_box=box_d2)
+            flowCoarse, _, _ = ops.compose_fine(flowFine_d2, None, None, homography_resize, clamp=True, want_match=False)
+            IsSample = ops.grid_sample(tensor_s, flowCoarse)
+            flowFine_org, match_org, f8, m8 = PredFlowMask_kitti_device(IsSample, tensor_resize, flowCoarse, (h_org, w_org), network,
+                                                                        featt=box_r.get("featt"), feat_box=box_r)
+            ops.remove_small_cc(match_org, 0.99, cc_th)
+            match = match_org.view(h_org, w_org)
+            rec = ops.kitti_region_step(match, Mask, bg, fgMask, status, alive, k == 0, cmin)
+            recs.append(torch.cat([rec[:1].float(), status.float(), cnt.float(), nb.float(), Hd, flowFine_d2.reshape(-1),
+                                   m8.reshape(-1), f8.reshape(-1)]))
+            maps.append((flowFine_org, match))
+            shapes = (tuple(flowFine_d2.shape), tuple(f8.shape))
+        packed = torch.cat(recs)
+    if segNet:
+        return packed, maps, (h_org, w_org), shapes, bg.to(torch.uint8)
+    return packed, maps, (h_org, w_org), shapes
+
+
+def _unpack_kitti(host, maps, size, shapes, maxH):
+    """The host side of ``_kitti_device``: the hypotheses up to the first dead one, in ``align_pair_kitti``'s dict."""
+    host = host.reshape(maxH, -1)
+    if any(host[i, 1] == 2 and host[:i, 0].all() for i in range(maxH)):
+        raise TypeError("'NoneType' object is not subscriptable")          # utils/outil.py:162
+    n = 0
+    while n < maxH and host[n, 0] > 0.5:
+        n += 1
+    base = dict(maps=list(maps[:n]), size=tuple(size), nbMatch=[int(v) for v in host[:n, 2]], nbInlier=[int(v) for v in host[:n, 3]],
+                capped=n == maxH)
+    if n == 0:
+        return dict(H=np.zeros((0,)), flow_d2=np.zeros((0,)), mask=np.zeros((0,)), flow=np.zeros((0,)), **base)
+    d2shape, f8shape = shapes
+    nd, n8 = int(np.prod(d2shape)), int(np.prod(f8shape))
+    o = 13
+    return dict(H=host[:n, 4:13].reshape(n, 3, 3).astype(np.float32),
+                flow_d2=host[:n, o:o + nd].reshape((n,) + tuple(d2shape[1:])),
+                mask=host[:n, o + nd:o + nd + n8].reshape((n,) + tuple(f8shape[1:])),
+                flow=host[:n, o + nd + n8:o + nd + 2 * n8].reshape((n,) + tuple(f8shape[1:])), **base)
+
+
+def _as_device_u8(coarseModel, I):
+    """A PIL image, numpy array or uint8 (H, W, 3) tensor as a uint8 CUDA image."""
+    if torch.is_tensor(I):
+        return I if I.is_cuda else I.cuda()
+    return coarseModel._to_device_u8(I)
+
+
+def align_pair_kitti_graph(coarseModel, network, Is, It, fineSize=650, cc_th=0.01, maskRegionTh=0.005, maxH=5, segNet=False, samples=None):
+    """``align_pair_kitti`` without any host round trip inside the pair (``_kitti_device``, run eagerly), then one pinned D2H of
+    the records.  ``Is`` / ``It``: PIL images, numpy arrays or uint8 (H, W, 3) tensors.  ``maxH`` is required: the reference's
+    ``while True`` becomes ``maxH`` unconditional iterations.  Returns ``align_pair_kitti``'s dict (``maps``: the accepted
+    hypotheses' (flow, match) as CUDA tensors) plus ``nbMatch`` / ``nbInlier`` per hypothesis and ``capped`` (all ``maxH``
+    hypotheses accepted: the reference might have gone on); with ``segNet`` also ``It_bg``.  Under ``torch.manual_seed(s)`` the
+    RANSAC samples are the reference's; the hypotheses after the first dead one still draw theirs.  ``samples``: optional
+    injected (nbIter, 4) tables, one per hypothesis."""
+    if maxH is None or int(maxH) < 1:
+        raise ValueError("align_pair_kitti_graph: maxH must be a positive hypothesis cap")
+    maxH = int(maxH)
+    packed, maps, size, shapes, *aux = _kitti_device(coarseModel, network, _as_device_u8(coarseModel, Is), _as_device_u8(coarseModel, It),
+                                                     fineSize, cc_th, maskRegionTh, maxH, segNet, samples)
+    out = _unpack_kitti(_to_host(packed).copy(), maps, size, shapes, maxH)
+    if segNet:
+        out["It_bg"] = _to_host(aux[0]).reshape(size).astype(bool)
+    return out
+
+
+class GraphedKittiAligner(GraphedAligner):
+    """evalKITTI's pair (``align_pair_kitti_graph``: trunk, matching, ``maxH`` x (RANSAC, two fine levels, remove_small_cc,
+    acceptance test and mask update)) as ONE CUDA graph per pair of input sizes, with the LRU eviction of ``GraphedAligner``.
+    It can be a ``ConcurrentAligner`` lane (``make_aligner``).  ``fetch`` returns ``align_pair_kitti_graph``'s dict; its
+    ``maps`` are cloned from the graph's static buffers (``copy=False``: the live buffers, overwritten by the next replay with
+    these input sizes)."""
+
+    def __init__(self, coarseModel, network, fineSize=650, cc_th=0.01, maskRegionTh=0.005, maxH=5, segNet=False, warmup=2, max_graphs=4):
+        if segNet and getattr(coarseModel, "segNet", None) is None:
+            raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
+        if maxH is None or int(maxH) < 1:
+            raise ValueError("GraphedKittiAligner: maxH must be a positive hypothesis cap")
+        super().__init__(coarseModel, network, warmup=warmup, max_graphs=max_graphs)
+        self.fineSize, self.cc_th, self.maskRegionTh, self.maxH, self.segNet = fineSize, cc_th, maskRegionTh, int(maxH), bool(segNet)
+
+    def _device(self, s_in, t_in):
+        return _kitti_device(self.coarse, self.net, s_in, t_in, self.fineSize, self.cc_th, self.maskRegionTh, self.maxH, self.segNet)
+
+    def _unpack(self, host, maps, size, shapes):
+        return _unpack_kitti(host, maps, size, shapes, self.maxH)
+
+    def fetch(self, ticket, copy=True):
+        c, done = ticket
+        done.synchronize()
+        out = self._unpack(c["host"].numpy().copy(), c["flow12"], c["size"], c["f8shape"])
+        if copy:
+            out["maps"] = [(f.clone(), m.clone()) for f, m in out["maps"]]
+        if c["bg"] is not None:
+            out["It_bg"] = c["host_bg"].numpy().reshape(c["size"]).astype(bool)
+        return out
 
 
 def getFlow_all_kitti(param, flowd2, flow, match, outH, outW, th=1.0, cc_th=0.01, multiH=True, interpolate=False):
