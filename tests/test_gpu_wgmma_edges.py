@@ -121,9 +121,10 @@ def test_dual_sixteen_image_batch_equals_images_alone(rf):
 
 
 # ------------------------------------------------------------------ correlation: arg-max keys of every precision
-def corr_call(rf, A, B, mode):
+def corr_call(rf, A, B, mode, planes=None):
     """Runs the mutual nearest-neighbour entry point (``mode`` = its precision, or "presplit") with a caller-owned workspace;
-    returns (row keys, column keys, idx1, idx2) as numpy."""
+    returns (row keys, column keys, idx1, idx2) as numpy.  ``planes``: ((A_hi, A_lo), (B_hi, B_lo)) CUDA planes the pre-split
+    form reads instead of the split of A and B."""
     lib, ptr = rf._lib.lib, rf._lib.ptr
     NA, Cc = A.shape
     NB = B.shape[0]
@@ -132,7 +133,7 @@ def corr_call(rf, A, B, mode):
     idx2 = torch.empty(cap, device="cuda", dtype=torch.int64)
     count = torch.zeros(1, device="cuda", dtype=torch.int32)
     if mode == "presplit":
-        a, b = R.to_split(A).cuda(), R.to_split(B).cuda()
+        a, b = planes if planes is not None else (R.to_split(A).cuda(), R.to_split(B).cuda())
         wsz = lib.rf_corr_mutual_nn_presplit_workspace(NA, NB)
         ws = torch.empty(wsz, device="cuda", dtype=torch.uint8)
         rf._lib.check(lib.rf_corr_mutual_nn_presplit(ptr(a[0]), ptr(a[1]), NA, ptr(b[0]), ptr(b[1]), NB, Cc, ptr(idx1), ptr(idx2), ptr(count),
@@ -196,7 +197,7 @@ def corr_data(case):
     return torch.from_numpy(A), torch.from_numpy(B)
 
 
-@pytest.mark.parametrize("case", ["ties", "negative", "c192", "c448", "row1", "col1"])
+@pytest.mark.parametrize("case", ["ties", "negative", "c192", "c448", "c1024", "row1", "col1"])
 @pytest.mark.parametrize("mode", [0, 1, 2, "presplit"])
 def test_corr_argmax_keys_vs_fp64(rf, mode, case):
     """The correlation's per-row / per-column arg-max keys (f2ord(score) << 32 | ~index) read from the workspace: scores within
@@ -204,7 +205,8 @@ def test_corr_argmax_keys_vs_fp64(rf, mode, case):
     (precision 2, pre-split planes) allowance of fp64 scores of the consumed operands, indices the fp64 arg-max wherever the
     gap allows, exact ties to the smallest index across row and column tiles, the two keys of a mutual pair with bit-identical
     scores, and the compacted pair list == the mutual pairs of the keys.  Sizes leave partial row and column tiles, down to a
-    single row (row1) or a single column (col1); C = 64 / 192 / 448 give 1 to 14 K blocks."""
+    single row (row1) or a single column (col1); C = 64 / 192 / 448 give 1 to 14 K blocks, C = 1024 is the pipeline's
+    feature depth (the 3xTF32 allowance scales with the number of truncating accumulations beyond C = 448: acc_tf32x3)."""
     A, B = corr_data(case)
     split = mode in (2, "presplit")
     Aq = R.from_split(R.to_split(A)) if split else A.double()
@@ -212,7 +214,7 @@ def test_corr_argmax_keys_vs_fp64(rf, mode, case):
     S = (Aq.cuda() @ Bq.cuda().T).cpu().numpy()
     absS = (Aq.abs().cuda() @ Bq.abs().cuda().T).cpu().numpy()
     cu = A.shape[1] * 2.0 ** -24
-    c = R.ACC["split"] if split else R.ACC["tf32x3"] if mode == 1 else cu / (1 - cu)
+    c = R.ACC["split"] if split else R.acc_tf32x3(A.shape[1]) if mode == 1 else cu / (1 - cu)
     rowk, colk, i1, i2 = corr_call(rf, A, B, mode)
     csc, cidx, cw = check_keys(colk, S.T, absS.T, c, "columns")
     rsc, ridx, rw = check_keys(rowk, S, absS, c, "rows")

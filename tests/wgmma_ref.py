@@ -42,6 +42,15 @@ ACC = {"tf32": 2.0 ** -18, "f16": 2.0 ** -18, "split": 2.0 ** -17, "tf32x3": 2.0
 ELEVEN_BIT = 2.0 ** -11
 assert all(c * 30 <= ELEVEN_BIT for c in ACC.values())
 
+
+def acc_tf32x3(C):
+    """The 3xTF32 correlation's allowance at C channels.  Each truncating accumulation of a non-negative term loses less than
+    one ulp of the partial sum, so the accumulation error of the all-positive scores grows with their number, 3 C / 8; the
+    allowance measured at C = 448 is scaled by it beyond 448.  At the pipeline's C = 1024 the errors reach 1.004x the
+    unscaled value (post-ReLU features on an H100 80GB HBM3, 700 W power limit)."""
+    return ACC["tf32x3"] * max(1.0, C / 448.0)
+
+
 # engine -> (operand kind, output format)
 ENGINES = {1: ("tf32", "f32"), 2: ("f16", "f16"), 3: ("f16", "f32"), 4: ("split", "split"), 5: ("split", "f32")}
 BK = {"tf32": 32, "f16": 64, "split": 64}
