@@ -97,6 +97,33 @@ int rf_ransac_homography(const float* match1, const float* match2, int M, const 
                          const int64_t* samples, int sample_mode, int nbIter, float tolerance, int chunk,
                          float* H_out, int64_t* nbInlier_out, uint8_t* mask_out, int* status_out,
                          void* ws, size_t ws_bytes, void* stream);
+/* rf_ransac_homography on the table a device slot chain picks: `tables` holds n_tables (nbIter x 4) tables back to back
+ * (table j = the j-th draw the reference would make), the kernel reads table *slot_in (clamped to n_tables - 1) and writes
+ * *slot_out = *slot_in + (M >= 4), M = min(*M_dev, M): a call that does not draw (the reference returns None before
+ * torch.randint) passes its table on to the next call.  slot_in and slot_out are two different int32 device scalars;
+ * chaining calls through slots[i] -> slots[i + 1] makes each call read the table the reference's draw sequence gives it. */
+int rf_ransac_homography_drawn(const float* match1, const float* match2, int M, const int* M_dev,
+                               const int64_t* tables, int n_tables, int sample_mode, int nbIter, float tolerance, int chunk,
+                               const int* slot_in, int* slot_out, float* H_out, int64_t* nbInlier_out, uint8_t* mask_out,
+                               int* status_out, void* ws, size_t ws_bytes, void* stream);
+/* evaluation/evalYFCC/evaluation.py:195-212 on the device, one CTA: the four rotations' RANSAC statuses (RF_RANSAC_*),
+ * match counts (read as min(*count[k], cap[k])) and inlier masks (u8, cap[k] entries) -> one int32 record of
+ * RF_YFCC_REC_WORDS words: the winner (first maximum of the scores), the four scores (popcount of mask[:M] for a rotation
+ * that drew, M >= nbPoint, and returned a model; 0 otherwise), the number of rotations that drew, an error flag (a rotation
+ * that drew returned RF_RANSAC_NO_MODEL: utils/outil.py:162 raises TypeError) and the winner's orientation class
+ * (winner & 1: 0 / 180 degrees share the resized target's shape, 90 / 270 the transposed one).  `status`, `count`, `mask`
+ * and `cap` are host arrays of 4 (a mask may be null where its cap is 0).  No atomics: deterministic, graph-capturable. */
+#define RF_YFCC_REC_WINNER 0
+#define RF_YFCC_REC_SCORES 1
+#define RF_YFCC_REC_DRAWN 5
+#define RF_YFCC_REC_ERROR 6
+#define RF_YFCC_REC_CLASS 7
+#define RF_YFCC_REC_WORDS 8
+int rf_yfcc_rotation_select(const int* const* status, const int* const* count, const uint8_t* const* mask, const int* cap,
+                            int nbPoint, int* rec_out, void* stream);
+/* dst[0:bytes] <- src[*sel][0:bytes] (src: a host array of nsrc <= 4 device pointers, null entries copy nothing), with the
+ * index read on the device: a graph copies the buffers of a rotation chosen by an earlier kernel. */
+int rf_select_copy(const void* const* src, int nsrc, const int* sel, void* dst, size_t bytes, void* stream);
 /* utils/outil.py:68-87 Homography alone: X,Y [N][4][3] -> H [N][9] (for tests). */
 int rf_homography_dlt(const float* X, const float* Y, int N, float* H_out, void* stream);
 /* utils/outil.py:97-100 Prediction: err [N][M]. */

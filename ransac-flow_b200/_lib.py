@@ -29,6 +29,9 @@ SIGNATURES = {
     "rf_corr_mutual_nn_presplit": (i32, [vp, vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, sz, vp]),
     "rf_ransac_workspace": (sz, [i32]),
     "rf_ransac_homography": (i32, [vp, vp, i32, vp, vp, i32, i32, f32, i32, vp, vp, vp, vp, vp, sz, vp]),
+    "rf_ransac_homography_drawn": (i32, [vp, vp, i32, vp, vp, i32, i32, i32, f32, i32, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
+    "rf_yfcc_rotation_select": (i32, [vp, vp, vp, vp, i32, vp, vp]),
+    "rf_select_copy": (i32, [vp, i32, vp, vp, sz, vp]),
     "rf_homography_dlt": (i32, [vp, vp, i32, vp, vp]),
     "rf_prediction": (i32, [vp, vp, i32, vp, i32, vp, vp]),
     "rf_build_matches": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]),

@@ -285,7 +285,11 @@ class _CoarseAlignBase:
 
     def _ransac_device(self, match1, match2, cnt, samples=None):
         """RANSAC on a device-resident match list of ``cnt`` matches (no host synchronisation): the reference's seeded
-        stream (``SAMPLES_PHILOX64``) or an injected (nbIter, 4) index table.  Returns (H [9], nbInlier [1], mask, status [1])."""
+        stream (``SAMPLES_PHILOX64``) or an injected (nbIter, 4) index table.  Returns (H [9], nbInlier [1], mask, status [1]).
+        ``samples`` may also be one call of a slot chain over tables drawn in advance (``yfcc_graph.DrawnTables``): the call
+        then reads the table its slot selects on the device."""
+        if hasattr(samples, "ransac"):
+            return samples.ransac(match1, match2, cnt, self.tolerance, 100)
         if samples is not None:
             raw, mode = torch.as_tensor(samples, dtype=torch.int64).to(match1.device).contiguous(), ops.SAMPLES_MOD
         else:
@@ -458,6 +462,19 @@ class CoarseAlignC(_CoarseAlignBase):
         self.ItTensor = self._to_tensor01(r["u8"])
         self._featt_raw = r["raw"]
         self._set_target_feats(r["normed"], r["i"])
+
+    def _set_static_target(self, u8, raw):
+        """Make the uint8 (h, w, 3) CUDA image ``u8`` with the un-normalised conv4 features ``raw`` (a one-image Ragged) the
+        current target: what ``_select_target`` sets except the normalised ``featt``, which the masked re-matching of
+        ``getCoarse_device`` does not read (it is dropped, not left stale).  The graphed YFCC loop copies the winning rotation
+        into these buffers on the device."""
+        self.It = self._as_pil(u8)
+        self.ItTensor = self._to_tensor01(u8)
+        self._featt_raw = raw
+        for k in ("_featt_rows", "featt", "_tgt_planes"):
+            self.__dict__.pop(k, None)
+        self.W2, self.H2 = raw.hw[0]
+        self.WtInt, self.HtInt, self.Wt, self.Ht = outil._wh(self.W2, self.H2, u8.device)
 
     def rotated_target_size(self, k):
         """(w, h) of rotation ``k`` of the resized target (``_set_rotated_pair``)."""

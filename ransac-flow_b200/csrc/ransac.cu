@@ -188,7 +188,8 @@ ransac_kernel(const float* __restrict__ match1, const float* __restrict__ match2
               const int* __restrict__ M_dev, const long long* __restrict__ samples, int sample_mode, int nbIter,
               float tol, int chunk, int G,
               RansacHeader* hdr, int* counts, float* Hall, int* chunk_nz,
-              float* H_out, long long* nbInlier_out, unsigned char* mask_out, int* status_out) {
+              float* H_out, long long* nbInlier_out, unsigned char* mask_out, int* status_out,
+              const int* __restrict__ slot_in, int* __restrict__ slot_out, int n_tables) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* sH = reinterpret_cast<float*>(smem_raw);
     int* sFlag = reinterpret_cast<int*>(sH + 9 * G);
@@ -199,6 +200,14 @@ ransac_kernel(const float* __restrict__ match1, const float* __restrict__ match2
     const int nwarps = RANSAC_THREADS / 32;
     const int M = (M_dev != nullptr) ? min(*M_dev, M_host) : M_host;
     const int nGroups = (nbIter + G - 1) / G;
+    if (slot_in != nullptr) {
+        // drawn tables (rf_ransac_homography_drawn): this call reads table *slot_in and passes the next slot on, advanced only
+        // when it draws (M >= 4, as the reference returns None before torch.randint otherwise).  slot_out is another buffer
+        // than slot_in, so no CTA can read the increment this one writes.
+        const int slot = *slot_in;
+        samples += (long long)min(slot, n_tables - 1) * nbIter * 4;
+        if (blockIdx.x == 0 && threadIdx.x == 0) *slot_out = slot + (M >= 4 ? 1 : 0);
+    }
 
     if (M >= 4) {
         for (int g = blockIdx.x; g < nGroups; g += gridDim.x) {
@@ -428,6 +437,85 @@ __global__ void build_matches_kernel(const long long* __restrict__ idx1, const l
     if (tid == 0) *count_out = s_off;
 }
 
+// evaluation/evalYFCC/evaluation.py:195-212 after the four RANSAC calls, as one CTA: per rotation k, drew = M_k >= nbPoint
+// (the reference's getCoarse returns None before RANSAC otherwise), score = popcount(mask_k[:M_k]) when it drew and RANSAC
+// returned a model (np.sum(InlierMask)), else 0; RF_RANSAC_NO_MODEL on a rotation that drew is utils/outil.py:162's TypeError;
+// the winner is the first maximum (np.argmax).  Integer sums in a fixed order: deterministic, no atomics.
+struct YfccSelectArgs {
+    const int* status[4];
+    const int* count[4];
+    const unsigned char* mask[4];
+    int cap[4];
+};
+
+constexpr int SELECT_THREADS = 256;
+
+__global__ void __launch_bounds__(SELECT_THREADS)
+yfcc_rotation_select_kernel(YfccSelectArgs a, int nbPoint, int* __restrict__ rec) {
+    __shared__ int s_part[SELECT_THREADS / 32];
+    __shared__ int s_score[4];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int M = min(*a.count[k], a.cap[k]);
+        const bool drew = M >= nbPoint;
+        const bool ok = drew && *a.status[k] == RF_RANSAC_OK;
+        int c = 0;
+        if (ok)
+            for (int m = tid; m < M; m += SELECT_THREADS) c += a.mask[k][m] != 0;
+        c = __reduce_add_sync(0xffffffffu, c);
+        if (lane == 0) s_part[warp] = c;
+        __syncthreads();
+        if (tid == 0) {
+            int t = 0;
+#pragma unroll
+            for (int w = 0; w < SELECT_THREADS / 32; ++w) t += s_part[w];
+            s_score[k] = t;
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        int best = 0, drawn = 0, err = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const int M = min(*a.count[k], a.cap[k]);
+            const bool drew = M >= nbPoint;
+            drawn += drew ? 1 : 0;
+            err |= (drew && *a.status[k] == RF_RANSAC_NO_MODEL) ? 1 : 0;
+            if (s_score[k] > s_score[best]) best = k;
+        }
+        rec[RF_YFCC_REC_WINNER] = best;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) rec[RF_YFCC_REC_SCORES + k] = s_score[k];
+        rec[RF_YFCC_REC_DRAWN] = drawn;
+        rec[RF_YFCC_REC_ERROR] = err;
+        rec[RF_YFCC_REC_CLASS] = best & 1;
+    }
+}
+
+// dst <- src[*sel] (nothing when that source is null): the winning rotation's buffers into the static ones a loop graph reads
+struct SelectCopyArgs {
+    const void* src[4];
+};
+
+__global__ void select_copy_kernel(SelectCopyArgs a, int nsrc, const int* __restrict__ sel, void* __restrict__ dst, size_t bytes,
+                                   int vec16) {
+    const int k = *sel;
+    if (k < 0 || k >= nsrc) return;
+    const void* src = k == 0 ? a.src[0] : k == 1 ? a.src[1] : k == 2 ? a.src[2] : a.src[3];     // constant indices: no local copy
+    if (src == nullptr) return;
+    const size_t t0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x, step = (size_t)gridDim.x * blockDim.x;
+    if (vec16) {
+        const uint4* s = static_cast<const uint4*>(src);
+        uint4* d = static_cast<uint4*>(dst);
+        for (size_t i = t0; i < bytes / 16; i += step) d[i] = s[i];
+    } else {
+        const unsigned char* s = static_cast<const unsigned char*>(src);
+        unsigned char* d = static_cast<unsigned char*>(dst);
+        for (size_t i = t0; i < bytes; i += step) d[i] = s[i];
+    }
+}
+
 }  // namespace rf
 
 using namespace rf;
@@ -441,13 +529,14 @@ extern "C" size_t rf_ransac_workspace(int nbIter) {
     return b;
 }
 
-extern "C" int rf_ransac_homography(const float* match1, const float* match2, int M, const int* M_dev,
-                                    const int64_t* samples, int sample_mode, int nbIter, float tolerance, int chunk,
-                                    float* H_out, int64_t* nbInlier_out, uint8_t* mask_out, int* status_out,
-                                    void* ws, size_t ws_bytes, void* stream) {
-    RF_REQUIRE(M >= 0 && nbIter >= 0 && chunk >= 1, "rf_ransac_homography: bad sizes");
+static int launch_ransac(const float* match1, const float* match2, int M, const int* M_dev,
+                         const int64_t* samples, int n_tables, int sample_mode, int nbIter, float tolerance, int chunk,
+                         const int* slot_in, int* slot_out, float* H_out, int64_t* nbInlier_out, uint8_t* mask_out,
+                         int* status_out, void* ws, size_t ws_bytes, void* stream) {
+    RF_REQUIRE(M >= 0 && nbIter >= 0 && chunk >= 1 && n_tables >= 1, "rf_ransac_homography: bad sizes");
     RF_REQUIRE(sample_mode >= RF_SAMPLES_INDEX && sample_mode <= RF_SAMPLES_PHILOX64, "rf_ransac_homography: unknown sample_mode");
     RF_REQUIRE(ws != nullptr && ws_bytes >= rf_ransac_workspace(nbIter), "rf_ransac_homography: workspace too small");
+    RF_REQUIRE(slot_in != slot_out || slot_in == nullptr, "rf_ransac_homography_drawn: slot_in and slot_out must be two buffers");
     cudaStream_t st = as_stream(stream);
     size_t n = (size_t)(nbIter > 0 ? nbIter : 1);
     unsigned char* p = static_cast<unsigned char*>(ws);
@@ -466,9 +555,26 @@ extern "C" int rf_ransac_homography(const float* match1, const float* match2, in
     size_t smem = (size_t)G * (9 * sizeof(float) + sizeof(int));
     ransac_kernel<<<grid, RANSAC_THREADS, smem, st>>>(match1, match2, M, M_dev, (const long long*)samples, sample_mode, nbIter, tolerance,
                                                       chunk, G, hdr, counts, Hall, chunk_nz, H_out,
-                                                      (long long*)nbInlier_out, mask_out, status_out);
+                                                      (long long*)nbInlier_out, mask_out, status_out, slot_in, slot_out, n_tables);
     RF_LAUNCHED();
     return 0;
+}
+
+extern "C" int rf_ransac_homography(const float* match1, const float* match2, int M, const int* M_dev,
+                                    const int64_t* samples, int sample_mode, int nbIter, float tolerance, int chunk,
+                                    float* H_out, int64_t* nbInlier_out, uint8_t* mask_out, int* status_out,
+                                    void* ws, size_t ws_bytes, void* stream) {
+    return launch_ransac(match1, match2, M, M_dev, samples, 1, sample_mode, nbIter, tolerance,
+                         chunk, nullptr, nullptr, H_out, nbInlier_out, mask_out, status_out, ws, ws_bytes, stream);
+}
+
+extern "C" int rf_ransac_homography_drawn(const float* match1, const float* match2, int M, const int* M_dev,
+                                          const int64_t* tables, int n_tables, int sample_mode, int nbIter, float tolerance,
+                                          int chunk, const int* slot_in, int* slot_out, float* H_out, int64_t* nbInlier_out,
+                                          uint8_t* mask_out, int* status_out, void* ws, size_t ws_bytes, void* stream) {
+    RF_REQUIRE(slot_in != nullptr && slot_out != nullptr, "rf_ransac_homography_drawn: slot_in and slot_out are required");
+    return launch_ransac(match1, match2, M, M_dev, tables, n_tables, sample_mode, nbIter,
+                         tolerance, chunk, slot_in, slot_out, H_out, nbInlier_out, mask_out, status_out, ws, ws_bytes, stream);
 }
 
 extern "C" int rf_homography_dlt(const float* X, const float* Y, int N, float* H_out, void* stream) {
@@ -494,6 +600,42 @@ extern "C" int rf_build_matches(const int64_t* idx1, const int64_t* idx2, const 
     build_matches_kernel<<<1, 256, 0, as_stream(stream)>>>((const long long*)idx1, (const long long*)idx2, count_in, W1, H1, W2, H2,
                                                             valid16, match1_out, match2_out, (long long*)idx2_kept_out,
                                                             count_out, capacity);
+    RF_LAUNCHED();
+    return 0;
+}
+
+extern "C" int rf_yfcc_rotation_select(const int* const* status, const int* const* count, const uint8_t* const* mask, const int* cap,
+                                       int nbPoint, int* rec_out, void* stream) {
+    RF_REQUIRE(status != nullptr && count != nullptr && mask != nullptr && cap != nullptr && rec_out != nullptr,
+               "rf_yfcc_rotation_select: null argument");
+    RF_REQUIRE(nbPoint >= 1, "rf_yfcc_rotation_select: bad nbPoint");
+    YfccSelectArgs a;
+    for (int k = 0; k < 4; ++k) {
+        RF_REQUIRE(status[k] != nullptr && count[k] != nullptr && cap[k] >= 0 && (mask[k] != nullptr || cap[k] == 0),
+                   "rf_yfcc_rotation_select: bad rotation");
+        a.status[k] = status[k];
+        a.count[k] = count[k];
+        a.mask[k] = mask[k];
+        a.cap[k] = cap[k];
+    }
+    yfcc_rotation_select_kernel<<<1, SELECT_THREADS, 0, as_stream(stream)>>>(a, nbPoint, rec_out);
+    RF_LAUNCHED();
+    return 0;
+}
+
+extern "C" int rf_select_copy(const void* const* src, int nsrc, const int* sel, void* dst, size_t bytes, void* stream) {
+    RF_REQUIRE(src != nullptr && sel != nullptr && dst != nullptr && nsrc >= 1 && nsrc <= 4, "rf_select_copy: bad arguments");
+    if (bytes == 0) return 0;
+    SelectCopyArgs a;
+    int vec16 = (bytes % 16 == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) ? 1 : 0;
+    for (int k = 0; k < 4; ++k) {
+        a.src[k] = k < nsrc ? src[k] : nullptr;
+        if (a.src[k] != nullptr && (reinterpret_cast<uintptr_t>(a.src[k]) & 15) != 0) vec16 = 0;
+    }
+    const size_t units = vec16 ? bytes / 16 : bytes;
+    const size_t want = (units + 255) / 256;
+    const int grid = (int)(want < (size_t)(4 * num_sms()) ? (want < 1 ? 1 : want) : (size_t)(4 * num_sms()));
+    select_copy_kernel<<<grid, 256, 0, as_stream(stream)>>>(a, nsrc, sel, dst, bytes, vec16);
     RF_LAUNCHED();
     return 0;
 }

@@ -248,14 +248,18 @@ def corr_mutual_nn(featA, featB, precision=0):
 SAMPLES_INDEX, SAMPLES_MOD, SAMPLES_PHILOX64 = 0, 1, 2
 
 
-def philox_words(nbIter, nbPoint, device, generator=None):
+def philox_words(nbIter, nbPoint, device, generator=None, out=None):
     """(nbIter, nbPoint) full-range 64-bit words from torch's CUDA generator: element i is (x << 32) | y of the curand4 call
     whose x torch.randint(M, (nbIter, nbPoint), device='cuda') reduces modulo M from the same generator state (and the
     generator advances by the same offset).  With ``SAMPLES_PHILOX64`` the RANSAC kernel therefore sees the reference's
     seeded sample stream (utils/outil.py:120) with M read on the device; the draw is graph-capturable.  ``generator``: a CUDA
-    generator of its own instead of torch's default one."""
+    generator of its own instead of torch's default one.  ``out``: a contiguous (nbIter, nbPoint) int64 tensor to draw into
+    (e.g. one table of a stack of tables)."""
     assert nbIter * nbPoint <= 256 * 1024, "beyond this size ATen maps several elements to one Philox subsequence"
-    return torch.empty((nbIter, nbPoint), dtype=torch.int64, device=device).random_(-2 ** 63, None, generator=generator)
+    if out is None:
+        out = torch.empty((nbIter, nbPoint), dtype=torch.int64, device=device)
+    assert tuple(out.shape) == (nbIter, nbPoint) and out.dtype == torch.int64 and out.is_contiguous()
+    return out.random_(-2 ** 63, None, generator=generator)
 
 
 def corr_mutual_nn_presplit(A_hi, A_lo, B_hi, B_lo):

@@ -297,38 +297,61 @@ def _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_ma
     the drivers save (evaluation.py:244-260); the full-resolution maps stay on the device and are not returned.
     ``segNet`` (the drivers' ``--segNet``): the background map of the target (``_sky_background``) masks every hypothesis,
     the first included (:211-243 with ``It_bg``); it is returned as a fifth item, a uint8 (h, w) CUDA map (1 = kept)."""
-    box = {}
     coarseModel.setPair(Is, It)
-    Itw, Ith = coarseModel.target_size
-    dev = coarseModel.ItTensor.device
     keep = _sky_background(coarseModel, It) if segNet else None
     bg = keep.float() if segNet else None
-    Mask = torch.zeros((Ith, Itw), device=dev)
-    alive = torch.ones((), device=dev, dtype=torch.bool)
-    recs, featt, f8shape = [], None, None
-    for k in range(maxCoarse + 1):
-        if bg is None:
-            fgMask = (Mask > 0.5).float()                                # It_bg = 1 everywhere: (Mask + (1 - It_bg)) > 0.5
-        else:
-            fgMask = ((Mask + (1 - bg)) > 0.5).float()
-        Hd, nb, mask, status, cnt = coarseModel.getCoarse_device(fgMask if k > 0 or bg is not None else None,
-                                                                 None if samples is None else samples[k])
-        flowCoarse = ops.warp_grid(Hd.view(1, 3, 3), Ith, Itw)
-        flow12, match, f8, mboth = PredFlowMask_device(coarseModel.IsTensor, featt, flowCoarse, (Ith, Itw), network, with_match21,
-                                                       ItTensor=coarseModel.ItTensor, feat_box=box)
-        if featt is None:
-            featt = box["featt"]            # computed with the first hypothesis' warped source in one batch
-        newreg = (match[0, 0] * (1 - fgMask)).mean()
-        ok = (status[0] == 0) & ((newreg > maskRegionTh) if k > 0 else torch.ones((), device=dev, dtype=torch.bool))
-        alive = alive & ok
-        # (evaluation.py:235 masks from the first hypothesis on; without a background the first mask is all zeros)
-        matchFine = match[0, 0] if (k == 0 and bg is None) else match[0, 0] * (1 - fgMask)
-        Mask = torch.where(alive, ((Mask + matchFine) >= 1.0).float(), Mask)
-        recs.append(torch.cat([alive.float().reshape(1), status.float(), cnt.float(), nb.float(), Hd, f8.reshape(-1), mboth.reshape(-1)]))
-        f8shape = tuple(f8.shape)
+    recs, f8shape = _hypothesis_loop(coarseModel, network, maxCoarse, maskRegionTh, with_match21, bg, samples)
+    Itw, Ith = coarseModel.target_size
     if segNet:
         return torch.cat(recs), None, (Ith, Itw), f8shape, keep.view(torch.uint8)
     return torch.cat(recs), None, (Ith, Itw), f8shape
+
+
+def _hypothesis_loop(coarseModel, network, maxCoarse, maskRegionTh, with_match21, bg, samples, region64=False):
+    """The ``maxCoarse + 1`` unconditional iterations of ``_multi_device`` on the target ``coarseModel`` currently holds, masked
+    with ``bg`` (a float (h, w) CUDA map, 1 = kept; None: nothing masked).  ``samples[k]``: what hypothesis k's ``getCoarse_device``
+    draws from (None: the generator).  ``region64``: the acceptance test compares the new-region mean with ``maskRegionTh`` in
+    float64, as the host-steered loop does once the mean is on the host.  Returns (per-hypothesis records, flowDown8 shape)."""
+    Itw, Ith = coarseModel.target_size
+    dev = coarseModel.ItTensor.device
+    Mask = torch.zeros((Ith, Itw), device=dev)
+    alive = torch.ones((), device=dev, dtype=torch.bool)
+    recs, featt, f8shape, box = [], None, None, {}
+    for k in range(maxCoarse + 1):
+        Mask, alive, featt, rec, f8shape = _hypothesis_step(coarseModel, network, k, Mask, alive, bg, featt, box, maskRegionTh,
+                                                            with_match21, None if samples is None else samples[k], region64)
+        recs.append(rec)
+    return recs, f8shape
+
+
+def _hypothesis_step(coarseModel, network, k, Mask, alive, bg, featt, box, maskRegionTh, with_match21, samples, region64=False):
+    """Hypothesis ``k`` of ``_hypothesis_loop``: getCoarse masked by (Mask, bg), the fine flow, the acceptance test and the mask
+    update gated by the ``alive`` flag.  Returns (Mask, alive, the target's fine features, the record, flowDown8 shape)."""
+    Itw, Ith = coarseModel.target_size
+    dev = coarseModel.ItTensor.device
+    if bg is None:
+        fgMask = (Mask > 0.5).float()                                # It_bg = 1 everywhere: (Mask + (1 - It_bg)) > 0.5
+    else:
+        fgMask = ((Mask + (1 - bg)) > 0.5).float()
+    Hd, nb, mask, status, cnt = coarseModel.getCoarse_device(fgMask if k > 0 or bg is not None else None, samples)
+    flowCoarse = ops.warp_grid(Hd.view(1, 3, 3), Ith, Itw)
+    flow12, match, f8, mboth = PredFlowMask_device(coarseModel.IsTensor, featt, flowCoarse, (Ith, Itw), network, with_match21,
+                                                   ItTensor=coarseModel.ItTensor, feat_box=box)
+    if featt is None:
+        featt = box["featt"]            # computed with the first hypothesis' warped source in one batch
+    newreg = (match[0, 0] * (1 - fgMask)).mean()
+    found = status[0] == 0
+    if k > 0:
+        region = (newreg.double() > maskRegionTh) if region64 else (newreg > maskRegionTh)
+    else:
+        region = torch.ones((), device=dev, dtype=torch.bool)
+    ok = found & region
+    alive = alive & ok
+    # (evaluation.py:235 masks from the first hypothesis on; without a background the first mask is all zeros)
+    matchFine = match[0, 0] if (k == 0 and bg is None) else match[0, 0] * (1 - fgMask)
+    Mask = torch.where(alive, ((Mask + matchFine) >= 1.0).float(), Mask)
+    rec = torch.cat([alive.float().reshape(1), status.float(), cnt.float(), nb.float(), Hd, f8.reshape(-1), mboth.reshape(-1)])
+    return Mask, alive, featt, rec, tuple(f8.shape)
 
 
 def _unpack_multi(host, size, f8shape, nhyp):
@@ -1114,3 +1137,7 @@ def getFlow_all(flow, param, match, outH, outW, th=0.95, multiH=True, with_match
             tmp = tmp.expand_as(flowGlobal)
             flowGlobal[tmp] = f.narrow(0, i, 1)[tmp]
     return flowGlobal
+
+
+# evalYFCC's pair from CUDA graphs (its kernel entries live with it, in yfcc_graph)
+from .yfcc_graph import GraphedYfccAligner, align_pair_yfcc_graph  # noqa: E402,F401
