@@ -8,10 +8,12 @@ restated on the library's kernels (no file IO, no metrics: those stay in the dri
   KITTI        : evaluation/evalKITTI/evaluation.py:49-100,216-344 (two-level flow, small connected components),
                  evaluation/evalKITTI/getResults.py:95-141 (two-level recomposition)
 """
+from typing import NamedTuple
+
 import numpy as np
 import torch
 
-from . import _lib, model, ops
+from . import _lib, model, ops, program
 from .kornia_geometry import HomographyWarper
 from .ops import Ragged
 
@@ -29,6 +31,31 @@ def fine_features(netFeatCoarse, img):
     return Ragged(ops.l2norm(f.data), f.hw)
 
 
+def _fine_corr(network, IsSample, ItSample, featt, feat_box):
+    """The fine features of the warped source and the target and their correlation pair: (corr12, [corr12 ; corr21], held).
+    ``featt = None``: both images' features in one two-image batch (twice the tiles per FeatureExtractor launch, half the
+    launches), the target's handed to ``feat_box`` (a dict, or None) for the next hypotheses; else the target's cached
+    features (a Ragged or the reference's (1,256,h8,w8) tensor) and the source's alone.  ``held``: the features and volumes
+    behind the pair, which the caller keeps until its heads have run (when they are freed sets the layout, and so the size,
+    of a captured graph's memory pool)."""
+    if featt is None:
+        f = fine_features(network["netFeatCoarse"], torch.cat([IsSample, ItSample], dim=0))
+        n = f.data.shape[0] // 2
+        fs, ft = Ragged(f.data[:n], f.hw[:1]), Ragged(f.data[n:], f.hw[1:])
+        if feat_box is not None:
+            feat_box["featt"] = ft
+    else:
+        fs = fine_features(network["netFeatCoarse"], IsSample)
+        ft = featt if isinstance(featt, Ragged) else Ragged.from_nchw(featt)
+    k, ld = network["netCorr"].kernelSize, network["netFlowCoarse"].CORR_LD
+    tc = model.fine_engine()            # 0 plain fp32, 1 TF32-rounded, 2 fp16, 4 split planes: the operand type of the heads
+    if tc == ops.ENGINE_SPLIT:          # one launch: corr12 standalone + the two-image [corr12 ; corr21] tensor, split planes
+        corr = ops.corr_neigh_pair_split(ft, fs, k, ld)
+    else:                               # both volumes from one launch, already laid out as the two-image batch
+        corr = ops.corr_neigh_pair(ft, fs, k, ld, tc)
+    return corr[0], corr[-1], (fs, ft, corr)
+
+
 def PredFlowMask_device(IsTensor, featt, flowCoarse, size, network, with_match21=False, align_corners=False, ItTensor=None, feat_box=None):
     """PredFlowMask without the device->host copies: returns CUDA tensors
     (flow12 (1,H,W,2), match (1,1,H,W), flowDown8 (1,2,h8,w8), matchDown8 (2,1,h8,w8) = [match12, match21]).
@@ -37,22 +64,7 @@ def PredFlowMask_device(IsTensor, featt, flowCoarse, size, network, with_match21
     ``feat_box`` (a dict) receives them for the next hypotheses."""
     with torch.no_grad():
         IsSample = ops.grid_sample(IsTensor, flowCoarse, align_corners)
-        if featt is None:
-            f = fine_features(network["netFeatCoarse"], torch.cat([IsSample, ItTensor], dim=0))
-            n = f.data.shape[0] // 2
-            fs, ft = Ragged(f.data[:n], f.hw[:1]), Ragged(f.data[n:], f.hw[1:])
-            if feat_box is not None:
-                feat_box["featt"] = ft
-        else:
-            fs = fine_features(network["netFeatCoarse"], IsSample)
-            ft = featt if isinstance(featt, Ragged) else Ragged.from_nchw(featt)
-        k = network["netCorr"].kernelSize
-        ld = network["netFlowCoarse"].CORR_LD
-        tc = model.fine_engine()            # 0 plain fp32, 1 TF32-rounded, 2 fp16, 4 split planes: the operand type of the heads
-        if tc == ops.ENGINE_SPLIT:              # one launch: corr12 standalone + the two-image [corr12 ; corr21] tensor, split planes
-            corr12, both = ops.corr_neigh_pair_split(ft, fs, k, ld)
-        else:                                   # both volumes from one launch, already laid out as the two-image batch
-            corr12, _, both = ops.corr_neigh_pair(ft, fs, k, ld, tc)
+        corr12, both, _held = _fine_corr(network, IsSample, ItTensor, featt, feat_box)
         # the two heads are independent: the flow head (one image: 152 tiles in its widest layer, more than one wave on 132
         # SMs) runs on the side stream and fills the tails of the matchability head's kernels (two images) and vice versa
         main, side = torch.cuda.current_stream(), _side_stream()
@@ -103,6 +115,22 @@ def _to_host(t):
     return h.numpy()
 
 
+class DevicePair(NamedTuple):
+    """One pair's results as its device path leaves them, nothing read back: ``packed`` the records the host reads, ``maps``
+    the device tensors handed to the caller (or None), ``size`` the target's (h, w), ``shapes`` the shapes the host needs to
+    cut the records, ``bg`` the device background map (None without one)."""
+    packed: torch.Tensor
+    maps: object
+    size: tuple
+    shapes: tuple
+    bg: object = None
+
+
+def _read_back(pair):
+    """The end of an eager entry point: one pinned D2H of the records and one of the background map (None without one)."""
+    return _to_host(pair.packed).copy(), None if pair.bg is None else _to_host(pair.bg).copy()
+
+
 def _single_device(coarseModel, network, Is, It, with_match21, samples=None):
     """Device part of the single-hypothesis path: everything queued on the current stream, nothing read back."""
     coarseModel.setPair(Is, It)
@@ -113,10 +141,11 @@ def _single_device(coarseModel, network, Is, It, with_match21, samples=None):
     flow12, match, f8, mboth = PredFlowMask_device(coarseModel.IsTensor, None, flowCoarse, (Ith, Itw), network, with_match21,
                                                    ItTensor=coarseModel.ItTensor)
     packed = torch.cat([status.float(), cnt.float(), nb.float(), Hd, match.reshape(-1), f8.reshape(-1), mboth.reshape(-1)])
-    return packed, flow12, (Ith, Itw), tuple(f8.shape)
+    return DevicePair(packed, flow12, (Ith, Itw), tuple(f8.shape))
 
 
 def _unpack_single(host, flow12, size, f8shape):
+    """The host side of ``_single_device``: ``align_pair_single``'s dict."""
     Ith, Itw = size
     st, n0, n8 = int(host[0]), Ith * Itw, int(np.prod(f8shape))
     if st != 0:                                    # the reference's `if bestPara is None: break` (evaluation.py:215-216)
@@ -137,15 +166,31 @@ def align_pair_single(coarseModel, network, Is, It, with_match21=False, samples=
     composition are queued back to back, then one pinned D2H brings back status, H, the matchability map and the /8
     tensors.  Same outputs as ``align_pair``; under ``torch.manual_seed(s)`` also the same RANSAC samples (the reference's
     stream, ``ops.philox_words``).  ``samples``: an injected (nbIter, 4) index table instead."""
-    packed, flow12, size, f8shape = _single_device(coarseModel, network, Is, It, with_match21, samples)
-    return _unpack_single(_to_host(packed).copy(), flow12, size, f8shape)
+    pair = _single_device(coarseModel, network, Is, It, with_match21, samples)
+    return _unpack_single(_read_back(pair)[0], pair.maps, pair.size, pair.shapes)
+
+
+def _as_tensor(a):
+    return torch.from_numpy(np.ascontiguousarray(a)) if isinstance(a, np.ndarray) else a
+
+
+def _clone(maps):
+    """A copy of a result's device maps: a tensor, a list of (flow, match) tensors, or None."""
+    if torch.is_tensor(maps):
+        return maps.clone()
+    return None if maps is None else [tuple(t.clone() for t in m) for m in maps]
 
 
 class GraphedAligner:
     """``align_pair_single`` captured once in a CUDA graph per input size and replayed per pair: the ~140 kernel
     launches of a pair (pyramid, ResNet-50 trunk, matching, RANSAC, fine flow) cost one graph launch on the host.
     Inputs are copied into static device buffers (H2D when they are host tensors / arrays); the RANSAC samples are
-    drawn inside the graph (torch's graph-safe Philox offsets), so successive replays use fresh samples."""
+    drawn inside the graph (torch's graph-safe Philox offsets), so successive replays use fresh samples.
+
+    It is also the capture core of the other graphed pairs: a subclass gives the device work of its pair (``_device``,
+    returning a ``DevicePair``) and its host unpacking (``_unpack``), or builds its own graphs from ``warm`` and ``capture``.
+    Each record pins the layer-program entries its graphs point into; evicting it unpins them, and an entry goes with its
+    last pin, whichever aligner holds the other graphs that point into it."""
 
     def __init__(self, coarseModel, network, with_match21=False, warmup=2, max_graphs=8):
         self.coarse, self.net, self.m21, self.warmup = coarseModel, network, with_match21, warmup
@@ -154,6 +199,7 @@ class GraphedAligner:
         self.max_graphs = max_graphs    # datasets with many image sizes (HPatches, MegaDepth, YFCC): LRU-bounded graph memory
         self.replayed_kernels = 0       # library kernels executed through graph replays (they bypass rf_launch_count)
         self.generator = None           # RANSAC sample stream: torch's default CUDA generator (the reference's stream)
+        self._entries = set()           # (program, key) the graphs of the record being built point into
 
     def use_generator(self, generator):
         """Draw this aligner's RANSAC samples from ``generator`` (a CUDA torch.Generator of its own) instead of torch's default
@@ -164,126 +210,136 @@ class GraphedAligner:
         self.coarse.sample_generator = generator
 
     def _device(self, s_in, t_in):
-        """The device work of one pair, queued on the current stream: (packed results, flow12 | None, (H, W), flowDown8 shape)."""
+        """The device work of one pair, queued on the current stream: a ``DevicePair``."""
         return _single_device(self.coarse, self.net, s_in, t_in, self.m21)
 
-    def _unpack(self, host, flow12, size, f8shape):
-        return _unpack_single(host, flow12, size, f8shape)
+    def _unpack(self, host, bg, maps, size, shapes):
+        """The pair's dict from its host records, host background map (None without one) and device maps."""
+        return _unpack_single(host, maps, size, shapes)
 
-    def _programs(self):
-        """Every LayerProgram whose cached activation buffers a captured graph of this aligner points into."""
-        progs = [p for p in (self.coarse.net.program, self.coarse.net._program_f16, self.coarse.net._program_split) if p is not None]
-        seg = getattr(self.coarse, "segNet", None)
-        if seg is not None:                     # segNet's encoder and head programs (used by the graphs of a segNet aligner)
-            progs += [seg.encoder, seg.head]
-        for m in self.net.values():
-            progs += list(getattr(m, "_fold", {}).values())
-        return progs
-
-    def _evict(self):
-        """Drop the least recently used graph TOGETHER with the activation buffers only it refers to: the graph holds raw
-        pointers into the layer programs' cached buffers, so neither may outlive the other (ADVICE r1: use-after-free)."""
-        key = next(iter(self.graphs))
-        torch.cuda.synchronize()
-        rec = self.graphs.pop(key)
-        live = set()
-        for r in self.graphs.values():
-            live |= r["prog_keys"]
-        for prog in self._programs():
-            for k in [k for k in prog._compiled if (id(prog), k) in rec["prog_keys"] and (id(prog), k) not in live]:
-                del prog._compiled[k]
-        del rec
-
-    def _build(self, Is, It):
-        dev = torch.device("cuda", torch.cuda.current_device())
-        s_in = torch.empty(tuple(Is.shape), dtype=torch.uint8, device=dev)
-        t_in = torch.empty(tuple(It.shape), dtype=torch.uint8, device=dev)
-        s_in.copy_(Is)
-        t_in.copy_(It)
+    def warm(self, fn):
+        """``warmup`` eager runs of ``fn()`` on a side stream (function attributes, TMA maps, caches, layer programs: nothing a
+        capture may do first), then a device barrier."""
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(self.warmup):                       # eager runs: func attributes, TMA maps, caches, buffers
-                self._device(s_in, t_in)
+        with torch.no_grad(), torch.cuda.stream(side):
+            for _ in range(self.warmup):
+                fn()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
+
+    def capture(self, fn, pool=None):
+        """``fn()`` captured in a new CUDA graph (in the memory pool ``pool`` when given) that replays draw from this aligner's
+        generator.  The layer-program entries the graph points into join those the record being built pins.  Returns (graph,
+        ``fn()``'s result, library kernels in the graph)."""
         g = torch.cuda.CUDAGraph()
         if self.generator is not None:
             g.register_generator_state(self.generator)
         n0 = _lib.launch_count()
-        with torch.cuda.graph(g):
-            packed, flow12, size, f8shape, *aux = self._device(s_in, t_in)
-        # the compiled program entries (activation buffers) this graph's kernels point into: every entry whose image-set
-        # signature the warm-up / capture of THIS input size touched
-        touched = {(id(p), k) for p in self._programs() for k in p._compiled if k in p.__dict__.get("_touched", ())}
-        for p in self._programs():
-            p.__dict__["_touched"] = set()
-        return dict(n_kernels=_lib.launch_count() - n0, graph=g, s_in=s_in, t_in=t_in, packed=packed, flow12=flow12, size=size, f8shape=f8shape,
-                    prog_keys=touched, bg=aux[0] if aux else None)
+        with torch.no_grad(), program.recording() as used, torch.cuda.graph(g, pool=pool):
+            res = fn()
+        self._entries |= used
+        return g, res, _lib.launch_count() - n0
 
-    def prepare(self, Is, It):
-        """Capture (once) the graph for this pair of input sizes; returns its record."""
-        if isinstance(Is, np.ndarray):
-            Is, It = torch.from_numpy(Is), torch.from_numpy(It)
-        key = (tuple(Is.shape), tuple(It.shape))
-        if key not in self.graphs:
-            while self.max_graphs and len(self.graphs) >= self.max_graphs:
-                self._evict()
-            for p in self._programs():
-                p.__dict__["_touched"] = set()
-            self.graphs[key] = self._build(Is, It)
-        else:
+    def _build(self, s_in, t_in, bg_in):
+        """The record of one input size: the pair in one graph."""
+        if bg_in is not None:
+            raise TypeError("%s takes no background map" % type(self).__name__)
+        self.warm(lambda: self._device(s_in, t_in))
+        g, pair, n = self.capture(lambda: self._device(s_in, t_in))
+        return dict(graph=g, pair=pair, flow12=pair.maps, n_kernels=n)      # flow12: the maps replays write (fetch's copy=False)
+
+    def prepare(self, Is, It, It_bg=None):
+        """Capture (once) the graphs for these input sizes, evicting the least recently used record beyond ``max_graphs``;
+        returns their record."""
+        inputs = [_as_tensor(a) for a in (Is, It, It_bg)]
+        key = tuple(None if a is None else tuple(a.shape) for a in inputs)
+        if key in self.graphs:
             self.graphs[key] = self.graphs.pop(key)            # most recently used last
-        return self.graphs[key]
+            return self.graphs[key]
+        while self.max_graphs and len(self.graphs) >= self.max_graphs:
+            self._evict()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        dtypes = (torch.uint8, torch.uint8, torch.float32)             # Is, It, It_bg
+        static = [None if a is None else torch.empty(tuple(a.shape), dtype=d, device=dev).copy_(a) for a, d in zip(inputs, dtypes)]
+        self._entries = set()
+        rec = self._build(*static)
+        for p, k in self._entries:
+            p.pin(k)
+        rec.update(inputs=static, pins=self._entries, prog_keys={(id(p), k) for p, k in self._entries})
+        self.graphs[key] = rec
+        return rec
 
-    def enqueue(self, Is, It):
+    def _evict(self):
+        """Drop the least recently used record, and unpin the layer-program entries its graphs point into: an entry no other
+        live graph pins goes with it (a graph holds raw pointers into the entries' buffers, so neither may outlive the other)."""
+        torch.cuda.synchronize()
+        rec = self.graphs.pop(next(iter(self.graphs)))
+        for p, k in rec["pins"]:
+            p.unpin(k)
+
+    def _replay(self, Is, It, It_bg=None):
+        """Copy the inputs into their record's static buffers and replay its graph on the current stream; returns the record."""
+        inputs = [_as_tensor(a) for a in (Is, It, It_bg)]
+        rec = self.prepare(*inputs)
+        for buf, a in zip(rec["inputs"], inputs):
+            if a is not None:
+                buf.copy_(a, non_blocking=True)
+        rec["graph"].replay()
+        self.replayed_kernels += rec["n_kernels"]
+        return rec
+
+    def _queue(self, L, *ctx):
+        """Queue the D2H of ``L["pair"]``'s records and background map into L's own pinned buffers; returns the ticket (``ctx``:
+        what ``_unpack`` takes after the shapes)."""
+        pair = L["pair"]
+        if "host" not in L:
+            L["host"] = torch.empty(pair.packed.numel(), dtype=pair.packed.dtype).pin_memory()
+            L["host_bg"] = None if pair.bg is None else torch.empty(pair.bg.numel(), dtype=pair.bg.dtype).pin_memory()
+        L["host"].copy_(pair.packed.reshape(-1), non_blocking=True)
+        if pair.bg is not None:
+            L["host_bg"].copy_(pair.bg.reshape(-1), non_blocking=True)
+        done = torch.cuda.Event()
+        done.record()
+        return (L, done, ctx)
+
+    def enqueue(self, Is, It, It_bg=None):
         """Queue one pair on the CURRENT stream without waiting for it: input copies (H2D when the images are pinned host
         tensors), one graph replay, one D2H of the packed results into this aligner's own pinned buffer.  Returns a
         ticket for ``fetch``.  The ticket's buffers are reused by the next ``enqueue`` with the same sizes."""
-        if isinstance(Is, np.ndarray):
-            Is, It = torch.from_numpy(Is), torch.from_numpy(It)
-        c = self.prepare(Is, It)
-        c["s_in"].copy_(Is, non_blocking=True)
-        c["t_in"].copy_(It, non_blocking=True)
-        c["graph"].replay()
-        self.replayed_kernels += c["n_kernels"]
-        if "host" not in c:
-            c["host"] = torch.empty(c["packed"].numel(), dtype=c["packed"].dtype).pin_memory()
-        c["host"].copy_(c["packed"].reshape(-1), non_blocking=True)
-        if c["bg"] is not None:                                # the background map: a uint8 buffer of its own
-            if "host_bg" not in c:
-                c["host_bg"] = torch.empty(c["bg"].numel(), dtype=torch.uint8).pin_memory()
-            c["host_bg"].copy_(c["bg"].reshape(-1), non_blocking=True)
-        done = torch.cuda.Event()
-        done.record()
-        return (c, done)
+        return self._queue(self._replay(Is, It, It_bg))
 
     def fetch(self, ticket, copy=True):
-        """Wait for a ticket and unpack it (same dict as ``align_pair_single``).  ``flow12`` is the graph's static output
-        buffer: it is cloned so that results collected over several replays stay valid (``copy=False`` returns the live
-        buffer, overwritten by the next replay with these input sizes)."""
-        c, done = ticket
+        """Wait for a ticket and unpack it (the dict of the eager entry point: ``align_pair_single``'s here).  The device maps
+        (``flow12``; KITTI's ``maps``) are the graph's static output buffers: they are cloned so that results collected over
+        several replays stay valid (``copy=False`` returns the live buffers, overwritten by the next replay with these input
+        sizes)."""
+        L, done, ctx = ticket
         done.synchronize()
-        f12 = c["flow12"]
-        out = self._unpack(c["host"].numpy().copy(), (f12.clone() if copy else f12) if f12 is not None else None, c["size"], c["f8shape"])
-        if c["bg"] is not None:
-            out["It_bg"] = c["host_bg"].numpy().reshape(c["size"]).astype(bool)
-        return out
+        pair = L["pair"]
+        bg = None if pair.bg is None else L["host_bg"].numpy()
+        return self._unpack(L["host"].numpy().copy(), bg, _clone(pair.maps) if copy else pair.maps, pair.size, pair.shapes, *ctx)
 
-    def __call__(self, Is, It, copy=True):
-        """Is, It: uint8 (H, W, 3) torch tensors (CUDA, or pinned host for an asynchronous H2D) or numpy arrays."""
-        return self.fetch(self.enqueue(Is, It), copy)
+    def __call__(self, Is, It, copy=True, It_bg=None):
+        """Is, It: uint8 (H, W, 3) torch tensors (CUDA, or pinned host for an asynchronous H2D) or numpy arrays.  ``It_bg``: a
+        float32 (H, W) background map of the target, for the aligners that take one (``GraphedYfccAligner``)."""
+        return self.fetch(self.enqueue(Is, It, It_bg), copy)
+
+
+def _require_segnet(coarseModel):
+    """``coarseModel``'s segNet; ``skyFromSeg``'s NotImplementedError without one."""
+    seg = getattr(coarseModel, "segNet", None)
+    if seg is None:
+        raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
+    return seg
 
 
 def _sky_background(coarseModel, It):
     """evaluation/evalCorr/evaluation.py:184-189 on the device: segNet's mask of the original target ``It`` (a path, PIL image or
     uint8 (H, W, 3) CUDA tensor), resized to the resized target like ``imresize(It_bg, (h, w)) < 128``.  Returns the bool
     (h, w) CUDA map (True = kept).  Nothing is read back to the host."""
-    seg = getattr(coarseModel, "segNet", None)
-    if seg is None:
-        raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
     Itw, Ith = coarseModel.target_size
-    return ops.imresize_keep(seg.run(It)[0], Ith, Itw)
+    return ops.imresize_keep(_require_segnet(coarseModel).run(It)[0], Ith, Itw)
 
 
 def _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_match21, samples=None, segNet=False):
@@ -296,15 +352,13 @@ def _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_ma
     One packed result tensor: per hypothesis [alive, status, nbMatch, nbInlier, H(9), flowDown8, matchDown8] - the tensors
     the drivers save (evaluation.py:244-260); the full-resolution maps stay on the device and are not returned.
     ``segNet`` (the drivers' ``--segNet``): the background map of the target (``_sky_background``) masks every hypothesis,
-    the first included (:211-243 with ``It_bg``); it is returned as a fifth item, a uint8 (h, w) CUDA map (1 = kept)."""
+    the first included (:211-243 with ``It_bg``); it is the pair's ``bg``, a bool (h, w) CUDA map (True = kept)."""
     coarseModel.setPair(Is, It)
     keep = _sky_background(coarseModel, It) if segNet else None
     bg = keep.float() if segNet else None
     recs, f8shape = _hypothesis_loop(coarseModel, network, maxCoarse, maskRegionTh, with_match21, bg, samples)
     Itw, Ith = coarseModel.target_size
-    if segNet:
-        return torch.cat(recs), None, (Ith, Itw), f8shape, keep.view(torch.uint8)
-    return torch.cat(recs), None, (Ith, Itw), f8shape
+    return DevicePair(torch.cat(recs), None, (Ith, Itw), f8shape, keep)
 
 
 def _hypothesis_loop(coarseModel, network, maxCoarse, maskRegionTh, with_match21, bg, samples, region64=False):
@@ -354,20 +408,47 @@ def _hypothesis_step(coarseModel, network, k, Mask, alive, bg, featt, box, maskR
     return Mask, alive, featt, rec, tuple(f8.shape)
 
 
-def _unpack_multi(host, size, f8shape, nhyp):
-    host = host.reshape(nhyp, -1)
-    if host[0, 1] == 2 or any(host[i, 1] == 2 and host[:i, 0].all() for i in range(nhyp)):
+# the per-hypothesis record of the device loops (multi-hypothesis, KITTI, YFCC): [alive, status, nbMatch, nbInlier, H(9), payload]
+_ALIVE, _STATUS, _NBMATCH, _NBINLIER, _H, _PAYLOAD = 0, 1, 2, 3, slice(4, 13), 13
+
+
+def _accepted(host, nhyp):
+    """The ``nhyp`` records of a device loop -> (n, the records of the hypotheses before the first dead one).  A RANSAC without
+    a model (status 2) in a hypothesis the reference reaches raises utils/outil.py:162's ``TypeError``."""
+    rows = host.reshape(nhyp, -1)
+    if any(rows[i, _STATUS] == 2 and rows[:i, _ALIVE].all() for i in range(nhyp)):
         raise TypeError("'NoneType' object is not subscriptable")          # utils/outil.py:162
     n = 0
-    while n < nhyp and host[n, 0] > 0.5:
+    while n < nhyp and rows[n, _ALIVE] > 0.5:
         n += 1
-    if n == 0:
-        return dict(H=np.zeros((0,)), flowDown8=np.zeros((0,)), matchDown8=np.zeros((0,)), flow12=[], match=[], nbMatch=[], nbInlier=[])
-    n8 = int(np.prod(f8shape))
-    return dict(H=host[:n, 4:13].reshape(n, 3, 3).astype(np.float32),
-                flowDown8=host[:n, 13:13 + n8].reshape((n,) + tuple(f8shape[1:])),
-                matchDown8=host[:n, 13 + n8:13 + 2 * n8].reshape(n, 2, f8shape[2], f8shape[3]),
-                flow12=[], match=[], nbMatch=[int(v) for v in host[:n, 2]], nbInlier=[int(v) for v in host[:n, 3]])
+    return n, rows[:n]
+
+
+def _split(rows, shapes):
+    """Accepted records -> [H (n,3,3) float32] + their payload cut into one (n,) + shape[1:] array per per-hypothesis shape;
+    np.zeros((0,)) for each when no hypothesis was accepted."""
+    if len(rows) == 0:
+        return [np.zeros((0,)) for _ in range(1 + len(shapes))]
+    out, o = [rows[:, _H].reshape(-1, 3, 3).astype(np.float32)], _PAYLOAD
+    for shape in shapes:
+        m = int(np.prod(shape))
+        out.append(rows[:, o:o + m].reshape((len(rows),) + tuple(shape[1:])))
+        o += m
+    return out
+
+
+def _counts(rows):
+    return dict(nbMatch=[int(v) for v in rows[:, _NBMATCH]], nbInlier=[int(v) for v in rows[:, _NBINLIER]])
+
+
+def _unpack_multi(host, size, f8shape, nhyp, bg=None):
+    """The host side of ``_multi_device``: the hypotheses up to the first dead one, in ``align_pair_multi``'s dict."""
+    n, rows = _accepted(host, nhyp)
+    out = dict(flow12=[], match=[], **_counts(rows))
+    out["H"], out["flowDown8"], out["matchDown8"] = _split(rows, [f8shape, (1, 2) + tuple(f8shape[2:])])
+    if bg is not None:
+        out["It_bg"] = bg.reshape(size).astype(bool)
+    return out
 
 
 def align_pair_multi(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.01, with_match21=True, samples=None, segNet=False):
@@ -375,11 +456,9 @@ def align_pair_multi(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.
     Returns H / flowDown8 / matchDown8 / nbMatch / nbInlier of the accepted hypotheses (what the drivers save).  ``segNet``:
     the sky of the target is masked as the drivers' ``--segNet`` masks it (the ``coarseModel`` needs ``segNet=True``), and the
     result has ``It_bg``, the (h, w) bool background map the drivers save as ``maskBG_*``."""
-    packed, _, size, f8shape, *aux = _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_match21, samples, segNet)
-    out = _unpack_multi(_to_host(packed).copy(), size, f8shape, maxCoarse + 1)
-    if segNet:
-        out["It_bg"] = _to_host(aux[0]).reshape(size).astype(bool)
-    return out
+    pair = _multi_device(coarseModel, network, Is, It, maxCoarse, maskRegionTh, with_match21, samples, segNet)
+    host, bg = _read_back(pair)
+    return _unpack_multi(host, pair.size, pair.shapes, maxCoarse + 1, bg)
 
 
 class GraphedMultiAligner(GraphedAligner):
@@ -390,16 +469,16 @@ class GraphedMultiAligner(GraphedAligner):
     def __init__(self, coarseModel, network, maxCoarse=10, maskRegionTh=0.01, with_match21=True, warmup=2, max_graphs=4, segNet=False):
         """``segNet`` (the drivers' ``--segNet``): segNet and the background-map resize run inside the graph, every hypothesis
         is masked with the background, and ``fetch`` also returns ``It_bg`` (``align_pair_multi(segNet=True)``)."""
-        if segNet and getattr(coarseModel, "segNet", None) is None:
-            raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
+        if segNet:
+            _require_segnet(coarseModel)
         super().__init__(coarseModel, network, with_match21=with_match21, warmup=warmup, max_graphs=max_graphs)
         self.maxCoarse, self.maskRegionTh, self.segNet = maxCoarse, maskRegionTh, bool(segNet)
 
     def _device(self, s_in, t_in):
         return _multi_device(self.coarse, self.net, s_in, t_in, self.maxCoarse, self.maskRegionTh, self.m21, segNet=self.segNet)
 
-    def _unpack(self, host, flow12, size, f8shape):
-        return _unpack_multi(host, size, f8shape, self.maxCoarse + 1)
+    def _unpack(self, host, bg, maps, size, shapes):
+        return _unpack_multi(host, size, shapes, self.maxCoarse + 1, bg)
 
 
 class ConcurrentAligner:
@@ -766,19 +845,7 @@ def PredFlowMask_kitti_device(IsSample, ItSample, flowCoarse, size, network, ali
     ``featt`` (a Ragged): the target's fine features from an earlier batch, so only the source goes through the
     FeatureExtractor; ``feat_box`` (a dict) receives the target's features of this batch under "featt"."""
     with torch.no_grad():
-        if featt is None:
-            f = fine_features(network["netFeatCoarse"], torch.cat([IsSample, ItSample], dim=0))
-            n = f.data.shape[0] // 2
-            fs, ft = Ragged(f.data[:n], f.hw[:1]), Ragged(f.data[n:], f.hw[1:])
-            if feat_box is not None:
-                feat_box["featt"] = ft
-        else:
-            fs, ft = fine_features(network["netFeatCoarse"], IsSample), featt
-        k, ld, tc = network["netCorr"].kernelSize, network["netFlowCoarse"].CORR_LD, model.fine_engine()
-        if tc == ops.ENGINE_SPLIT:
-            corr12, both = ops.corr_neigh_pair_split(ft, fs, k, ld)
-        else:
-            corr12, _, both = ops.corr_neigh_pair(ft, fs, k, ld, tc)
+        corr12, both, _held = _fine_corr(network, IsSample, ItSample, featt, feat_box)
         flowDown8 = network["netFlowCoarse"].forward_ragged(corr12)
         mboth = network["netMatch"].forward_ragged(both)                    # (2,1,h8,w8): match12, match21
         flow12, match, _ = ops.compose_fine(flowDown8, mboth[0:1], mboth[1:2], flowCoarse, clamp=True, align_corners=align_corners,
@@ -909,8 +976,9 @@ def _kitti_device(coarseModel, network, Is_u8, It_u8, fineSize, cc_th, maskRegio
         computed but dropped by the host when it unpacks.
     ``Is_u8`` / ``It_u8``: uint8 (H, W, 3) CUDA images.  ``segNet``: the background of :245-250 is segNet's map of the target,
     byte-scaled to the original size (``ops.imresize_mask``).  Returns (packed records, per-hypothesis (flow (1,H,W,2),
-    match (H,W)) CUDA maps, (h_org, w_org), (flow_d2 shape, flow shape)[, the uint8 (h_org, w_org) background map]); one record
-    per hypothesis: [alive, status, nbMatch, nbInlier, H(9), Finetune_D2, Finetune_Mask, Finetune]."""
+    match (H,W)) CUDA maps, (h_org, w_org), (flow_d2 shape, flow shape)[, the uint8 (h_org, w_org) background map]), the
+    fields of a ``DevicePair`` in order; one record per hypothesis: [alive, status, nbMatch, nbInlier, H(9), Finetune_D2,
+    Finetune_Mask, Finetune]."""
     with torch.no_grad():
         h_org, w_org = int(It_u8.shape[0]), int(It_u8.shape[1])
         w_r, h_r = fine_sizes(w_org, h_org, 8, fineSize)
@@ -922,10 +990,7 @@ def _kitti_device(coarseModel, network, Is_u8, It_u8, fineSize, cc_th, maskRegio
         coarseModel.setPair(Is_u8, It_u8)
         dev = It_u8.device
         if segNet:
-            seg = getattr(coarseModel, "segNet", None)
-            if seg is None:
-                raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
-            bg = ops.imresize_mask(seg.run(It_u8)[0], h_org, w_org)              # :248
+            bg = ops.imresize_mask(_require_segnet(coarseModel).run(It_u8)[0], h_org, w_org)              # :248
         else:
             bg = torch.ones((h_org, w_org), device=dev)
         Mask = torch.zeros((h_org, w_org), device=dev)
@@ -954,30 +1019,19 @@ def _kitti_device(coarseModel, network, Is_u8, It_u8, fineSize, cc_th, maskRegio
             maps.append((flowFine_org, match))
             shapes = (tuple(flowFine_d2.shape), tuple(f8.shape))
         packed = torch.cat(recs)
-    if segNet:
-        return packed, maps, (h_org, w_org), shapes, bg.to(torch.uint8)
-    return packed, maps, (h_org, w_org), shapes
+    out = (packed, maps, (h_org, w_org), shapes)
+    return out + (bg.to(torch.uint8),) if segNet else out
 
 
-def _unpack_kitti(host, maps, size, shapes, maxH):
-    """The host side of ``_kitti_device``: the hypotheses up to the first dead one, in ``align_pair_kitti``'s dict."""
-    host = host.reshape(maxH, -1)
-    if any(host[i, 1] == 2 and host[:i, 0].all() for i in range(maxH)):
-        raise TypeError("'NoneType' object is not subscriptable")          # utils/outil.py:162
-    n = 0
-    while n < maxH and host[n, 0] > 0.5:
-        n += 1
-    base = dict(maps=list(maps[:n]), size=tuple(size), nbMatch=[int(v) for v in host[:n, 2]], nbInlier=[int(v) for v in host[:n, 3]],
-                capped=n == maxH)
-    if n == 0:
-        return dict(H=np.zeros((0,)), flow_d2=np.zeros((0,)), mask=np.zeros((0,)), flow=np.zeros((0,)), **base)
+def _unpack_kitti(host, maps, size, shapes, maxH, bg=None):
+    """The host side of ``_kitti_device``: the hypotheses up to the first dead one, in ``align_pair_kitti_graph``'s dict."""
+    n, rows = _accepted(host, maxH)
+    out = dict(maps=list(maps[:n]), size=tuple(size), capped=n == maxH, **_counts(rows))
     d2shape, f8shape = shapes
-    nd, n8 = int(np.prod(d2shape)), int(np.prod(f8shape))
-    o = 13
-    return dict(H=host[:n, 4:13].reshape(n, 3, 3).astype(np.float32),
-                flow_d2=host[:n, o:o + nd].reshape((n,) + tuple(d2shape[1:])),
-                mask=host[:n, o + nd:o + nd + n8].reshape((n,) + tuple(f8shape[1:])),
-                flow=host[:n, o + nd + n8:o + nd + 2 * n8].reshape((n,) + tuple(f8shape[1:])), **base)
+    out["H"], out["flow_d2"], out["mask"], out["flow"] = _split(rows, [d2shape, f8shape, f8shape])
+    if bg is not None:
+        out["It_bg"] = bg.reshape(size).astype(bool)
+    return out
 
 
 def _as_device_u8(coarseModel, I):
@@ -998,12 +1052,10 @@ def align_pair_kitti_graph(coarseModel, network, Is, It, fineSize=650, cc_th=0.0
     if maxH is None or int(maxH) < 1:
         raise ValueError("align_pair_kitti_graph: maxH must be a positive hypothesis cap")
     maxH = int(maxH)
-    packed, maps, size, shapes, *aux = _kitti_device(coarseModel, network, _as_device_u8(coarseModel, Is), _as_device_u8(coarseModel, It),
-                                                     fineSize, cc_th, maskRegionTh, maxH, segNet, samples)
-    out = _unpack_kitti(_to_host(packed).copy(), maps, size, shapes, maxH)
-    if segNet:
-        out["It_bg"] = _to_host(aux[0]).reshape(size).astype(bool)
-    return out
+    pair = DevicePair(*_kitti_device(coarseModel, network, _as_device_u8(coarseModel, Is), _as_device_u8(coarseModel, It), fineSize,
+                                     cc_th, maskRegionTh, maxH, segNet, samples))
+    host, bg = _read_back(pair)
+    return _unpack_kitti(host, pair.maps, pair.size, pair.shapes, maxH, bg)
 
 
 class GraphedKittiAligner(GraphedAligner):
@@ -1014,28 +1066,19 @@ class GraphedKittiAligner(GraphedAligner):
     these input sizes)."""
 
     def __init__(self, coarseModel, network, fineSize=650, cc_th=0.01, maskRegionTh=0.005, maxH=5, segNet=False, warmup=2, max_graphs=4):
-        if segNet and getattr(coarseModel, "segNet", None) is None:
-            raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
+        if segNet:
+            _require_segnet(coarseModel)
         if maxH is None or int(maxH) < 1:
             raise ValueError("GraphedKittiAligner: maxH must be a positive hypothesis cap")
         super().__init__(coarseModel, network, warmup=warmup, max_graphs=max_graphs)
         self.fineSize, self.cc_th, self.maskRegionTh, self.maxH, self.segNet = fineSize, cc_th, maskRegionTh, int(maxH), bool(segNet)
 
     def _device(self, s_in, t_in):
-        return _kitti_device(self.coarse, self.net, s_in, t_in, self.fineSize, self.cc_th, self.maskRegionTh, self.maxH, self.segNet)
+        return DevicePair(*_kitti_device(self.coarse, self.net, s_in, t_in, self.fineSize, self.cc_th, self.maskRegionTh, self.maxH,
+                                         self.segNet))
 
-    def _unpack(self, host, maps, size, shapes):
-        return _unpack_kitti(host, maps, size, shapes, self.maxH)
-
-    def fetch(self, ticket, copy=True):
-        c, done = ticket
-        done.synchronize()
-        out = self._unpack(c["host"].numpy().copy(), c["flow12"], c["size"], c["f8shape"])
-        if copy:
-            out["maps"] = [(f.clone(), m.clone()) for f, m in out["maps"]]
-        if c["bg"] is not None:
-            out["It_bg"] = c["host_bg"].numpy().reshape(c["size"]).astype(bool)
-        return out
+    def _unpack(self, host, bg, maps, size, shapes):
+        return _unpack_kitti(host, maps, size, shapes, self.maxH, bg)
 
 
 def getFlow_all_kitti(param, flowd2, flow, match, outH, outW, th=1.0, cc_th=0.01, multiH=True, interpolate=False):

@@ -5,6 +5,7 @@ The topology is written in Python next to the mirror of the reference module it 
 (model.py, coarseAlignFeatMatch.py); this class only assigns buffer slots, sizes and caches the
 activation buffers (stable device pointers => the library's TMA-descriptor cache always hits).
 """
+import contextlib
 import ctypes as C
 
 import torch
@@ -26,6 +27,20 @@ class rf_layer_t(C.Structure):
 lib.rf_run_layers.restype = C.c_int
 lib.rf_run_layers.argtypes = [C.POINTER(rf_layer_t), C.c_int, C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_int), C.c_int, C.c_void_p]
 
+_recordings = []
+
+
+@contextlib.contextmanager
+def recording():
+    """Collects the (program, key) of every compiled entry that ``LayerProgram.run`` uses inside the scope: a CUDA graph
+    captured in it points into those entries' activation buffers."""
+    used = set()
+    _recordings.append(used)
+    try:
+        yield used
+    finally:
+        _recordings.pop()
+
 
 class LayerProgram:
     """Symbolic tensors are integers; tensor 0 is the input."""
@@ -39,6 +54,7 @@ class LayerProgram:
         self.dual = {}           # op index -> (second input tensor, its channels, its stride)   (RF_OP_CONV_DUAL, split engine only)
         self.dil = {}            # op index -> dilation of a 3x3 / stride-1 conv (split engine only)
         self._compiled = {}
+        self._pins = {}          # compiled key -> number of live CUDA graphs pointing into its buffers
 
     # -- topology --------------------------------------------------------------------------------
     def conv(self, src, fc, relu, res=None, out_f32=False, tf32=False, dil=1):
@@ -224,12 +240,12 @@ class LayerProgram:
         assert split or not getattr(self, "split_only", False), "this program uses split-engine-only layers (conv_dual, dilation)"
         key = (tuple(x.hw), str(x.data.device), int(engine) if (f16 or split) else 0)
         if key not in self._compiled:
-            # compiled entries own the activation buffers; captured CUDA graphs hold raw pointers into them, so entries are
-            # never evicted behind a live graph's back: the cache only grows (one entry per image-set signature; callers with
-            # many sizes bound it with `release()` once no graph / result refers to the buffers any more)
+            # compiled entries own the activation buffers, and captured CUDA graphs hold raw pointers into them: an entry goes
+            # only with the last ``unpin`` of the graphs that pinned it; entries no graph pinned stay (one per image-set signature)
             self._compiled[key] = self._compile(x.hw, x.data.device, f16, split)
         c = self._compiled[key]
-        self.__dict__.setdefault("_touched", set()).add(key)       # pipeline.GraphedAligner ties graphs to the entries they use
+        for used in _recordings:
+            used.add((self, key))
         assert x.data.dtype == c["in_dtype"], (x.data.dtype, c["in_dtype"])
         slots = (C.c_void_p * c["nslots"])()
         slots[0] = x.data.data_ptr()
@@ -240,8 +256,12 @@ class LayerProgram:
         out = out.view(2, -1, self.chan[-1]) if c["out_split"] else out.view(-1, self.chan[-1])
         return out, c["out_hw"]
 
-    def release(self, keep=()):
-        """Drop the compiled entries (activation buffers) of every image-set signature except those in ``keep``.  Only safe
-        when no captured CUDA graph and no live result view refers to them (pipeline.GraphedAligner.release does both)."""
-        for k in [k for k in self._compiled if k not in keep]:
-            del self._compiled[k]
+    def pin(self, key):
+        """One more CUDA graph points into the buffers of the compiled entry ``key``: it stays until the matching ``unpin``."""
+        self._pins[key] = self._pins.get(key, 0) + 1
+
+    def unpin(self, key):
+        """Drops one pin of entry ``key``; the last one deletes the entry (a later run at its signature compiles it again)."""
+        self._pins[key] -= 1
+        if not self._pins[key]:
+            del self._pins[key], self._compiled[key]

@@ -18,7 +18,7 @@ import ctypes as C
 import numpy as np
 import torch
 
-from . import _lib, ops, pipeline
+from . import ops, pipeline
 from ._lib import check, lib, need_cuda, ptr, stream
 from .ops import Ragged
 
@@ -148,10 +148,7 @@ def _search_device(c, Is_u8, It_u8, maxCoarse, It_bg=None, segNet=False, samples
     c._set_rotated_pair(Is_u8, It_u8)
     dev = It_u8.device
     if segNet:
-        seg = getattr(c, "segNet", None)
-        if seg is None:
-            raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
-        It_bg = seg.run(It_u8)[0]
+        It_bg = pipeline._require_segnet(c).run(It_u8)[0]
     draws = DrawnTables(c.nbIter, c.nbPoint, 4 + maxCoarse + 1, dev, c.sample_generator, samples)
     bgs, found = [], []
     for k in range(4):
@@ -175,7 +172,8 @@ def _loop_device(c, network, S, cls, maxCoarse, maskRegionTh):
     """The hypothesis loop on the winner of ``S`` (``_search_device``), for the rotations of orientation class ``cls``: the
     winner's uint8 target, raw conv4 rows and background map are copied by the record's device index into buffers of this
     loop, then ``pipeline._hypothesis_loop`` runs ``maxCoarse + 1`` hypotheses, RANSAC calls 4.. of the slot chain.  Returns
-    the packed records, the background map (or None), the target size (h, w) and the flowDown8 shape."""
+    the packed records, the background map (or None), the target size (h, w), the flowDown8 shape and the loop's copies of the
+    winner (``u8``, ``raw``: a captured loop writes them on every replay, so they live as long as this dict)."""
     ks = S["classes"][cls]
     k0 = ks[0]
     c.__dict__.update(S["src"])
@@ -194,6 +192,11 @@ def _loop_device(c, network, S, cls, maxCoarse, maskRegionTh):
     return dict(packed=torch.cat(recs), bg=bg, size=(h, w), f8shape=f8shape, u8=u8, raw=raw)
 
 
+def _loop_pair(L):
+    """A ``_loop_device`` result as the ``pipeline.DevicePair`` it is (no maps; ``bg`` the float32 background map or None)."""
+    return pipeline.DevicePair(L["packed"], None, L["size"], L["f8shape"], L["bg"])
+
+
 def unpack_record(rec):
     """The select record as (winner, the four scores, rotations that drew, error flag, orientation class) host ints."""
     rec = np.asarray(rec).reshape(-1)
@@ -207,11 +210,12 @@ def _raise_on_error(rec):
 
 
 def _result(rec, host, bg_host, size, f8shape, maxCoarse):
-    """``align_pair_yfcc``'s dict (without the full-resolution maps) from the record and the loop's records."""
+    """``align_pair_yfcc``'s dict (without the full-resolution maps) from the search's select record and the loop's records
+    and background map."""
     winner, scores, _, _, _ = unpack_record(rec)
-    out = pipeline._unpack_multi(host, size, f8shape, maxCoarse + 1)
-    It_bg = np.ones(size, dtype=bool) if bg_host is None else bg_host.reshape(size).astype(bool)
-    out.update(angle=pipeline.YFCC_ANGLES[winner], nbInlierRot=scores, It_bg=It_bg)
+    out = pipeline._unpack_multi(host, size, f8shape, maxCoarse + 1, bg_host)
+    out.setdefault("It_bg", np.ones(size, dtype=bool))
+    out.update(angle=pipeline.YFCC_ANGLES[winner], nbInlierRot=scores)
     return out
 
 
@@ -231,130 +235,62 @@ def align_pair_yfcc_graph(coarseModel, network, Is, It, maxCoarse=10, maskRegion
         if It_bg is not None and not It_bg.is_cuda:
             It_bg = It_bg.to(torch.device("cuda", torch.cuda.current_device()))
         S = _search_device(c, pipeline._as_device_u8(c, Is), pipeline._as_device_u8(c, It), maxCoarse, It_bg, segNet, samples)
-        rec = pipeline._to_host(S["rec"]).copy()
-        _raise_on_error(rec)
-        L = _loop_device(c, network, S, unpack_record(rec)[4], maxCoarse, maskRegionTh)
-        host = pipeline._to_host(L["packed"]).copy()
-        bg = pipeline._to_host(L["bg"]).copy() if L["bg"] is not None else None
-    return _result(rec, host, bg, L["size"], L["f8shape"], maxCoarse)
+        sel = pipeline._to_host(S["rec"]).copy()
+        _raise_on_error(sel)
+        L = _loop_device(c, network, S, unpack_record(sel)[4], maxCoarse, maskRegionTh)
+        host, bg = pipeline._read_back(_loop_pair(L))
+    return _result(sel, host, bg, L["size"], L["f8shape"], maxCoarse)
 
 
 class GraphedYfccAligner(pipeline.GraphedAligner):
-    """evalYFCC's pair as CUDA graphs per (source shape, target shape[, background given]): the search graph and one loop graph
+    """evalYFCC's pair as CUDA graphs per (source shape, target shape[, background shape]): the search graph and one loop graph
     per orientation class (one for a square target), sharing one memory pool and held by one LRU record.  ``enqueue`` replays
     the search graph, waits for its record alone, replays the loop graph of the winner's class and queues the D2H of its
-    records; ``fetch`` returns ``align_pair_yfcc_graph``'s dict.  It can be a ``ConcurrentAligner`` lane (``make_aligner``)."""
+    records; ``fetch`` returns ``align_pair_yfcc_graph``'s dict (``copy`` is accepted for the lanes' interface: no device map
+    is returned).  ``It_bg`` (``prepare`` / ``enqueue`` / call): a float32 (H, W) background map of the target instead of
+    segNet's.  It can be a ``ConcurrentAligner`` lane (``make_aligner``)."""
 
     def __init__(self, coarseModel, network, maxCoarse=10, maskRegionTh=0.01, segNet=False, warmup=2, max_graphs=4):
         """``segNet``: segNet's map of the target masks the sky inside the search graph (``align_pair_yfcc_graph(segNet=True)``)."""
-        if segNet and getattr(coarseModel, "segNet", None) is None:
-            raise NotImplementedError("skyFromSeg needs a CoarseAlign built with segNet=True")
+        if segNet:
+            pipeline._require_segnet(coarseModel)
         super().__init__(coarseModel, network, with_match21=True, warmup=warmup, max_graphs=max_graphs)
         self.maxCoarse, self.maskRegionTh, self.segNet = int(maxCoarse), maskRegionTh, bool(segNet)
 
-    def _search(self, s_in, t_in, bg_in):
-        return _search_device(self.coarse, s_in, t_in, self.maxCoarse, bg_in, self.segNet)
+    def _unpack(self, host, bg, maps, size, shapes, sel):
+        return _result(sel, host, bg, size, shapes, self.maxCoarse)
 
-    def _loop(self, S, cls):
-        return _loop_device(self.coarse, self.net, S, cls, self.maxCoarse, self.maskRegionTh)
+    def _build(self, s_in, t_in, bg_in):
+        search = lambda: _search_device(self.coarse, s_in, t_in, self.maxCoarse, bg_in, self.segNet)
+        loop = lambda S, cls: _loop_device(self.coarse, self.net, S, cls, self.maxCoarse, self.maskRegionTh)
 
-    @staticmethod
-    def _inputs(Is, It, It_bg):
-        conv = lambda a: torch.from_numpy(np.ascontiguousarray(a)) if isinstance(a, np.ndarray) else a
-        return conv(Is), conv(It), (None if It_bg is None else conv(It_bg).float())
-
-    def _build(self, Is, It, It_bg):
-        dev = torch.device("cuda", torch.cuda.current_device())
-        s_in = torch.empty(tuple(Is.shape), dtype=torch.uint8, device=dev).copy_(Is)
-        t_in = torch.empty(tuple(It.shape), dtype=torch.uint8, device=dev).copy_(It)
-        bg_in = None if It_bg is None else torch.empty(tuple(It_bg.shape), dtype=torch.float32, device=dev).copy_(It_bg)
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.no_grad(), torch.cuda.stream(side):
-            for _ in range(self.warmup):                       # eager runs: func attributes, TMA maps, caches, layer programs
-                S = self._search(s_in, t_in, bg_in)
-                for cls in sorted({min(S["classes"][c]) for c in (0, 1)}):          # one loop for a square target
-                    S["rec"][REC_WINNER].fill_(cls)                                # the selection forced to this class
-                    self._loop(S, cls)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        if self.generator is not None:
-            g.register_generator_state(self.generator)
-        n0 = _lib.launch_count()
-        with torch.no_grad(), torch.cuda.graph(g):
-            S = self._search(s_in, t_in, bg_in)
-        n_search = _lib.launch_count() - n0
+        def warm():
+            S = search()
+            for cls in sorted({min(S["classes"][c]) for c in (0, 1)}):          # one loop for a square target
+                S["rec"][REC_WINNER].fill_(cls)                                # the selection forced to this class
+                loop(S, cls)
+        self.warm(warm)
+        g, S, n_search = self.capture(search)
         loops, class_map = {}, {}
         for cls in (0, 1):
             first = min(S["classes"][cls])                      # the class of a square target's rotations 1 and 3 is 0's
-            if first in loops:
-                class_map[cls] = first
-                continue
-            gl = torch.cuda.CUDAGraph()
-            n0 = _lib.launch_count()
-            with torch.no_grad(), torch.cuda.graph(gl, pool=g.pool()):
-                L = self._loop(S, cls)
-            loops[first] = dict(graph=gl, n_kernels=_lib.launch_count() - n0, **L)
+            if first not in loops:
+                gl, L, n = self.capture(lambda: loop(S, cls), pool=g.pool())
+                loops[first] = dict(L, graph=gl, pair=_loop_pair(L), n_kernels=n)
             class_map[cls] = first
-        touched = {(id(p), k) for p in self._programs() for k in p._compiled if k in p.__dict__.get("_touched", ())}
-        for p in self._programs():
-            p.__dict__["_touched"] = set()
-        return dict(search=g, S=S, loops=loops, class_map=class_map, n_kernels=n_search, s_in=s_in, t_in=t_in, bg_in=bg_in,
-                    prog_keys=touched, host_rec=torch.empty(REC_WORDS, dtype=torch.int32).pin_memory())
-
-    def prepare(self, Is, It, It_bg=None):
-        """Capture (once) the search graph and every loop graph for these input sizes; returns their record."""
-        Is, It, It_bg = self._inputs(Is, It, It_bg)
-        key = (tuple(Is.shape), tuple(It.shape), It_bg is not None)
-        if key not in self.graphs:
-            while self.max_graphs and len(self.graphs) >= self.max_graphs:
-                self._evict()
-            for p in self._programs():
-                p.__dict__["_touched"] = set()
-            self.graphs[key] = self._build(Is, It, It_bg)
-        else:
-            self.graphs[key] = self.graphs.pop(key)            # most recently used last
-        return self.graphs[key]
+        return dict(graph=g, S=S, loops=loops, class_map=class_map, n_kernels=n_search,
+                    host_rec=torch.empty(REC_WORDS, dtype=torch.int32).pin_memory())
 
     def enqueue(self, Is, It, It_bg=None):
         """Queue one pair on the CURRENT stream: input copies, the search graph, a D2H of its record and a wait for it (the one
         host read inside the pair; ``TypeError`` when RANSAC found no model in a rotation that drew), the loop graph of the
         winner's class and the D2H of its records.  Returns a ticket for ``fetch``."""
-        Is, It, It_bg = self._inputs(Is, It, It_bg)
-        c = self.prepare(Is, It, It_bg)
-        c["s_in"].copy_(Is, non_blocking=True)
-        c["t_in"].copy_(It, non_blocking=True)
-        if It_bg is not None:
-            c["bg_in"].copy_(It_bg, non_blocking=True)
-        c["search"].replay()
-        self.replayed_kernels += c["n_kernels"]
+        c = self._replay(Is, It, It_bg)
         c["host_rec"].copy_(c["S"]["rec"], non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        ev.synchronize()
-        rec = c["host_rec"].numpy().copy()
-        _raise_on_error(rec)
-        L = c["loops"][c["class_map"][unpack_record(rec)[4]]]
+        torch.cuda.current_stream().synchronize()
+        sel = c["host_rec"].numpy().copy()
+        _raise_on_error(sel)
+        L = c["loops"][c["class_map"][unpack_record(sel)[4]]]
         L["graph"].replay()
         self.replayed_kernels += L["n_kernels"]
-        if "host" not in L:
-            L["host"] = torch.empty(L["packed"].numel(), dtype=L["packed"].dtype).pin_memory()
-            L["host_bg"] = None if L["bg"] is None else torch.empty(L["bg"].numel(), dtype=torch.float32).pin_memory()
-        L["host"].copy_(L["packed"].reshape(-1), non_blocking=True)
-        if L["bg"] is not None:
-            L["host_bg"].copy_(L["bg"].reshape(-1), non_blocking=True)
-        done = torch.cuda.Event()
-        done.record()
-        return (L, rec, done)
-
-    def fetch(self, ticket, copy=True):
-        """Wait for a ticket and unpack it (``align_pair_yfcc_graph``'s dict).  ``copy`` is accepted for the lanes' interface: no
-        device map is returned."""
-        L, rec, done = ticket
-        done.synchronize()
-        bg = None if L["host_bg"] is None else L["host_bg"].numpy().copy()
-        return _result(rec, L["host"].numpy().copy(), bg, L["size"], L["f8shape"], self.maxCoarse)
-
-    def __call__(self, Is, It, copy=True, It_bg=None):
-        return self.fetch(self.enqueue(Is, It, It_bg), copy)
+        return self._queue(L, sel)

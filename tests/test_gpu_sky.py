@@ -169,8 +169,6 @@ def test_segnet_graph_launches_and_eviction(rf, sky_pair):
     plain = rf.pipeline.GraphedMultiAligner(c, net, maxCoarse=2, with_match21=True)
     withseg = rf.pipeline.GraphedMultiAligner(c, net, maxCoarse=2, with_match21=True, segNet=True, max_graphs=1)
     n_plain = plain.prepare(s, t)["n_kernels"]
-    del plain                                     # its graph shares the trunk's buffers, which the eviction below may free
-    torch.cuda.synchronize()
     rec = withseg.prepare(s, t)
     H, W = sky_pair["tgt"].shape[:2]
     distinct, _ = seg.plan(H, W)
@@ -193,6 +191,32 @@ def test_segnet_graph_launches_and_eviction(rf, sky_pair):
     left = {(id(p), k) for p in (seg.encoder, seg.head) for k in p._compiled}
     assert len(withseg.graphs) == 1 and not (mine & left) and left
     assert left <= withseg.graphs[next(iter(withseg.graphs))]["prog_keys"]
+
+
+def test_eviction_keeps_what_another_aligner_graph_uses(rf, sky_pair):
+    """Two aligners on one model: their graphs point into the same layer-program entries (the key is the image-set signature).
+    B's eviction leaves every entry A's live graph uses, and A's next replay equals the eager pair bit for bit."""
+    net = networks(rf)
+    c = coarse_seg(rf, sky_pair["segId"])
+    s, t = torch.from_numpy(sky_pair["src"]).cuda(), torch.from_numpy(sky_pair["tgt"]).cuda()
+    A = rf.pipeline.GraphedMultiAligner(c, net, maxCoarse=2, with_match21=True)
+    B = rf.pipeline.GraphedMultiAligner(c, net, maxCoarse=2, with_match21=True, segNet=True, max_graphs=1)
+    a = A.prepare(s, t)
+    b = B.prepare(s, t)
+    shared = a["prog_keys"] & b["prog_keys"]
+    assert shared and {(id(p), k) for p, k in a["pins"]} == a["prog_keys"]
+    src2, tgt2, _ = synth.make_pair(13, 120, 160)
+    B.prepare(torch.from_numpy(src2).cuda(), torch.from_numpy(tgt2).cuda())           # evicts B's first graph
+    assert len(B.graphs) == 1 and all(r is not b for r in B.graphs.values())
+    assert all(k in p._compiled for p, k in a["pins"]), "an entry A's live graph points into was freed"
+    torch.manual_seed(5)
+    got = A(s, t)
+    torch.manual_seed(5)
+    want = rf.pipeline.align_pair_multi(c, net, s, t, maxCoarse=2, with_match21=True)
+    assert len(got["H"]) == len(want["H"]) >= 1
+    for key in ("H", "flowDown8", "matchDown8"):
+        assert np.array_equal(got[key], want[key]), key
+    assert got["nbMatch"] == want["nbMatch"] and got["nbInlier"] == want["nbInlier"]
 
 
 def test_two_lanes_with_segnet_equal_each_lane_alone(rf, sky_pair):
