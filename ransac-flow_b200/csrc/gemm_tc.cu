@@ -26,6 +26,7 @@
 #include <climits>
 #include <mutex>
 #include <unordered_map>
+#include <vector>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -61,8 +62,34 @@ struct alignas(64) WgParams {
     unsigned long long* rowbest;          // correlation
     unsigned long long* colbest;
     int NA, NB;
+#ifdef RF_TILE_TIMELINE
+    unsigned long long* timeline;         // TL_WORDS %globaltimer stamps per convolution tile (null: none)
+#endif
 };
 static_assert(sizeof(WgParams) <= 32764, "kernel parameter space (CUDA 12.1+ large kernel parameters)");
+
+// Per-tile timeline (built only with -DRF_TILE_TIMELINE, by tools/conv_tile_timeline.py): for tile t, words
+// [TL_WORDS t + 5 a + i] hold the %globaltimer (ns) of point i of agent a.  Agents 0 / 1 = thread 0 of consumer warpgroup
+// 0 / 1: tile start, first full barrier passed, last MMA retired, residual barrier passed, store committed (warpgroup 1:
+// its epilogue writes done).  Agent 2 = the producer lane: tile start, first K block issued, last K block issued, the
+// residual's buffer acquired, residual issued.  Word 15: the SM id.
+#ifdef RF_TILE_TIMELINE
+constexpr int TL_WORDS = 16;
+__device__ __forceinline__ unsigned long long tl_now() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
+    return t;
+}
+__device__ __forceinline__ unsigned smid() {
+    unsigned s;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+    return s;
+}
+#define TL_STAMP_IF(c, t, a, i) do { if ((c) && p.timeline) p.timeline[(long long)(t) * TL_WORDS + 5 * (a) + (i)] = tl_now(); } while (0)
+#else
+#define TL_STAMP_IF(c, t, a, i) do {} while (0)
+#endif
+#define TL_STAMP(t, a, i) TL_STAMP_IF(true, t, a, i)
 
 template <int KIND, int BN, int MODE>
 struct WgCfg {
@@ -123,6 +150,7 @@ wg_kernel(const __grid_constant__ WgParams p) {
     constexpr bool SLOT = MODE == MODE_CONV && OUT != O_F32;
     constexpr int BOX_BYTES = (OUT == O_SPLIT ? 2 : 1) * 128 * 128;
     static_assert(!SLOT || (BN / 64) * BOX_BYTES <= Cfg::STAGE_BYTES, "the output tile fits one stage");
+    constexpr int EPI_JC = Cfg::ONE_CTA ? 4 : 2;  // channel pairs per group of epilogue loads: as many as fit without spills
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
@@ -172,6 +200,7 @@ wg_kernel(const __grid_constant__ WgParams p) {
             uint32_t ph = 0;
             for (int t = t_first; t < t_end; t += t_step) {
                 const Tile T = decode(t);
+                TL_STAMP(t, 2, 0);
                 if (!((prefetched >> T.img) & 1u)) {
                     prefetched |= 1u << T.img;
                     tma_prefetch_desc(&p.mapA[T.img]);
@@ -206,10 +235,13 @@ wg_kernel(const __grid_constant__ WgParams p) {
                             tma_load_2d(sb, &p.mapB, &full[st], kcol, T.n0);
                         }
                     }
+                    TL_STAMP_IF(it == 0, t, 2, 1);
+                    TL_STAMP_IF(it == KI - 1, t, 2, 2);
                     if (++st == STAGES) { st = 0; ph ^= 1; }
                 }
                 if constexpr (SLOT) {                  // the epilogue slot: the residual tile, or just the hand-over
                     mbar_wait(&empty[st], ph ^ 1);
+                    TL_STAMP(t, 2, 3);
                     if (p.residual) {
                         const int nb = boxes(T);
                         uint8_t* slot = smem + st * Cfg::STAGE_BYTES;
@@ -221,6 +253,7 @@ wg_kernel(const __grid_constant__ WgParams p) {
                     } else {
                         mbar_arrive(&full[st]);
                     }
+                    TL_STAMP(t, 2, 4);
                     if (++st == STAGES) { st = 0; ph ^= 1; }
                 }
             }
@@ -237,8 +270,12 @@ wg_kernel(const __grid_constant__ WgParams p) {
     int st = 0;
     uint32_t ph = 0;
     bool stored = false;                          // the stage before `st` is an epilogue slot a TMA store may still be reading
+#ifdef RF_TILE_TIMELINE
+    const bool tl = MODE == MODE_CONV && (threadIdx.x & 127) == 0;     // thread 0 of its warpgroup stamps the timeline
+#endif
     for (int t = t_first; t < t_end; t += t_step) {
         const Tile T = decode(t);
+        TL_STAMP_IF(tl, t, g, 0);
         float acc[NACC][BN / 2];
 #pragma unroll
         for (int a = 0; a < NACC; ++a)
@@ -246,6 +283,7 @@ wg_kernel(const __grid_constant__ WgParams p) {
             for (int i = 0; i < BN / 2; ++i) acc[a][i] = 0.f;
         for (int it = 0; it < KI; ++it) {
             mbar_wait(&full[st], ph);
+            TL_STAMP_IF(tl && it == 0, t, g, 1);
             const uint32_t sa = smem_u32(smem + st * Cfg::STAGE_BYTES);
             wg_fence();
             mma_block<KIND, BN, NACC>(acc, sa + g * (64 * 128), sa + Cfg::A_BYTES);
@@ -262,6 +300,7 @@ wg_kernel(const __grid_constant__ WgParams p) {
         wg_wait<0>();
 #pragma unroll
         for (int a = 0; a < NACC; ++a) wg_fence_regs(acc[a]);
+        TL_STAMP_IF(tl, t, g, 2);
         mbar_arrive(&empty[before(st)]);         // the tile's last K block
 
         auto value = [&](int i) -> float {
@@ -274,34 +313,57 @@ wg_kernel(const __grid_constant__ WgParams p) {
             // 128 rows further.  Each thread reads its residual elements and overwrites them with its outputs.
             mbar_wait(&full[st], ph);
             uint8_t* slot = smem + st * Cfg::STAGE_BYTES;
+            TL_STAMP_IF(tl, t, g, 3);
+            // The channel pairs go in groups of EPI_JC: the group's bias (global memory) and residual (the slot) loads are issued
+            // together before its arithmetic, so that a tile pays one load latency per group rather than one per pair (the
+            // guard on n keeps each load from being hoisted past the stores of the pair before it).  The bias of a channel
+            // pair serves both of the thread's rows.
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int m = rbase + 8 * h;
+            for (int j0 = 0; j0 < BN / 8; j0 += EPI_JC) {
+                float2 bv[EPI_JC];
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j) {
-                    const int c = 8 * j + cbase, n = T.n0 + c;
-                    if (n >= p.Cout) continue;    // Cout % 8 == 0: both channels of the pair exist
-                    float v0 = value(4 * j + 2 * h), v1 = value(4 * j + 2 * h + 1);
-                    if (p.bias) { v0 += __ldg(p.bias + n); v1 += __ldg(p.bias + n + 1); }
-                    uint8_t* e = slot + (c >> 6) * BOX_BYTES + m * 128 + ((((c & 63) >> 3) ^ (m & 7)) << 4) + (c & 7) * 2;
-                    if (p.residual) {
-                        if constexpr (OUT == O_F16) {
-                            const float2 r = __half22float2(*reinterpret_cast<const __half2*>(e));
-                            v0 += r.x; v1 += r.y;
-                        } else {
-                            const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(e));
-                            const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(e + 128 * 128));
-                            v0 += fmaf(rl.x, 0.00048828125f, rh.x); v1 += fmaf(rl.y, 0.00048828125f, rh.y);
+                for (int jj = 0; jj < EPI_JC; ++jj) {
+                    const int n = T.n0 + 8 * (j0 + jj) + cbase;
+                    bv[jj] = p.bias && n < p.Cout ? make_float2(__ldg(p.bias + n), __ldg(p.bias + n + 1)) : make_float2(0.f, 0.f);
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int m = rbase + 8 * h;
+                    uint8_t* e[EPI_JC];
+                    __half2 rh[EPI_JC], rl[EPI_JC];
+#pragma unroll
+                    for (int jj = 0; jj < EPI_JC; ++jj) {
+                        const int c = 8 * (j0 + jj) + cbase;
+                        e[jj] = slot + (c >> 6) * BOX_BYTES + m * 128 + ((((c & 63) >> 3) ^ (m & 7)) << 4) + (c & 7) * 2;
+                        if (p.residual) {             // inside the slot whether or not the channels exist
+                            rh[jj] = *reinterpret_cast<const __half2*>(e[jj]);
+                            if constexpr (OUT == O_SPLIT) rl[jj] = *reinterpret_cast<const __half2*>(e[jj] + 128 * 128);
                         }
                     }
-                    if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-                    if constexpr (OUT == O_F16) {
-                        *reinterpret_cast<__half2*>(e) = pack_sat(v0, v1);
-                    } else {
-                        __half2 hi, lo;
-                        split2(v0, v1, hi, lo);
-                        *reinterpret_cast<__half2*>(e) = hi;
-                        *reinterpret_cast<__half2*>(e + 128 * 128) = lo;
+#pragma unroll
+                    for (int jj = 0; jj < EPI_JC; ++jj) {
+                        const int j = j0 + jj, n = T.n0 + 8 * j + cbase;
+                        if (n >= p.Cout) continue;    // Cout % 8 == 0: both channels of the pair exist
+                        float v0 = value(4 * j + 2 * h), v1 = value(4 * j + 2 * h + 1);
+                        if (p.bias) { v0 += bv[jj].x; v1 += bv[jj].y; }
+                        if (p.residual) {
+                            if constexpr (OUT == O_F16) {
+                                const float2 r = __half22float2(rh[jj]);
+                                v0 += r.x; v1 += r.y;
+                            } else {
+                                const float2 fh = __half22float2(rh[jj]), fl = __half22float2(rl[jj]);
+                                v0 += fmaf(fl.x, 0.00048828125f, fh.x); v1 += fmaf(fl.y, 0.00048828125f, fh.y);
+                            }
+                        }
+                        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                        if constexpr (OUT == O_F16) {
+                            *reinterpret_cast<__half2*>(e[jj]) = pack_sat(v0, v1);
+                        } else {
+                            __half2 hi, lo;
+                            split2(v0, v1, hi, lo);
+                            *reinterpret_cast<__half2*>(e[jj]) = hi;
+                            *reinterpret_cast<__half2*>(e[jj] + 128 * 128) = lo;
+                        }
                     }
                 }
             }
@@ -315,6 +377,10 @@ wg_kernel(const __grid_constant__ WgParams p) {
                 }
                 bulk_commit();
             }
+            TL_STAMP_IF(tl, t, g, 4);
+#ifdef RF_TILE_TIMELINE
+            if (threadIdx.x == 0 && p.timeline) p.timeline[(long long)t * TL_WORDS + 15] = smid();
+#endif
             stored = true;
             if (++st == STAGES) { st = 0; ph ^= 1; }
         } else if constexpr (MODE == MODE_CONV) {
@@ -864,6 +930,27 @@ int pick_tw(int Ho, int Wo) {
     return best;
 }
 
+#ifdef RF_TILE_TIMELINE
+// The timeline build's host side: convolution launches take consecutive regions of the caller's buffer, TL_WORDS words per tile,
+// and each launch is listed as TL_LAUNCH_WORDS numbers: word offset (-1: the buffer was full), tiles, CTAs, K blocks, Cout,
+// residual.
+constexpr int TL_LAUNCH_WORDS = 6;
+static std::mutex g_tl_mu;
+static unsigned long long* g_tl_buf = nullptr;
+static long long g_tl_words = 0, g_tl_used = 0;
+static std::vector<long long> g_tl_launches;
+
+static void tl_assign(WgParams& p, int grid, int KI) {
+    std::lock_guard<std::mutex> g(g_tl_mu);
+    const long long need = (long long)p.ntiles * TL_WORDS;
+    const bool fits = g_tl_buf != nullptr && g_tl_used + need <= g_tl_words;
+    p.timeline = fits ? g_tl_buf + g_tl_used : nullptr;
+    const long long rec[TL_LAUNCH_WORDS] = {fits ? g_tl_used : -1, p.ntiles, grid, KI, p.Cout, p.residual != nullptr};
+    g_tl_launches.insert(g_tl_launches.end(), rec, rec + TL_LAUNCH_WORDS);
+    if (fits) g_tl_used += need;
+}
+#endif
+
 template <int KIND, int BN, int MODE, int OUT>
 static int launch_wg(const WgParams& p, dim3 grid, cudaStream_t st) {
     using Cfg = WgCfg<KIND, BN, MODE>;
@@ -882,7 +969,14 @@ static int launch_wg(const WgParams& p, dim3 grid, cudaStream_t st) {
 template <int KIND, int BN, int OUT>
 static int launch_conv_bn(const WgParams& p, cudaStream_t st) {
     const int resident = WgCfg<KIND, BN, MODE_CONV>::CTAS_PER_SM * num_sms();
-    return launch_wg<KIND, BN, MODE_CONV, OUT>(p, dim3(p.ntiles < resident ? p.ntiles : resident), st);
+    const int grid = p.ntiles < resident ? p.ntiles : resident;
+#ifdef RF_TILE_TIMELINE
+    WgParams q = p;
+    tl_assign(q, grid, p.R * p.S * p.Cin / (KIND == K_TF32 ? TC_BK : TC_BK_F16));
+    return launch_wg<KIND, BN, MODE_CONV, OUT>(q, dim3(grid), st);
+#else
+    return launch_wg<KIND, BN, MODE_CONV, OUT>(p, dim3(grid), st);
+#endif
 }
 template <int KIND, int OUT>
 static int launch_conv(const WgParams& p, int BN, cudaStream_t st) {
@@ -1095,6 +1189,26 @@ int rf_stem(ActFormat f, const float* x, int nimg, const int* hw_host, int k, in
     RF_REQUIRE(k == 3 && stride == 1 && !pool, "rf_stem: the 7x7 / stride 2 stem (optionally pooled) or the 3x3 / stride 1 stem");
     return split ? stem_impl<3, 1, true>(x, nimg, hw_host, w, bias, y, 0, stream) : stem_impl<3, 1, false>(x, nimg, hw_host, w, bias, y, 0, stream);
 }
+
+#ifdef RF_TILE_TIMELINE
+// Timeline build only: the convolutions launched from here on stamp their tiles into `buf` (device, `words` 64-bit words,
+// zeroed by the caller), and the launch table starts again.
+extern "C" int rf_tile_timeline_begin(void* buf, long long words) {
+    std::lock_guard<std::mutex> g(g_tl_mu);
+    g_tl_buf = static_cast<unsigned long long*>(buf);
+    g_tl_words = buf ? words : 0;
+    g_tl_used = 0;
+    g_tl_launches.clear();
+    return 0;
+}
+// The launch table since rf_tile_timeline_begin, TL_LAUNCH_WORDS numbers per launch, into out[0 .. max_words); returns its length.
+extern "C" long long rf_tile_timeline_launches(long long* out, long long max_words) {
+    std::lock_guard<std::mutex> g(g_tl_mu);
+    const long long n = (long long)g_tl_launches.size();
+    for (long long i = 0; i < n && i < max_words; ++i) out[i] = g_tl_launches[i];
+    return n;
+}
+#endif
 
 size_t rf_corr_tc_workspace(int NA, int NB, int C) { return 2ull * ((size_t)NA + NB) * C * sizeof(float) + 1024; }
 
