@@ -302,6 +302,11 @@ int rf_warp_grid(const float* H, int N, int h, int w, float* grid_out, void* str
 int rf_grid_sample(const float* in, int N, int C, int Hin, int Win, const long long* in_s_host,
                    const float* grid, int Hout, int Wout, int align_corners,
                    float* out, const long long* out_s_host, void* stream);
+/* train/generate_coarse_aligned_pair.ipynb cells 13 + ToPILImage in one pass: out [h][w][3] uint8 = (uint8)(255 * grid_sample(
+ * ToTensor(src), warp_grid(H, h, w))), truncated, with rf_warp_grid's, rf_grid_sample's and rf_preproc_u8's arithmetic (bit for bit
+ * the composition of the three and the quantisation).  H: 9 floats in DEVICE memory (a non-finite H samples nothing: zeros);
+ * src [Hin][Win][3] uint8. */
+int rf_warp_sample_u8(const float* H, const uint8_t* src, int Hin, int Win, int h, int w, int align_corners, uint8_t* out, void* stream);
 /* F.interpolate(mode='bilinear', align_corners=False): NCHW [NC][h][w] -> [NC][H][W] */
 int rf_upsample_bilinear(const float* in, int NC, int h, int w, int H, int W, float* out, void* stream);
 /* PredFlowMask tail, evaluation/evalHpatch/evaluation.py:37-51 fused:

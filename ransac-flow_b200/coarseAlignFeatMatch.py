@@ -98,15 +98,20 @@ class ResNet50Conv4:
         return Ragged(out, ohw)
 
 
+def resnet50_state(sd):
+    """A ResNet-50 state dict in torchvision's key layout from either a torchvision state dict or a MoCo checkpoint
+    ``{'model': {'module.<key>': ...}}`` (coarseAlignFeatMatch.py:44-47, train/generate_coarse_aligned_pair.ipynb cell 2)."""
+    if "model" in sd:
+        sd = {k.replace("module.", ""): v for k, v in sd["model"].items()}
+    return sd
+
+
 def _load_resnet50_state(imageNet, resnet_state_dict):
     if resnet_state_dict is not None:
         return resnet_state_dict
     path = os.environ.get("RF_RESNET50_WEIGHTS")
     if path:
-        sd = torch.load(path, map_location="cpu")
-        if "model" in sd:           # MoCo checkpoint layout (coarseAlignFeatMatch.py:44-47)
-            sd = {k.replace("module.", ""): v for k, v in sd["model"].items()}
-        return sd
+        return resnet50_state(torch.load(path, map_location="cpu"))
     if imageNet:
         import torchvision.models as models
         return models.resnet50(weights="IMAGENET1K_V1").state_dict()       # needs the torchvision cache / network
@@ -117,6 +122,35 @@ def scale_list(nbScale, scaleR):
     if nbScale == 1:
         return [1]
     return np.linspace(scaleR, 1, nbScale // 2 + 1).tolist() + np.linspace(1, 1 / scaleR, nbScale // 2 + 1).tolist()[1:]
+
+
+def conv4_features(net, u8):
+    """uint8 (H, W, 3) CUDA images -> (their L2-normalised conv4 features as one Ragged, ``u8``): ImageNet ``ToTensor + Normalize``,
+    the ResNet-50 trunk ``net`` on one ragged batch, ``F.normalize`` per row."""
+    hw = [(int(t.shape[0]), int(t.shape[1])) for t in u8]
+    flat = torch.cat([t.reshape(-1, 3) for t in u8], dim=0) if len(u8) > 1 else u8[0].reshape(-1, 3)
+    x = Ragged(ops.preproc_u8(flat, normalize=True), hw)
+    f = net(x)
+    if f.split and outil.corr_precision == 2:
+        # engine 'f16x3' + fp16-split correlation: the normalisation writes the correlation's operand planes directly;
+        # the fp32 views the reference exposes (featsMultiScale, featt) are rebuilt on first access (__getattr__)
+        return Ragged(ops.l2norm_planes(f.data), f.hw), u8
+    return Ragged(ops.l2norm(f.data), f.hw), u8
+
+
+def ransac_device(match1, match2, cnt, nbIter, nbPoint, tolerance, generator=None, samples=None):
+    """utils/outil.py's RANSAC on a device-resident match list of ``cnt`` matches (no host synchronisation): the reference's
+    seeded stream drawn from ``generator`` (None: torch's default CUDA generator; ``SAMPLES_PHILOX64``) or an injected
+    (nbIter, 4) index table.  Returns (H [9], nbInlier [1], mask, status [1]).  ``samples`` may also be one call of a slot
+    chain over tables drawn in advance (``yfcc_graph.DrawnTables``): the call then reads the table its slot selects on the
+    device."""
+    if hasattr(samples, "ransac"):
+        return samples.ransac(match1, match2, cnt, tolerance, 100)
+    if samples is not None:
+        raw, mode = torch.as_tensor(samples, dtype=torch.int64).to(match1.device).contiguous(), ops.SAMPLES_MOD
+    else:
+        raw, mode = ops.philox_words(nbIter, nbPoint, match1.device, generator), ops.SAMPLES_PHILOX64
+    return ops.ransac_homography(match1, match2, raw, tolerance, 100, cnt, mode)
 
 
 class _CoarseAlignBase:
@@ -175,16 +209,7 @@ class _CoarseAlignBase:
 
     def _features(self, images):
         """list of PIL images (or uint8 CUDA HxWx3 tensors) -> (Ragged normalised conv4 features, list of uint8 CUDA images)."""
-        u8 = [im if torch.is_tensor(im) else self._to_device_u8(im) for im in images]
-        hw = [(int(t.shape[0]), int(t.shape[1])) for t in u8]
-        flat = torch.cat([t.reshape(-1, 3) for t in u8], dim=0) if len(u8) > 1 else u8[0].reshape(-1, 3)
-        x = Ragged(ops.preproc_u8(flat, normalize=True), hw)
-        f = self.net(x)
-        if f.split and outil.corr_precision == 2:
-            # engine 'f16x3' + fp16-split correlation: the normalisation writes the correlation's operand planes directly;
-            # the fp32 views the reference exposes (featsMultiScale, featt) are rebuilt on first access (__getattr__)
-            return Ragged(ops.l2norm_planes(f.data), f.hw), u8
-        return Ragged(ops.l2norm(f.data), f.hw), u8
+        return conv4_features(self.net, [im if torch.is_tensor(im) else self._to_device_u8(im) for im in images])
 
     def _pyramid(self, I_org, sizes):
         """Resize ``I_org`` to each (w, h) in ``sizes``: PIL on the host, or the device resampler (always for a CUDA image)."""
@@ -284,17 +309,8 @@ class _CoarseAlignBase:
         return None
 
     def _ransac_device(self, match1, match2, cnt, samples=None):
-        """RANSAC on a device-resident match list of ``cnt`` matches (no host synchronisation): the reference's seeded
-        stream (``SAMPLES_PHILOX64``) or an injected (nbIter, 4) index table.  Returns (H [9], nbInlier [1], mask, status [1]).
-        ``samples`` may also be one call of a slot chain over tables drawn in advance (``yfcc_graph.DrawnTables``): the call
-        then reads the table its slot selects on the device."""
-        if hasattr(samples, "ransac"):
-            return samples.ransac(match1, match2, cnt, self.tolerance, 100)
-        if samples is not None:
-            raw, mode = torch.as_tensor(samples, dtype=torch.int64).to(match1.device).contiguous(), ops.SAMPLES_MOD
-        else:
-            raw, mode = ops.philox_words(self.nbIter, self.nbPoint, match1.device, self.sample_generator), ops.SAMPLES_PHILOX64
-        return ops.ransac_homography(match1, match2, raw, self.tolerance, 100, cnt, mode)
+        """``ransac_device`` with this model's settings and sample generator."""
+        return ransac_device(match1, match2, cnt, self.nbIter, self.nbPoint, self.tolerance, self.sample_generator, samples)
 
     def skyFromSeg(self, path):
         """evaluation/evalHpatch/coarseAlignFeatMatch.py:152-153: the segNet mask of the image at ``path`` (float32 H x W)."""

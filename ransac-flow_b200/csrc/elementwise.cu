@@ -631,6 +631,15 @@ __device__ __forceinline__ float lin11(int i, int n) {
     return (i < n / 2) ? (-1.f + step * (float)i) : (1.f - step * (float)(n - 1 - i));
 }
 
+// the grid point of output pixel (r, c) of an h x w homography grid (H: 9 floats), one rounding per operation
+__device__ __forceinline__ float2 homography_grid_point(const float* __restrict__ H, int r, int c, int h, int w) {
+    float x = lin11(c, w), y = lin11(r, h);
+    float px = __fadd_rn(__fadd_rn(__fmul_rn(H[0], x), __fmul_rn(H[1], y)), H[2]);
+    float py = __fadd_rn(__fadd_rn(__fmul_rn(H[3], x), __fmul_rn(H[4], y)), H[5]);
+    float pz = __fadd_rn(__fadd_rn(__fmul_rn(H[6], x), __fmul_rn(H[7], y)), H[8]);
+    return make_float2(__fdiv_rn(px, pz), __fdiv_rn(py, pz));
+}
+
 __global__ void warp_grid_kernel(const float* __restrict__ Hm, int N, int h, int w, float* __restrict__ grid) {
     long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     long long hw = (long long)h * w;
@@ -638,12 +647,7 @@ __global__ void warp_grid_kernel(const float* __restrict__ Hm, int N, int h, int
     int n = (int)(t / hw);
     int rem = (int)(t - n * hw);
     int r = rem / w, c = rem - r * w;
-    const float* H = Hm + n * 9;
-    float x = lin11(c, w), y = lin11(r, h);
-    float px = __fadd_rn(__fadd_rn(__fmul_rn(H[0], x), __fmul_rn(H[1], y)), H[2]);
-    float py = __fadd_rn(__fadd_rn(__fmul_rn(H[3], x), __fmul_rn(H[4], y)), H[5]);
-    float pz = __fadd_rn(__fadd_rn(__fmul_rn(H[6], x), __fmul_rn(H[7], y)), H[8]);
-    reinterpret_cast<float2*>(grid)[t] = make_float2(__fdiv_rn(px, pz), __fdiv_rn(py, pz));
+    reinterpret_cast<float2*>(grid)[t] = homography_grid_point(Hm + n * 9, r, c, h, w);
 }
 
 __device__ __forceinline__ float unnormalize(float coord, int size, int align_corners) {
@@ -659,6 +663,40 @@ __device__ __forceinline__ float in_int_range(float c) {
 
 struct Strides4 { long long n, c, h, w; };
 
+// F.grid_sample(bilinear, zeros) at one grid point: the top-left tap, the four tap weights and which taps lie inside
+struct BilinearTaps {
+    int x0, y0;
+    float nw, ne, sw, se;
+    bool vx0, vx1, vy0, vy1;
+};
+__device__ __forceinline__ BilinearTaps bilinear_taps(float2 g, int Hin, int Win, int align_corners) {
+    BilinearTaps t;
+    float ix = in_int_range(unnormalize(g.x, Win, align_corners)), iy = in_int_range(unnormalize(g.y, Hin, align_corners));
+    float fx = floorf(ix), fy = floorf(iy);
+    t.x0 = (int)fx;
+    t.y0 = (int)fy;
+    int x1 = t.x0 + 1, y1 = t.y0 + 1;
+    t.nw = (fx + 1.f - ix) * (fy + 1.f - iy);
+    t.ne = (ix - fx) * (fy + 1.f - iy);
+    t.sw = (fx + 1.f - ix) * (iy - fy);
+    t.se = (ix - fx) * (iy - fy);
+    t.vx0 = t.x0 >= 0 && t.x0 < Win;
+    t.vx1 = x1 >= 0 && x1 < Win;
+    t.vy0 = t.y0 >= 0 && t.y0 < Hin;
+    t.vy1 = y1 >= 0 && y1 < Hin;
+    return t;
+}
+// the inside taps' weighted sum, in nw, ne, sw, se order; load(y, x) reads the input value at an inside tap
+template <typename Load>
+__device__ __forceinline__ float bilinear_sum(const BilinearTaps& t, Load load) {
+    float acc = 0.f;
+    if (t.vy0 && t.vx0) acc += load(t.y0, t.x0) * t.nw;
+    if (t.vy0 && t.vx1) acc += load(t.y0, t.x0 + 1) * t.ne;
+    if (t.vy1 && t.vx0) acc += load(t.y0 + 1, t.x0) * t.sw;
+    if (t.vy1 && t.vx1) acc += load(t.y0 + 1, t.x0 + 1) * t.se;
+    return acc;
+}
+
 __global__ void grid_sample_kernel(const float* __restrict__ in, int N, int C, int Hin, int Win, Strides4 is,
                                    const float* __restrict__ grid, int Hout, int Wout, int align_corners,
                                    float* __restrict__ out, Strides4 os) {
@@ -668,23 +706,27 @@ __global__ void grid_sample_kernel(const float* __restrict__ in, int N, int C, i
     int n = (int)(t / hw);
     int rem = (int)(t - n * hw);
     int r = rem / Wout, c = rem - r * Wout;
-    float2 g = __ldg(reinterpret_cast<const float2*>(grid) + t);
-    float ix = in_int_range(unnormalize(g.x, Win, align_corners)), iy = in_int_range(unnormalize(g.y, Hin, align_corners));
-    float fx = floorf(ix), fy = floorf(iy);
-    int x0 = (int)fx, y0 = (int)fy, x1 = x0 + 1, y1 = y0 + 1;
-    float nw = (fx + 1.f - ix) * (fy + 1.f - iy), ne = (ix - fx) * (fy + 1.f - iy);
-    float sw = (fx + 1.f - ix) * (iy - fy), se = (ix - fx) * (iy - fy);
-    bool vx0 = x0 >= 0 && x0 < Win, vx1 = x1 >= 0 && x1 < Win, vy0 = y0 >= 0 && y0 < Hin, vy1 = y1 >= 0 && y1 < Hin;
+    const BilinearTaps tap = bilinear_taps(__ldg(reinterpret_cast<const float2*>(grid) + t), Hin, Win, align_corners);
     const float* base = in + n * is.n;
     float* ob = out + n * os.n + r * os.h + c * os.w;
     for (int ch = 0; ch < C; ++ch) {
         const float* p = base + ch * is.c;
-        float acc = 0.f;
-        if (vy0 && vx0) acc += __ldg(p + y0 * is.h + x0 * is.w) * nw;
-        if (vy0 && vx1) acc += __ldg(p + y0 * is.h + x1 * is.w) * ne;
-        if (vy1 && vx0) acc += __ldg(p + y1 * is.h + x0 * is.w) * sw;
-        if (vy1 && vx1) acc += __ldg(p + y1 * is.h + x1 * is.w) * se;
-        ob[ch * os.c] = acc;
+        ob[ch * os.c] = bilinear_sum(tap, [&](int y, int x) { return __ldg(p + y * is.h + x * is.w); });
+    }
+}
+
+// train/generate_coarse_aligned_pair.ipynb cell 13 and ToPILImage in one pass: output pixel (r, c) of the h x w homography
+// grid of H (device memory), bilinear zero-padded sampling of ToTensor(src) (uint8 HWC / 255, preproc_one), x 255 truncated
+// to uint8.  The grid, the fp32 copy of the source and the fp32 sampled image are never stored.
+__global__ void __launch_bounds__(256) warp_sample_u8_kernel(const float* __restrict__ H, const unsigned char* __restrict__ src, int Hin,
+                                                             int Win, int h, int w, int align_corners, unsigned char* __restrict__ out) {
+    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)h * w) return;
+    int r = (int)(t / w), c = (int)(t - (long long)r * w);
+    const BilinearTaps tap = bilinear_taps(homography_grid_point(H, r, c, h, w), Hin, Win, align_corners);
+    for (int ch = 0; ch < 3; ++ch) {
+        float v = bilinear_sum(tap, [&](int y, int x) { return preproc_one(__ldg(src + ((long long)y * Win + x) * 3 + ch), ch, 0); });
+        out[t * 3 + ch] = (unsigned char)__float2uint_rz(__fmul_rn(v, 255.f));
     }
 }
 
@@ -1521,6 +1563,16 @@ extern "C" int rf_grid_sample(const float* in, int N, int C, int Hin, int Win, c
     Strides4 is{in_s_host[0], in_s_host[1], in_s_host[2], in_s_host[3]};
     Strides4 os{out_s_host[0], out_s_host[1], out_s_host[2], out_s_host[3]};
     grid_sample_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(in, N, C, Hin, Win, is, grid, Hout, Wout, align_corners, out, os);
+    RF_LAUNCHED();
+    return 0;
+}
+
+extern "C" int rf_warp_sample_u8(const float* H, const uint8_t* src, int Hin, int Win, int h, int w, int align_corners, uint8_t* out,
+                                 void* stream) {
+    RF_REQUIRE(Hin > 0 && Win > 0, "rf_warp_sample_u8: empty source");
+    long long total = (long long)h * w;
+    if (total <= 0) return 0;
+    warp_sample_u8_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(H, src, Hin, Win, h, w, align_corners, out);
     RF_LAUNCHED();
     return 0;
 }

@@ -1184,3 +1184,6 @@ def getFlow_all(flow, param, match, outH, outW, th=0.95, multiH=True, with_match
 
 # evalYFCC's pair from CUDA graphs (its kernel entries live with it, in yfcc_graph)
 from .yfcc_graph import GraphedYfccAligner, align_pair_yfcc_graph  # noqa: E402,F401
+
+# train/generate_coarse_aligned_pair.ipynb's pair (its kernel entry lives with it, in train_pairs)
+from .train_pairs import GraphedTrainPairAligner, TrainPairModel, align_train_pair  # noqa: E402,F401

@@ -10,6 +10,7 @@ that results written here are read by the reference's ``getResults.py`` and vice
   epe_hpatches                     : evaluation/evalHpatch/getResults.py:147-157,224-250
   alignment_error                  : evaluation/evalCorr/getResults.py:15-38
   epe_kitti                        : evaluation/evalKITTI/getResults.py:221-230
+  save_train_pair / write_train_pairs : train/generate_coarse_aligned_pair.ipynb's pairs in the layout data/dataloader.py:40-60 reads
 
 File IO and the sparse-keypoint lookups are host code as in the reference; the dense compositions run on the library's
 kernels (``pipeline.getFlow_all`` / ``getFlow_all_kitti``), the dense metrics are elementwise torch on the tensors' device.
@@ -337,3 +338,52 @@ def epe_kitti(flow, u, v, valid):
     val = torch.as_tensor(np.asarray(valid, dtype=np.float64), device=dev)
     error = ((upred - u_t) ** 2 + (vpred - v_t) ** 2) ** 0.5
     return (torch.sum(error * val) / torch.sum(val)).item()
+
+
+# --------------------------------------------------------------------------- training pairs (README §4.1)
+def save_train_pair(outDir, index, out):
+    """Write a kept pair of ``pipeline.align_train_pair`` as ``outDir/{index}_1.jpg`` (the resized source) and ``{index}_2.jpg``
+    (the target warped into its frame), with PIL's JPEG defaults: the two images ``ImageFolder`` (data/dataloader.py:43-60)
+    reads for ``index``."""
+    import PIL.Image as Image
+    for k, key in ((1, "I1"), (2, "I2")):
+        img = out[key]
+        img = img.cpu().numpy() if torch.is_tensor(img) else np.asarray(img, dtype=np.uint8)
+        Image.fromarray(img).save(os.path.join(outDir, "%d_%d.jpg" % (int(index), k)))
+
+
+def _load_rgb(I):
+    """A path (opened as the notebook opens it, ``Image.open(path).convert('RGB')``) or an image, as a uint8 (H, W, 3) array
+    or tensor."""
+    import PIL.Image as Image
+    if isinstance(I, (str, os.PathLike)):
+        return np.asarray(Image.open(I).convert("RGB"))
+    if isinstance(I, Image.Image):
+        return np.asarray(I.convert("RGB"))
+    return I
+
+
+def write_train_pairs(aligner, pairs, outDir, chunk=8):
+    """The notebook over a dataset: every (I1, I2) in ``pairs`` (paths or images) through ``aligner`` (a
+    ``GraphedTrainPairAligner``, a ``ConcurrentAligner`` of them, or any callable ``aligner(I1, I2)`` returning
+    ``align_train_pair``'s dict), and the kept pairs written by ``save_train_pair``.  ``ImageFolder`` counts the files
+    (``nbImg = len(listdir) // 2``) and reads indices 0 .. nbImg - 1, so kept pairs are numbered contiguously from 0 and
+    rejected ones leave no hole; ``outDir`` (created if missing) must hold nothing else.  Returns, per input pair, its
+    output index or None.  Reading and JPEG coding are host code; ``chunk`` pairs are queued at a time through a
+    ``ConcurrentAligner``."""
+    os.makedirs(outDir, exist_ok=True)
+    if os.listdir(outDir):
+        raise ValueError("write_train_pairs: %s is not empty (ImageFolder counts every file in it)" % outDir)
+    run = aligner.run if hasattr(aligner, "run") else (lambda ps: [aligner(a, b) for a, b in ps])
+    pairs = list(pairs)
+    index, n = [], 0
+    for s in range(0, len(pairs), chunk):
+        loaded = [(_load_rgb(a), _load_rgb(b)) for a, b in pairs[s:s + chunk]]
+        for out in run(loaded):
+            if out["kept"]:
+                save_train_pair(outDir, n, out)
+                index.append(n)
+                n += 1
+            else:
+                index.append(None)
+    return index
