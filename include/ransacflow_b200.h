@@ -307,6 +307,19 @@ int rf_grid_sample(const float* in, int N, int C, int Hin, int Win, const long l
  * the composition of the three and the quantisation).  H: 9 floats in DEVICE memory (a non-finite H samples nothing: zeros);
  * src [Hin][Win][3] uint8. */
 int rf_warp_sample_u8(const float* H, const uint8_t* src, int Hin, int Win, int h, int w, int align_corners, uint8_t* out, void* stream);
+/* train/validation.py:80,98-99 in one pass: out_nhwc [h][w][3] fp32 = F.grid_sample(ToTensor(src), F.affine_grid(theta, (1, 3, h, w)))
+ * (bilinear, zeros, align_corners=False), written where the FeatureExtractor's input row of the image goes.  theta: 6 floats
+ * (2 x 3, row-major) in DEVICE memory (a non-finite theta samples zeros); src [Hin][Win][3] uint8. */
+int rf_affine_sample_u8(const float* theta, const uint8_t* src, int Hin, int Win, int h, int w, float* out_nhwc, void* stream);
+/* train/validation.py:93-107 + alignmentError (:33-53) at the keypoints only, from flowDown8 = softmax_flow's (2, h8, w8) on the
+ * H x W target: kpts [capacity][4] int32 (xa, ya, xb, yb), *count (DEVICE) of them used; theta 6 floats in DEVICE memory; wA, hA
+ * the resized source's size.  counts [T + 1] uint64 (DEVICE) accumulate, per threshold, the keypoints whose fp64 distance is
+ * strictly below it, and the keypoints scored; an index outside torch's [-n, n) range sets *err = min(*err, pair).
+ * dist_out [capacity] fp64 and flow_out [capacity][4] fp32 (16-byte aligned: the clamped fine flow at (yb, xb), then the composed
+ * flow, i.e. the affine grid sampled there) are optional (NULL). */
+int rf_val_keypoints(const float* flowDown8, int h8, int w8, const float* theta, int H, int W, int wA, int hA, const int* kpts,
+                     const int* count, int capacity, int pair, const double* thresholds_host, int T, unsigned long long* counts,
+                     int* err, double* dist_out, float* flow_out, void* stream);
 /* F.interpolate(mode='bilinear', align_corners=False): NCHW [NC][h][w] -> [NC][H][W] */
 int rf_upsample_bilinear(const float* in, int NC, int h, int w, int H, int W, float* out, void* stream);
 /* PredFlowMask tail, evaluation/evalHpatch/evaluation.py:37-51 fused:

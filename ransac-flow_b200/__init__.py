@@ -14,3 +14,12 @@ from . import ops, outil, model, kornia_geometry, coarseAlignFeatMatch, pipeline
 from .coarseAlignFeatMatch import CoarseAlign, CoarseAlignA, CoarseAlignB, CoarseAlignC  # noqa: F401
 
 __version__ = "0.1.0"
+
+
+def __getattr__(name):
+    """``validation`` (train/validation.py on the device) is imported on first use, so that ``python -m
+    ransac_flow_b200.validation`` runs the module once, as ``__main__``, instead of after a package-level import of it."""
+    if name == "validation":
+        import importlib
+        return importlib.import_module(".validation", __name__)
+    raise AttributeError("module %r has no attribute %r" % (__name__, name))

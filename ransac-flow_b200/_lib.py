@@ -57,6 +57,8 @@ SIGNATURES = {
     "rf_warp_grid": (i32, [vp, i32, i32, i32, vp, vp]),
     "rf_grid_sample": (i32, [vp, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp, vp, vp]),
     "rf_warp_sample_u8": (i32, [vp, vp, i32, i32, i32, i32, i32, vp, vp]),
+    "rf_affine_sample_u8": (i32, [vp, vp, i32, i32, i32, i32, vp, vp]),
+    "rf_val_keypoints": (i32, [vp, i32, i32, vp, i32, i32, i32, i32, vp, vp, i32, i32, vp, i32, vp, vp, vp, vp, vp]),
     "rf_upsample_bilinear": (i32, [vp, i32, i32, i32, i32, i32, vp, vp]),
     "rf_compose_fine": (i32, [vp, vp, vp, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp]),
     "rf_compose_fine_ex": (i32, [vp, vp, vp, i32, i32, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp, vp]),

@@ -730,6 +730,35 @@ __global__ void __launch_bounds__(256) warp_sample_u8_kernel(const float* __rest
     }
 }
 
+// F.affine_grid(theta, (N, C, h, w), align_corners=False) at output pixel (r, c), theta 2 x 3 row-major.  The base coordinate
+// is ATen's linspace(-1, 1, n) * (n - 1) / n on the CUDA linspace: the product by n - 1, then the division by the scalar n,
+// which ATen's CUDA division performs as a product with the fp32 reciprocal 1 / n; n = 1 gives 0.  theta is applied as one
+// FMA chain (x, y, then the constant); torch runs that product as a cuBLAS bmm, so the grid equals torch's to a few ulps
+// of its largest term, not bit for bit.
+__device__ __forceinline__ float affine_base(int i, int n) {
+    if (n <= 1) return 0.f;
+    return __fmul_rn(__fmul_rn(lin11(i, n), (float)(n - 1)), __fdiv_rn(1.f, (float)n));
+}
+__device__ __forceinline__ float2 affine_grid_point(const float* __restrict__ theta, int r, int c, int h, int w) {
+    float x = affine_base(c, w), y = affine_base(r, h);
+    float px = __fadd_rn(__fmaf_rn(__ldg(theta + 1), y, __fmul_rn(__ldg(theta + 0), x)), __ldg(theta + 2));
+    float py = __fadd_rn(__fmaf_rn(__ldg(theta + 4), y, __fmul_rn(__ldg(theta + 3), x)), __ldg(theta + 5));
+    return make_float2(px, py);
+}
+
+// train/validation.py:80,98-99 in one pass: output pixel (r, c) of the h x w affine grid of theta (device memory), bilinear
+// zero-padded sampling (align_corners=False) of ToTensor(src) (uint8 HWC / 255, preproc_one), written as the fp32 NHWC row
+// the FeatureExtractor reads.  The grid and the fp32 copy of the source are never stored; a non-finite theta samples zeros.
+__global__ void __launch_bounds__(256) affine_sample_u8_kernel(const float* __restrict__ theta, const unsigned char* __restrict__ src,
+                                                               int Hin, int Win, int h, int w, float* __restrict__ out) {
+    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)h * w) return;
+    int r = (int)(t / w), c = (int)(t - (long long)r * w);
+    const BilinearTaps tap = bilinear_taps(affine_grid_point(theta, r, c, h, w), Hin, Win, 0);
+    for (int ch = 0; ch < 3; ++ch)
+        out[t * 3 + ch] = bilinear_sum(tap, [&](int y, int x) { return preproc_one(__ldg(src + ((long long)y * Win + x) * 3 + ch), ch, 0); });
+}
+
 // F.interpolate(bilinear, align_corners=False) source index / weights
 __device__ __forceinline__ void up_coord(int dst, int in_size, int out_size, int& i0, int& i1, float& l0, float& l1) {
     float scale = (float)in_size / (float)out_size;
@@ -760,6 +789,72 @@ __global__ void upsample_kernel(const float* __restrict__ in, int NC, int h, int
     int rem = (int)(t - nc * HW);
     int Y = rem / W, X = rem - Y * W;
     out[t] = up_sample(in + (long long)nc * h * w, h, w, H, W, Y, X);
+}
+
+// train/validation.py:93-107 and alignmentError (:33-53) at the annotated keypoints only.  Per keypoint (xa, ya, xb, yb):
+// torch's index rule on (yb, xb) in the H x W target (a negative index wraps once; anything else records the pair in *err);
+// F.upsample_bilinear (align_corners=True) of flowDown8 at that pixel with ATen's CUDA arithmetic (fp32 scale, (int) floor,
+// the h1p / w1p edge step, the lambda order of up_blend); + the grid of validation.py:93-95, a CPU torch.linspace, which
+// lin11 reproduces (ATen's AVX2 / AVX-512 CPU kernel contracts both branches into one FMA, as nvcc does here: the scalar
+// "default" build, which rounds twice, differs by an ulp in places); clamped to [-1, 1] with NaN kept; the
+// F.grid_sample (bilinear, zeros, align_corners=False) of the H x W affine grid of theta at that point, its four taps
+// recomputed; estim = (flow + 1) * 0.5 * (size - 1) in fp32 (wA, hA: the resized source); the distance to (xa, ya) in fp64;
+// counts[t] += (dist < thresholds[t]) and counts[T] += 1 over the block, one atomic per counter.
+#define RF_VAL_MAX_THRESHOLDS 16
+struct ValThresholds { double t[RF_VAL_MAX_THRESHOLDS]; int n; };
+
+__device__ __forceinline__ float clamp11_nan(float v) { return isnan(v) ? v : fminf(fmaxf(v, -1.f), 1.f); }
+
+__global__ void __launch_bounds__(256) val_keypoints_kernel(const float* __restrict__ flow8, int h8, int w8, const float* __restrict__ theta,
+                                                            int H, int W, int wA, int hA, const int* __restrict__ kpts,
+                                                            const int* __restrict__ count, int capacity, int pair,
+                                                            const __grid_constant__ ValThresholds th, unsigned long long* __restrict__ counts,
+                                                            int* __restrict__ err, double* __restrict__ dist_out, float* __restrict__ flow_out) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n = min(__ldg(count), capacity);
+    bool live = j < n;
+    double dist = 0.0;
+    if (live) {
+        const int xa = __ldg(kpts + 4 * j), ya = __ldg(kpts + 4 * j + 1);
+        int xb = __ldg(kpts + 4 * j + 2), yb = __ldg(kpts + 4 * j + 3);
+        if (yb < 0 && yb >= -H) yb += H;
+        if (xb < 0 && xb >= -W) xb += W;
+        if (yb < 0 || yb >= H || xb < 0 || xb >= W) {
+            atomicMin(err, pair);
+            live = false;
+            if (dist_out) dist_out[j] = __longlong_as_double(0x7ff8000000000000ll);
+        } else {
+            const float rh = H > 1 ? __fdiv_rn((float)(h8 - 1), (float)(H - 1)) : 0.f;
+            const float rw = W > 1 ? __fdiv_rn((float)(w8 - 1), (float)(W - 1)) : 0.f;
+            const float h1r = __fmul_rn(rh, (float)yb), w1r = __fmul_rn(rw, (float)xb);
+            const int h1 = (int)h1r, w1 = (int)w1r;
+            const int h1p = h1 < h8 - 1 ? 1 : 0, w1p = w1 < w8 - 1 ? 1 : 0;
+            const float h1l = h1r - (float)h1, w1l = w1r - (float)w1;
+            const float h0l = 1.f - h1l, w0l = 1.f - w1l;
+            const float* p0 = flow8 + (long long)h1 * w8 + w1;
+            const float* p1 = p0 + (long long)h8 * w8;
+            const long long dy = (long long)h1p * w8;
+            float fx = up_blend(__ldg(p0), __ldg(p0 + w1p), __ldg(p0 + dy), __ldg(p0 + dy + w1p), h0l, h1l, w0l, w1l);
+            float fy = up_blend(__ldg(p1), __ldg(p1 + w1p), __ldg(p1 + dy), __ldg(p1 + dy + w1p), h0l, h1l, w0l, w1l);
+            fx = clamp11_nan(__fadd_rn(fx, lin11(xb, W)));
+            fy = clamp11_nan(__fadd_rn(fy, lin11(yb, H)));
+            const BilinearTaps tap = bilinear_taps(make_float2(fx, fy), H, W, 0);
+            const float ox = bilinear_sum(tap, [&](int y, int x) { return affine_grid_point(theta, y, x, H, W).x; });
+            const float oy = bilinear_sum(tap, [&](int y, int x) { return affine_grid_point(theta, y, x, H, W).y; });
+            if (flow_out) reinterpret_cast<float4*>(flow_out)[j] = make_float4(fx, fy, ox, oy);
+            const float ex = __fmul_rn(__fmul_rn(__fadd_rn(ox, 1.f), 0.5f), (float)(wA - 1));
+            const float ey = __fmul_rn(__fmul_rn(__fadd_rn(oy, 1.f), 0.5f), (float)(hA - 1));
+            const double ddx = __dsub_rn((double)ex, (double)xa), ddy = __dsub_rn((double)ey, (double)ya);
+            dist = __dsqrt_rn(__dadd_rn(__dmul_rn(ddx, ddx), __dmul_rn(ddy, ddy)));
+            if (dist_out) dist_out[j] = dist;
+        }
+    }
+    for (int t = 0; t < th.n; ++t) {
+        const int c = __syncthreads_count(live && dist < th.t[t]);
+        if (threadIdx.x == 0 && c) atomicAdd(counts + t, (unsigned long long)c);
+    }
+    const int c = __syncthreads_count(live);
+    if (threadIdx.x == 0 && c) atomicAdd(counts + th.n, (unsigned long long)c);
 }
 
 // evaluation/evalHpatch/evaluation.py:37-51 (and evalCorr :50-55) in one pass over the full-res grid.  The coarse grid
@@ -1573,6 +1668,31 @@ extern "C" int rf_warp_sample_u8(const float* H, const uint8_t* src, int Hin, in
     long long total = (long long)h * w;
     if (total <= 0) return 0;
     warp_sample_u8_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(H, src, Hin, Win, h, w, align_corners, out);
+    RF_LAUNCHED();
+    return 0;
+}
+
+extern "C" int rf_affine_sample_u8(const float* theta, const uint8_t* src, int Hin, int Win, int h, int w, float* out_nhwc, void* stream) {
+    RF_REQUIRE(Hin > 0 && Win > 0, "rf_affine_sample_u8: empty source");
+    long long total = (long long)h * w;
+    if (total <= 0) return 0;
+    affine_sample_u8_kernel<<<blocks_for(total, 256), 256, 0, as_stream(stream)>>>(theta, src, Hin, Win, h, w, out_nhwc);
+    RF_LAUNCHED();
+    return 0;
+}
+
+extern "C" int rf_val_keypoints(const float* flowDown8, int h8, int w8, const float* theta, int H, int W, int wA, int hA, const int* kpts,
+                                const int* count, int capacity, int pair, const double* thresholds_host, int T, unsigned long long* counts,
+                                int* err, double* dist_out, float* flow_out, void* stream) {
+    RF_REQUIRE(h8 > 0 && w8 > 0 && H > 0 && W > 0, "rf_val_keypoints: empty flow or target");
+    RF_REQUIRE(T >= 1 && T <= RF_VAL_MAX_THRESHOLDS && thresholds_host, "rf_val_keypoints: 1..16 thresholds");
+    RF_REQUIRE(counts && err && count, "rf_val_keypoints: counts, error word and count are required");
+    if (capacity <= 0) return 0;
+    ValThresholds th{};
+    for (int t = 0; t < T; ++t) th.t[t] = thresholds_host[t];
+    th.n = T;
+    val_keypoints_kernel<<<blocks_for(capacity, 256), 256, 0, as_stream(stream)>>>(flowDown8, h8, w8, theta, H, W, wA, hA, kpts, count, capacity,
+                                                                                   pair, th, counts, err, dist_out, flow_out);
     RF_LAUNCHED();
     return 0;
 }

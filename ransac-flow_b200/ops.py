@@ -590,22 +590,29 @@ def fill_nearest_matched(flow, matched, want_index=False):
 _coeff_cache = {}
 
 
-def resample_coeffs(in_size, out_size, device, fn):
-    """PIL's 8bpc resampling tables (``fn``: rf_lanczos_coeffs_host or rf_bilinear_coeffs_host) as device tensors, cached."""
+def resample_coeffs(in_size, out_size, device, fn, non_blocking=False):
+    """PIL's 8bpc resampling tables (``fn``: rf_lanczos_coeffs_host or rf_bilinear_coeffs_host) as device tensors, cached.
+    ``non_blocking``: the tables go up from pinned memory on the current stream, without a host synchronisation.  Such
+    tables are ordered on that stream only, so they are cached for that stream alone: blocking callers and other streams
+    never see them."""
     key = (in_size, out_size, str(device), fn)
+    if non_blocking:
+        key += (torch.cuda.current_stream(device).cuda_stream,)
     if key not in _coeff_cache:
         ks = C.c_int(0)
         check(getattr(lib, fn)(in_size, out_size, None, None, 0, C.byref(ks)))
         bounds = np.zeros(2 * out_size, dtype=np.int32)
         kk = np.zeros(ks.value * out_size, dtype=np.int32)
         check(getattr(lib, fn)(in_size, out_size, bounds.ctypes.data_as(C.c_void_p), kk.ctypes.data_as(C.c_void_p), kk.size, C.byref(ks)))
-        _coeff_cache[key] = (torch.from_numpy(bounds).to(device), torch.from_numpy(kk).to(device), ks.value)
+        up = (lambda a: torch.from_numpy(a).pin_memory().to(device, non_blocking=True)) if non_blocking else (lambda a: torch.from_numpy(a).to(device))
+        _coeff_cache[key] = (up(bounds), up(kk), ks.value)
     return _coeff_cache[key]
 
 
-def resize_lanczos_u8(img, out_w, out_h):
-    """PIL ``Image.resize((out_w, out_h), LANCZOS)`` on a uint8 [H, W, 3] CUDA tensor (bit-exact)."""
-    return _resize_u8(img, out_w, out_h, "rf_lanczos_coeffs_host")
+def resize_lanczos_u8(img, out_w, out_h, non_blocking=False):
+    """PIL ``Image.resize((out_w, out_h), LANCZOS)`` on a uint8 [H, W, 3] CUDA tensor (bit-exact).  ``non_blocking``: see
+    ``resample_coeffs``."""
+    return _resize_u8(img, out_w, out_h, "rf_lanczos_coeffs_host", non_blocking)
 
 
 def resize_bilinear_u8(img, out_w, out_h):
@@ -613,18 +620,18 @@ def resize_bilinear_u8(img, out_w, out_h):
     return _resize_u8(img, out_w, out_h, "rf_bilinear_coeffs_host")
 
 
-def _resize_u8(img, out_w, out_h, fn):
+def _resize_u8(img, out_w, out_h, fn, non_blocking=False):
     """PIL's two-pass 8bpc resampling (horizontal, then vertical) with the tables ``fn`` builds."""
     need_cuda(img)
     H, W, ch = img.shape
     cur = img.contiguous()
     if out_w != W:
-        b, k, ks = resample_coeffs(W, out_w, img.device, fn)
+        b, k, ks = resample_coeffs(W, out_w, img.device, fn, non_blocking)
         nxt = torch.empty((H, out_w, ch), device=img.device, dtype=torch.uint8)
         check(lib.rf_resample_u8(ptr(cur), H, W, ch, 1, ptr(b), ptr(k), ks, out_w, ptr(nxt), stream()))
         cur, W = nxt, out_w
     if out_h != H:
-        b, k, ks = resample_coeffs(H, out_h, img.device, fn)
+        b, k, ks = resample_coeffs(H, out_h, img.device, fn, non_blocking)
         nxt = torch.empty((out_h, W, ch), device=img.device, dtype=torch.uint8)
         check(lib.rf_resample_u8(ptr(cur), H, W, ch, 0, ptr(b), ptr(k), ks, out_h, ptr(nxt), stream()))
         cur = nxt
