@@ -131,15 +131,25 @@ def _read_back(pair):
     return _to_host(pair.packed).copy(), None if pair.bg is None else _to_host(pair.bg).copy()
 
 
+def _hypothesis(coarseModel, network, fgMask, samples, featt, with_match21, feat_box=None):
+    """One hypothesis's device work on the pair ``coarseModel`` holds: ``getCoarse_device`` masked by ``fgMask`` (None: nothing
+    masked), the warp grid of its homography and ``PredFlowMask_device`` (``featt``: the target's cached fine features; None:
+    the target and the warped source as one two-image batch, the target's handed to ``feat_box``).  Nothing is read back.
+    Returns (H [9], nbInlier [1], status [1], nbMatch [1], flow12, match, flowDown8, matchDown8)."""
+    Itw, Ith = coarseModel.target_size
+    Hd, nb, _, status, cnt = coarseModel.getCoarse_device(fgMask, samples)
+    flowCoarse = ops.warp_grid(Hd.view(1, 3, 3), Ith, Itw)
+    flow12, match, f8, mboth = PredFlowMask_device(coarseModel.IsTensor, featt, flowCoarse, (Ith, Itw), network, with_match21,
+                                                   ItTensor=coarseModel.ItTensor, feat_box=feat_box)
+    return Hd, nb, status, cnt, flow12, match, f8, mboth
+
+
 def _single_device(coarseModel, network, Is, It, with_match21, samples=None):
     """Device part of the single-hypothesis path: everything queued on the current stream, nothing read back."""
     coarseModel.setPair(Is, It)
     Itw, Ith = coarseModel.target_size
-    Hd, nb, mask, status, cnt = coarseModel.getCoarse_device(None, samples)
-    flowCoarse = ops.warp_grid(Hd.view(1, 3, 3), Ith, Itw)
     # target and warped source through the FeatureExtractor as one two-image batch (bit-identical features)
-    flow12, match, f8, mboth = PredFlowMask_device(coarseModel.IsTensor, None, flowCoarse, (Ith, Itw), network, with_match21,
-                                                   ItTensor=coarseModel.ItTensor)
+    Hd, nb, status, cnt, flow12, match, f8, mboth = _hypothesis(coarseModel, network, None, samples, None, with_match21)
     packed = torch.cat([status.float(), cnt.float(), nb.float(), Hd, match.reshape(-1), f8.reshape(-1), mboth.reshape(-1)])
     return DevicePair(packed, flow12, (Ith, Itw), tuple(f8.shape))
 
@@ -381,16 +391,13 @@ def _hypothesis_loop(coarseModel, network, maxCoarse, maskRegionTh, with_match21
 def _hypothesis_step(coarseModel, network, k, Mask, alive, bg, featt, box, maskRegionTh, with_match21, samples, region64=False):
     """Hypothesis ``k`` of ``_hypothesis_loop``: getCoarse masked by (Mask, bg), the fine flow, the acceptance test and the mask
     update gated by the ``alive`` flag.  Returns (Mask, alive, the target's fine features, the record, flowDown8 shape)."""
-    Itw, Ith = coarseModel.target_size
     dev = coarseModel.ItTensor.device
     if bg is None:
         fgMask = (Mask > 0.5).float()                                # It_bg = 1 everywhere: (Mask + (1 - It_bg)) > 0.5
     else:
         fgMask = ((Mask + (1 - bg)) > 0.5).float()
-    Hd, nb, mask, status, cnt = coarseModel.getCoarse_device(fgMask if k > 0 or bg is not None else None, samples)
-    flowCoarse = ops.warp_grid(Hd.view(1, 3, 3), Ith, Itw)
-    flow12, match, f8, mboth = PredFlowMask_device(coarseModel.IsTensor, featt, flowCoarse, (Ith, Itw), network, with_match21,
-                                                   ItTensor=coarseModel.ItTensor, feat_box=box)
+    Hd, nb, status, cnt, _, match, f8, mboth = _hypothesis(coarseModel, network, fgMask if k > 0 or bg is not None else None,
+                                                           samples, featt, with_match21, box)
     if featt is None:
         featt = box["featt"]            # computed with the first hypothesis' warped source in one batch
     newreg = (match[0, 0] * (1 - fgMask)).mean()
@@ -404,12 +411,17 @@ def _hypothesis_step(coarseModel, network, k, Mask, alive, bg, featt, box, maskR
     # (evaluation.py:235 masks from the first hypothesis on; without a background the first mask is all zeros)
     matchFine = match[0, 0] if (k == 0 and bg is None) else match[0, 0] * (1 - fgMask)
     Mask = torch.where(alive, ((Mask + matchFine) >= 1.0).float(), Mask)
-    rec = torch.cat([alive.float().reshape(1), status.float(), cnt.float(), nb.float(), Hd, f8.reshape(-1), mboth.reshape(-1)])
-    return Mask, alive, featt, rec, tuple(f8.shape)
+    return Mask, alive, featt, _record(alive, status, cnt, nb, Hd, f8, mboth), tuple(f8.shape)
 
 
-# the per-hypothesis record of the device loops (multi-hypothesis, KITTI, YFCC): [alive, status, nbMatch, nbInlier, H(9), payload]
+# the per-hypothesis record of the hypothesis loops (multi-hypothesis, KITTI, YFCC, align_pair_device):
+# [alive, status, nbMatch, nbInlier, H(9), payload]
 _ALIVE, _STATUS, _NBMATCH, _NBINLIER, _H, _PAYLOAD = 0, 1, 2, 3, slice(4, 13), 13
+
+
+def _record(alive, status, cnt, nb, Hd, *payload):
+    """One hypothesis's record as a flat float32 CUDA tensor; ``payload``: the device tensors after H, each flattened."""
+    return torch.cat([alive.float().reshape(1), status.float(), cnt.float(), nb.float(), Hd] + [p.reshape(-1) for p in payload])
 
 
 def _accepted(host, nhyp):
@@ -565,6 +577,14 @@ def align_pair(coarseModel, network, Is, It, maxCoarse=0, maskRegionTh=0.01, wit
     Itw, Ith = coarseModel.target_size
     if It_bg is None:
         It_bg = np.ones((Ith, Itw), dtype=np.float32)
+    return _host_hypotheses(coarseModel.getCoarse, coarseModel, network, It_bg, maxCoarse, maskRegionTh, with_match21)
+
+
+def _host_hypotheses(getCoarse, coarseModel, network, bg, maxCoarse, maskRegionTh, with_match21):
+    """The host-steered hypothesis loop of evaluation/evalHpatch/evaluation.py:211-243 (evalYFCC/evaluation.py:214-243) on the
+    target ``coarseModel`` holds, in numpy as the scripts write it.  ``getCoarse(fgMask)``: the homography, or None where the
+    reference's ``getCoarse`` returns None; ``bg``: the numpy (h, w) background map of the target (1 = kept)."""
+    Ith, Itw = bg.shape
     featt = fine_features(network["netFeatCoarse"], coarseModel.ItTensor)
     grid = torch.empty((1, Ith, Itw, 2), device="meta")                    # size carrier only
     warper = HomographyWarper(Ith, Itw)
@@ -572,12 +592,11 @@ def align_pair(coarseModel, network, Is, It, maxCoarse=0, maskRegionTh=0.01, wit
     Hs, flows8, matches8, flows, matches = [], [], [], [], []
     nbCoarse = 0
     while nbCoarse <= maxCoarse:
-        fgMask = ((Mask + (1 - It_bg)) > 0.5).astype(np.float32)
-        bestPara = coarseModel.getCoarse(fgMask)
+        fgMask = ((Mask + (1 - bg)) > 0.5).astype(np.float32)
+        bestPara = getCoarse(fgMask)
         if bestPara is None:
             break
-        bestParaT = torch.from_numpy(bestPara).unsqueeze(0).cuda()
-        flowCoarse = warper.warp_grid(bestParaT)
+        flowCoarse = warper.warp_grid(torch.from_numpy(bestPara).unsqueeze(0).cuda())
         flowFine, matchFine, f8, m8 = PredFlowMask(coarseModel.IsTensor, featt, flowCoarse, grid, network, with_match21)
         if (matchFine * (1 - fgMask)).mean() > maskRegionTh or nbCoarse == 0:
             Hs.append(bestPara[None])
@@ -586,8 +605,8 @@ def align_pair(coarseModel, network, Is, It, maxCoarse=0, maskRegionTh=0.01, wit
             flows.append(flowFine)
             matches.append(matchFine)
             nbCoarse += 1
-            matchFine = matchFine if len(matches8) == 0 else matchFine * (1 - fgMask)
-            Mask = ((Mask + matchFine) >= 1.0).astype(np.float32)
+            # evaluation.py:235 tests len(...) == 0 after the append: the new matchability is always masked
+            Mask = ((Mask + matchFine * (1 - fgMask)) >= 1.0).astype(np.float32)
         else:
             break
     cat = lambda l: np.concatenate(l, axis=0) if l else np.zeros((0,))
@@ -614,7 +633,8 @@ def _hypotheses_device(coarseModel, network, maxCoarse, maskRegionTh, with_match
     bg = torch.ones((Ith, Itw), device=dev) if It_bg is None else torch.as_tensor(It_bg, dtype=torch.float32, device=dev)
     featt = fine_features(network["netFeatCoarse"], coarseModel.ItTensor)
     Mask = torch.zeros((Ith, Itw), device=dev)
-    acc = []
+    accepted = torch.ones(1, device=dev)         # the alive flag of every record kept: the host accepted it
+    recs, flows, shapes = [], [], [None] * 3
     nbCoarse = ncall = 0
     gen = None
     if rewind_too_few and samples is None:
@@ -622,15 +642,15 @@ def _hypotheses_device(coarseModel, network, maxCoarse, maskRegionTh, with_match
     while nbCoarse <= maxCoarse:
         fgMask = ((Mask + (1 - bg)) > 0.5).float()
         state = gen.get_state() if gen is not None else None
-        Hd, nb, mask, status, cnt = coarseModel.getCoarse_device(fgMask if nbCoarse > 0 or It_bg is not None else None,
-                                                                 None if samples is None else samples[ncall])
-        ncall += 1
         # the fine stage is queued before the status is known (no host round trip between RANSAC and the networks); a failed
         # RANSAC leaves H = 0, whose warp grid is NaN: harmless (the results are dropped below) and finite work
-        flowCoarse = ops.warp_grid(Hd.view(1, 3, 3), Ith, Itw)
-        flow12, match, f8, mboth = PredFlowMask_device(coarseModel.IsTensor, featt, flowCoarse, (Ith, Itw), network, with_match21)
+        Hd, nb, status, cnt, flow12, match, f8, mboth = _hypothesis(coarseModel, network,
+                                                                    fgMask if nbCoarse > 0 or It_bg is not None else None,
+                                                                    None if samples is None else samples[ncall], featt, with_match21)
+        ncall += 1
         newreg = (match[0, 0] * (1 - fgMask)).mean()
-        ctl = _to_host(torch.cat([status.float(), newreg.reshape(1), cnt.float()])).copy()        # 12 bytes per hypothesis
+        status, cnt = status.float(), cnt.float()
+        ctl = _to_host(torch.cat([status, newreg.reshape(1), cnt])).copy()                         # 12 bytes per hypothesis
         st = int(ctl[0])
         if st == 2:
             raise TypeError("'NoneType' object is not subscriptable")     # utils/outil.py:162
@@ -639,7 +659,9 @@ def _hypotheses_device(coarseModel, network, maxCoarse, maskRegionTh, with_match
         if st != 0:
             break                                                          # bestPara is None (evaluation.py:215-216)
         if float(ctl[1]) > maskRegionTh or nbCoarse == 0:
-            acc.append((Hd, f8, mboth, flow12, match, int(ctl[2])))
+            recs.append(_record(accepted, status, cnt, nb, Hd, f8, mboth, match))
+            flows.append(flow12)
+            shapes = [tuple(f8.shape), (1, 2) + tuple(f8.shape[2:]), (1, Ith, Itw)]
             # evaluation.py:235 tests len(...) == 0 after the append: always masked (a no-op on the first hypothesis unless
             # a background mask is given)
             matchFine = match[0, 0] * (1 - fgMask)
@@ -647,17 +669,9 @@ def _hypotheses_device(coarseModel, network, maxCoarse, maskRegionTh, with_match
             Mask = ((Mask + matchFine) >= 1.0).float()
         else:
             break
-    if not acc:
-        return dict(H=np.zeros((0,)), flowDown8=np.zeros((0,)), matchDown8=np.zeros((0,)), flow12=[], match=[], nbMatch=[])
-    packed = torch.cat([torch.cat([a[0], a[1].reshape(-1), a[2].reshape(-1), a[4].reshape(-1)]) for a in acc])
-    host = _to_host(packed).copy().reshape(len(acc), -1)
-    n8 = acc[0][1].numel()
-    f8shape = tuple(acc[0][1].shape)
-    return dict(H=host[:, :9].reshape(-1, 3, 3).astype(np.float32),
-                flowDown8=host[:, 9:9 + n8].reshape((len(acc),) + f8shape[1:]),
-                matchDown8=host[:, 9 + n8:9 + 2 * n8].reshape(len(acc), 2, f8shape[2], f8shape[3]),
-                flow12=[a[3] for a in acc], match=[host[i, 9 + 2 * n8:].reshape(Ith, Itw) for i in range(len(acc))],
-                nbMatch=[a[5] for a in acc])
+    rows = _to_host(torch.cat(recs)).copy().reshape(len(recs), -1) if recs else np.zeros((0, _PAYLOAD), dtype=np.float32)
+    H, flowDown8, matchDown8, match = _split(rows, shapes)
+    return dict(H=H, flowDown8=flowDown8, matchDown8=matchDown8, flow12=flows, match=list(match), nbMatch=_counts(rows)["nbMatch"])
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -735,14 +749,8 @@ def _rotation_search(c, It_bg, samples):
     bgs, found = [], []
     for k in range(4):
         c._select_target(k)
-        bg = yfcc_background(It_bg, k, c.rotated_target_size(k))
+        bg, Mt = _rotation_mask(It_bg, k, c.rotated_target_size(k))
         bgs.append(bg)
-        if It_bg is None:
-            Mt = None
-        elif torch.is_tensor(bg):
-            Mt = ((1 - bg) > 0.5).float()
-        else:
-            Mt = ((1 - bg) > 0.5).astype(np.float32)
         m1, m2, _, cnt = c._match_device(Mt)
         found.append((m1, m2, cnt))
     counts = _to_host(torch.cat([f[2] for f in found])).copy()               # the one read the draw decision needs
@@ -756,7 +764,17 @@ def _rotation_search(c, It_bg, samples):
     nbInlierRot = rotation_scores(ran, res[:, 0], res[:, 1])
     best = int(np.argmax(nbInlierRot))                                          # np.argmax: the first maximum wins
     c._select_target(best)
-    return best, nbInlierRot, (bgs[best] if It_bg is not None else None), len(ran)
+    return best, nbInlierRot, bgs[best], len(ran)
+
+
+def _rotation_mask(It_bg, k, size):
+    """Rotation ``k``'s (background map, match mask ``Mt``) in the rotation search (evaluation.py:193-200): ``yfcc_background``
+    and the cells it masks, on the device when ``It_bg`` is a CUDA tensor; (None, None) without ``It_bg``."""
+    if It_bg is None:
+        return None, None
+    bg = yfcc_background(It_bg, k, size)
+    masked = (1 - bg) > 0.5
+    return bg, masked.float() if torch.is_tensor(bg) else masked.astype(np.float32)
 
 
 def align_pair_yfcc_host(coarseModel, network, Is, It, maxCoarse=10, maskRegionTh=0.01, It_bg=None):
@@ -776,34 +794,10 @@ def align_pair_yfcc_host(coarseModel, network, Is, It, maxCoarse=10, maskRegionT
             nbInlier.append(0 if bestPara is None else int(np.sum(InlierMask)))
         best = int(np.argmax(nbInlier))
         c.setTarget(ItList[best])
-        Itw, Ith = c.It.size
-        bg = yfcc_background(It_bg, best, (Itw, Ith))
-        featt = fine_features(network["netFeatCoarse"], c.ItTensor)
-        grid = torch.empty((1, Ith, Itw, 2), device="meta")                     # size carrier only
-        warper = HomographyWarper(Ith, Itw)
-        Mask = np.zeros((Ith, Itw), dtype=np.float32)
-        Hs, flows8, matches8, flows, matches = [], [], [], [], []
-        nbCoarse = 0
-        while nbCoarse <= maxCoarse:
-            fgMask = ((Mask + (1 - bg)) > 0.5).astype(np.float32)
-            bestPara, _ = c.getCoarse(fgMask)
-            if bestPara is None:
-                break
-            flowCoarse = warper.warp_grid(torch.from_numpy(bestPara).unsqueeze(0).cuda())
-            flowFine, matchFine, f8, m8 = PredFlowMask(c.IsTensor, featt, flowCoarse, grid, network, with_match21=True)
-            if (matchFine * (1 - fgMask)).mean() > maskRegionTh or nbCoarse == 0:
-                Hs.append(bestPara[None])
-                flows8.append(f8)
-                matches8.append(m8)
-                flows.append(flowFine)
-                matches.append(matchFine)
-                nbCoarse += 1
-                Mask = ((Mask + matchFine * (1 - fgMask)) >= 1.0).astype(np.float32)
-            else:
-                break
-    cat = lambda l: np.concatenate(l, axis=0) if l else np.zeros((0,))
-    return dict(H=cat(Hs), flowDown8=cat(flows8), matchDown8=cat(matches8), flow12=flows, match=matches, angle=YFCC_ANGLES[best],
-                nbInlierRot=nbInlier, It_bg=bg.astype(bool))
+        bg = yfcc_background(It_bg, best, c.It.size)
+        out = _host_hypotheses(lambda fgMask: c.getCoarse(fgMask)[0], c, network, bg, maxCoarse, maskRegionTh, True)
+    out.update(angle=YFCC_ANGLES[best], nbInlierRot=nbInlier, It_bg=bg.astype(bool))
+    return out
 
 
 def align2images(coarseModel, network, img1, img2, align_corners=False):
@@ -860,6 +854,29 @@ def PredFlowMask_kitti(IsSample, ItSample, flowCoarse, grid, network):
     return flow12, match[0, 0].cpu().numpy(), f8, m8
 
 
+def _kitti_levels(network, Hd, tensor_s, tensor_d2, tensor_resize, size_org, cc_th, boxes=(None, None)):
+    """One hypothesis's two fine levels (evaluation/evalKITTI/evaluation.py:283-311): the d2 level on the homography's grid at
+    ``tensor_d2``'s size, its flow composed onto the grid of ``tensor_resize`` (:291-294), the org level on that grid at the
+    original ``size_org`` = (h, w), and ``remove_small_cc`` on its matchability (:311).  ``Hd``: the homography (9 floats);
+    ``boxes``: per level, a dict that caches the target's fine features for the next hypotheses (None: the target's features
+    are computed every time).  Returns (flow_d2, flow (1,H,W,2), match (1,1,H,W), flowDown8, matchDown8) CUDA tensors."""
+    size_d2, (h_r, w_r) = tuple(tensor_d2.shape[2:]), tensor_resize.shape[2:]
+    box_d2, box_r = boxes
+    featt = lambda box: None if box is None else box.get("featt")
+    bp = Hd.view(1, 3, 3)
+    homography_d2 = ops.warp_grid(bp, *size_d2)
+    homography_resize = ops.warp_grid(bp, h_r, w_r)
+    IsSample_d2 = ops.grid_sample(tensor_s, homography_d2)
+    _, _, flowFine_d2, _ = PredFlowMask_kitti_device(IsSample_d2, tensor_d2, homography_d2, size_d2, network,
+                                                     featt=featt(box_d2), feat_box=box_d2)
+    flowCoarse, _, _ = ops.compose_fine(flowFine_d2, None, None, homography_resize, clamp=True, want_match=False)
+    IsSample = ops.grid_sample(tensor_s, flowCoarse)
+    flowFine_org, match_org, f8, m8 = PredFlowMask_kitti_device(IsSample, tensor_resize, flowCoarse, size_org, network,
+                                                                featt=featt(box_r), feat_box=box_r)
+    ops.remove_small_cc(match_org, 0.99, cc_th)
+    return flowFine_d2, flowFine_org, match_org, f8, m8
+
+
 def remove_small_cc(matchFine, match_th, cc_th):
     """evaluation/evalKITTI/evaluation.py:85-100 for a numpy (H, W) map, on the device (connected components by union-find)."""
     m = torch.from_numpy(np.ascontiguousarray(matchFine, dtype=np.float32)).cuda()
@@ -883,8 +900,7 @@ def align_pair_kitti(coarseModel, network, Is, It, fineSize=650, cc_th=0.01, mas
     It_d2 = outil.resizeImg(It, strideNet, fineSize // 2)
     w_org, h_org = It.size
     tensor_s = to_t(Is)
-    (w_r, h_r), tensor_resize = It_resize.size, to_t(It_resize)
-    (w_d2, h_d2), tensor_d2 = It_d2.size, to_t(It_d2)
+    tensor_resize, tensor_d2 = to_t(It_resize), to_t(It_d2)
     coarseModel.setPair(Is, It)
     given = It_bg is not None
     if given:                    # :248 (the reference's It_bg_tensor at the d2 size, :247, is never used)
@@ -900,15 +916,8 @@ def align_pair_kitti(coarseModel, network, Is, It, fineSize=650, cc_th=0.01, mas
         if bestPara is None:
             break
         with torch.no_grad():
-            bp = torch.from_numpy(bestPara).unsqueeze(0).cuda()
-            homography_d2 = ops.warp_grid(bp, h_d2, w_d2)
-            homography_resize = ops.warp_grid(bp, h_r, w_r)
-            IsSample_d2 = ops.grid_sample(tensor_s, homography_d2)
-            _, _, flowFine_d2, _ = PredFlowMask_kitti_device(IsSample_d2, tensor_d2, homography_d2, (h_d2, w_d2), network)
-            flowCoarse, _, _ = ops.compose_fine(flowFine_d2, None, None, homography_resize, clamp=True, want_match=False)     # :291-294
-            IsSample = ops.grid_sample(tensor_s, flowCoarse)
-            flowFine_org, match_org, f8, m8 = PredFlowMask_kitti_device(IsSample, tensor_resize, flowCoarse, (h_org, w_org), network)
-            ops.remove_small_cc(match_org, 0.99, cc_th)                                                                        # :311
+            flowFine_d2, flowFine_org, match_org, f8, m8 = _kitti_levels(network, torch.from_numpy(bestPara).cuda(), tensor_s,
+                                                                         tensor_d2, tensor_resize, (h_org, w_org), cc_th)
             matchFine = match_org[0, 0].cpu().numpy()
         if ((matchFine > 0.9999) * (1 - fgMask)).mean() > maskRegionTh or nbCoarse == 0:
             Hs.append(bestPara[None])
@@ -975,9 +984,9 @@ def _kitti_device(coarseModel, network, Is_u8, It_u8, fineSize, cc_th, maskRegio
         acceptance test and mask update (:316-326) into a device ``alive`` flag.  Hypotheses after the first dead one are
         computed but dropped by the host when it unpacks.
     ``Is_u8`` / ``It_u8``: uint8 (H, W, 3) CUDA images.  ``segNet``: the background of :245-250 is segNet's map of the target,
-    byte-scaled to the original size (``ops.imresize_mask``).  Returns (packed records, per-hypothesis (flow (1,H,W,2),
-    match (H,W)) CUDA maps, (h_org, w_org), (flow_d2 shape, flow shape)[, the uint8 (h_org, w_org) background map]), the
-    fields of a ``DevicePair`` in order; one record per hypothesis: [alive, status, nbMatch, nbInlier, H(9), Finetune_D2,
+    byte-scaled to the original size (``ops.imresize_mask``).  Returns a ``DevicePair``: the packed records, per-hypothesis
+    (flow (1,H,W,2), match (H,W)) CUDA maps, (h_org, w_org), (flow_d2 shape, flow shape) and, with ``segNet``, the uint8
+    (h_org, w_org) background map; one record per hypothesis: [alive, status, nbMatch, nbInlier, H(9), Finetune_D2,
     Finetune_Mask, Finetune]."""
     with torch.no_grad():
         h_org, w_org = int(It_u8.shape[0]), int(It_u8.shape[1])
@@ -1001,26 +1010,15 @@ def _kitti_device(coarseModel, network, Is_u8, It_u8, fineSize, cc_th, maskRegio
         recs, maps, shapes = [], [], None
         for k in range(maxH):
             Hd, nb, _, status, cnt = coarseModel.getCoarse_device(fgMask, None if samples is None else samples[k])
-            bp = Hd.view(1, 3, 3)
-            homography_d2 = ops.warp_grid(bp, h_d2, w_d2)
-            homography_resize = ops.warp_grid(bp, h_r, w_r)
-            IsSample_d2 = ops.grid_sample(tensor_s, homography_d2)
-            _, _, flowFine_d2, _ = PredFlowMask_kitti_device(IsSample_d2, tensor_d2, homography_d2, (h_d2, w_d2), network,
-                                                             featt=box_d2.get("featt"), feat_box=box_d2)
-            flowCoarse, _, _ = ops.compose_fine(flowFine_d2, None, None, homography_resize, clamp=True, want_match=False)
-            IsSample = ops.grid_sample(tensor_s, flowCoarse)
-            flowFine_org, match_org, f8, m8 = PredFlowMask_kitti_device(IsSample, tensor_resize, flowCoarse, (h_org, w_org), network,
-                                                                        featt=box_r.get("featt"), feat_box=box_r)
-            ops.remove_small_cc(match_org, 0.99, cc_th)
+            flowFine_d2, flowFine_org, match_org, f8, m8 = _kitti_levels(network, Hd, tensor_s, tensor_d2, tensor_resize,
+                                                                         (h_org, w_org), cc_th, (box_d2, box_r))
             match = match_org.view(h_org, w_org)
             rec = ops.kitti_region_step(match, Mask, bg, fgMask, status, alive, k == 0, cmin)
-            recs.append(torch.cat([rec[:1].float(), status.float(), cnt.float(), nb.float(), Hd, flowFine_d2.reshape(-1),
-                                   m8.reshape(-1), f8.reshape(-1)]))
+            recs.append(_record(rec[:1], status, cnt, nb, Hd, flowFine_d2, m8, f8))
             maps.append((flowFine_org, match))
             shapes = (tuple(flowFine_d2.shape), tuple(f8.shape))
         packed = torch.cat(recs)
-    out = (packed, maps, (h_org, w_org), shapes)
-    return out + (bg.to(torch.uint8),) if segNet else out
+    return DevicePair(packed, maps, (h_org, w_org), shapes, bg.to(torch.uint8) if segNet else None)
 
 
 def _unpack_kitti(host, maps, size, shapes, maxH, bg=None):
@@ -1052,8 +1050,8 @@ def align_pair_kitti_graph(coarseModel, network, Is, It, fineSize=650, cc_th=0.0
     if maxH is None or int(maxH) < 1:
         raise ValueError("align_pair_kitti_graph: maxH must be a positive hypothesis cap")
     maxH = int(maxH)
-    pair = DevicePair(*_kitti_device(coarseModel, network, _as_device_u8(coarseModel, Is), _as_device_u8(coarseModel, It), fineSize,
-                                     cc_th, maskRegionTh, maxH, segNet, samples))
+    pair = _kitti_device(coarseModel, network, _as_device_u8(coarseModel, Is), _as_device_u8(coarseModel, It), fineSize, cc_th,
+                         maskRegionTh, maxH, segNet, samples)
     host, bg = _read_back(pair)
     return _unpack_kitti(host, pair.maps, pair.size, pair.shapes, maxH, bg)
 
@@ -1074,11 +1072,49 @@ class GraphedKittiAligner(GraphedAligner):
         self.fineSize, self.cc_th, self.maskRegionTh, self.maxH, self.segNet = fineSize, cc_th, maskRegionTh, int(maxH), bool(segNet)
 
     def _device(self, s_in, t_in):
-        return DevicePair(*_kitti_device(self.coarse, self.net, s_in, t_in, self.fineSize, self.cc_th, self.maskRegionTh, self.maxH,
-                                         self.segNet))
+        return _kitti_device(self.coarse, self.net, s_in, t_in, self.fineSize, self.cc_th, self.maskRegionTh, self.maxH, self.segNet)
 
     def _unpack(self, host, bg, maps, size, shapes):
         return _unpack_kitti(host, maps, size, shapes, self.maxH, bg)
+
+
+def _compose_all(flow, param, match, outH, outW, with_match21=True, flowd2=None):
+    """The per-hypothesis composition of the getResults scripts: flow (nH,2,h8,w8) 'Finetune', param (nH,3,3), match
+    (nH,2,h8,w8) -> (f (nH,outH,outW,2) clamped to [-1, 1], m (nH,1,outH,outW)), CUDA.  Each hypothesis' flow is composed by
+    the fused kernel onto its homography's grid (``flowd2``, KITTI's 'Finetune_D2': onto that flow's composition with the
+    grid, evalKITTI/getResults.py:104-107); its matchability is ``match12 [* grid_sample(match21) (with_match21)] * inside``."""
+    flow = torch.as_tensor(flow, dtype=torch.float32).cuda()
+    param = torch.as_tensor(param, dtype=torch.float32).cuda()
+    match = torch.as_tensor(match, dtype=torch.float32).cuda()
+    if flowd2 is not None:
+        flowd2 = torch.as_tensor(flowd2, dtype=torch.float32).cuda()
+    coarse = ops.warp_grid(param, outH, outW)
+    fl, ms = [], []
+    for i in range(flow.shape[0]):
+        grid = coarse[i:i + 1]
+        if flowd2 is not None:
+            grid, _, _ = ops.compose_fine(flowd2[i:i + 1], None, None, grid, clamp=True, want_match=False)
+        f12, m, _ = ops.compose_fine(flow[i:i + 1], match[i:i + 1, 0:1], match[i:i + 1, 1:2] if with_match21 else None, grid,
+                                     clamp=True)
+        fl.append(f12)
+        ms.append(m)
+    return torch.clamp(torch.cat(fl, dim=0), min=-1, max=1), torch.cat(ms, dim=0)
+
+
+def _merge(f, m, th, multiH, with_match):
+    """``merge_first_wins``; without ``with_match`` the matchabilities are not merged and matchGlobal is None."""
+    flowGlobal = f[:1].clone()
+    matchGlobal = m[:1].clone() if with_match else None
+    mb = m[:1] >= th
+    if multiH:
+        for i in range(1, len(m)):
+            tmp = (m.narrow(0, i, 1) >= th) * (~mb)
+            if with_match:
+                matchGlobal[tmp] = m.narrow(0, i, 1)[tmp]
+            mb = mb + tmp
+            tmp = tmp.expand_as(flowGlobal)
+            flowGlobal[tmp] = f.narrow(0, i, 1)[tmp]
+    return flowGlobal, matchGlobal, mb
 
 
 def getFlow_all_kitti(param, flowd2, flow, match, outH, outW, th=1.0, cc_th=0.01, multiH=True, interpolate=False):
@@ -1087,27 +1123,9 @@ def getFlow_all_kitti(param, flowd2, flow, match, outH, outW, th=1.0, cc_th=0.01
     map), both CUDA.  The two levels are composed with the fused kernel, small connected components are removed on the
     device, the first-hypothesis-wins merge is elementwise torch.  ``interpolate``: the EDT hole filling of :87-93
     (``ops.fill_nearest_matched``: exact nearest matched pixel; between equidistant ones the choice may differ from scipy's)."""
-    param = torch.as_tensor(param, dtype=torch.float32).cuda()
-    flowd2 = torch.as_tensor(flowd2, dtype=torch.float32).cuda()
-    flow = torch.as_tensor(flow, dtype=torch.float32).cuda()
-    match = torch.as_tensor(match, dtype=torch.float32).cuda()
-    homography_org = ops.warp_grid(param, outH, outW)
-    fl, ms = [], []
-    for i in range(flow.shape[0]):
-        fd2, _, _ = ops.compose_fine(flowd2[i:i + 1], None, None, homography_org[i:i + 1], clamp=True, want_match=False)     # :104-107
-        f12, m, _ = ops.compose_fine(flow[i:i + 1], match[i:i + 1, 0:1], match[i:i + 1, 1:2], fd2, clamp=True)              # :110-123
-        fl.append(f12)
-        ms.append(m)
-    m = ops.remove_small_cc(torch.cat(ms, dim=0).contiguous(), 0.99, cc_th).permute(0, 2, 3, 1)
-    f = torch.clamp(torch.cat(fl, dim=0), min=-1, max=1)
-    flowGlobal = f[:1].clone()
-    mb = m[:1] >= th
-    if multiH:
-        for i in range(1, len(m)):
-            tmp = (m.narrow(0, i, 1) >= th) * (~mb)
-            mb = mb + tmp
-            tmp = tmp.expand_as(flowGlobal)
-            flowGlobal[tmp] = f.narrow(0, i, 1)[tmp]
+    f, m = _compose_all(flow, param, match, outH, outW, flowd2=flowd2)
+    m = ops.remove_small_cc(m, 0.99, cc_th).permute(0, 2, 3, 1)
+    flowGlobal, _, mb = _merge(f, m, th, multiH, False)
     if interpolate:
         flowGlobal = ops.fill_nearest_matched(flowGlobal, mb)
     return flowGlobal, mb
@@ -1117,16 +1135,7 @@ def merge_first_wins(f, m, th, multiH=True):
     """The first-hypothesis-wins merge every getResults script ends with (evaluation/evalCorr/getResults.py:121-134):
     f (nH,H,W,2) clamped flows, m (nH,H,W,1) matchabilities -> (flowGlobal (1,H,W,2), matchGlobal (1,H,W,1), binary map).
     Elementwise torch on the tensors' device."""
-    flowGlobal, matchGlobal = f[:1].clone(), m[:1].clone()
-    mb = m[:1] >= th
-    if multiH:
-        for i in range(1, len(m)):
-            tmp = (m.narrow(0, i, 1) >= th) * (~mb)
-            matchGlobal[tmp] = m.narrow(0, i, 1)[tmp]
-            mb = mb + tmp
-            tmp = tmp.expand_as(flowGlobal)
-            flowGlobal[tmp] = f.narrow(0, i, 1)[tmp]
-    return flowGlobal, matchGlobal, mb
+    return _merge(f, m, th, multiH, True)
 
 
 def getFlow_corr(flow, param, match, th=0.95, multiH=True):
@@ -1140,46 +1149,18 @@ def getFlow_corr(flow, param, match, th=0.95, multiH=True):
 def getFlow_corr_binary(flow, param, match, th=0.95, multiH=True):
     """``getFlow_corr`` plus the merge's binary map (1,8h8,8w8,1) bool, which evalYFCC's ``_getFlow`` returns instead of the
     matchability (evalYFCC/getResults.py:178-187)."""
-    flow = torch.as_tensor(flow, dtype=torch.float32).cuda()
-    param = torch.as_tensor(param, dtype=torch.float32).cuda()
-    match = torch.as_tensor(match, dtype=torch.float32).cuda()
-    H, W = int(flow.shape[2]) * 8, int(flow.shape[3]) * 8
-    coarse = ops.warp_grid(param, H, W)
-    fl, ms = [], []
-    for i in range(flow.shape[0]):
-        f12, m, _ = ops.compose_fine(flow[i:i + 1], match[i:i + 1, 0:1], match[i:i + 1, 1:2], coarse[i:i + 1], clamp=True)
-        fl.append(f12)
-        ms.append(m)
-    f = torch.clamp(torch.cat(fl, dim=0), min=-1, max=1)
-    m = torch.cat(ms, dim=0).permute(0, 2, 3, 1)
-    return merge_first_wins(f, m, th, multiH)
+    f, m = _compose_all(flow, param, match, int(np.shape(flow)[2]) * 8, int(np.shape(flow)[3]) * 8)
+    return merge_first_wins(f, m.permute(0, 2, 3, 1), th, multiH)
 
 
 def getFlow_all(flow, param, match, outH, outW, th=0.95, multiH=True, with_match21=False):
     """evaluation/evalHpatch/getResults.py:16-63 on device tensors: flow (nH,2,h8,w8), param (nH,3,3),
     match (nH,2,h8,w8) -> flowGlobal (1,outH,outW,2).  The reference runs this on CPU tensors; the
     composition here is the fused kernel, the first-hypothesis-wins merge is elementwise torch."""
-    flow = torch.as_tensor(flow, dtype=torch.float32).cuda()
-    param = torch.as_tensor(param, dtype=torch.float32).cuda()
-    match = torch.as_tensor(match, dtype=torch.float32).cuda()
-    coarse = ops.warp_grid(param, outH, outW)
-    fl, ms = [], []
-    for i in range(flow.shape[0]):
-        f12, m, _ = ops.compose_fine(flow[i:i + 1], match[i:i + 1, 0:1], match[i:i + 1, 1:2] if with_match21 else None,
-                                     coarse[i:i + 1], clamp=True)
-        fl.append(f12)
-        ms.append(m)
-    f = torch.clamp(torch.cat(fl, dim=0), min=-1, max=1)
-    m = torch.cat(ms, dim=0).permute(0, 2, 3, 1)
-    flowGlobal = f[:1].clone()
-    if multiH:
-        mb = m[:1] >= th
-        for i in range(1, len(m)):
-            tmp = (m.narrow(0, i, 1) >= th) * (~mb)
-            mb = mb + tmp
-            tmp = tmp.expand_as(flowGlobal)
-            flowGlobal[tmp] = f.narrow(0, i, 1)[tmp]
-    return flowGlobal
+    f, m = _compose_all(flow, param, match, outH, outW, with_match21)
+    if not multiH:
+        return f[:1].clone()
+    return _merge(f, m.permute(0, 2, 3, 1), th, True, False)[0]
 
 
 # evalYFCC's pair from CUDA graphs (its kernel entries live with it, in yfcc_graph)

@@ -153,10 +153,7 @@ def _search_device(c, Is_u8, It_u8, maxCoarse, It_bg=None, segNet=False, samples
     bgs, found = [], []
     for k in range(4):
         c._select_target(k)
-        bg, Mt = None, None
-        if It_bg is not None:
-            bg = pipeline.yfcc_background(It_bg, k, c.rotated_target_size(k))
-            Mt = ((1 - bg) > 0.5).float()
+        bg, Mt = pipeline._rotation_mask(It_bg, k, c.rotated_target_size(k))
         m1, m2, _, cnt = c._match_device(Mt)
         _, _, mask, status = draws.call(k).ransac(m1, m2, cnt, c.tolerance, 100)
         bgs.append(bg)

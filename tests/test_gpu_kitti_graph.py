@@ -160,7 +160,7 @@ def assert_same_pair(eager, dev, size):
 def device_pair(rf, c, net, src, tgt, fineSize, th, maxH):
     """``align_pair_kitti_graph``'s own steps, keeping the raw records: (its dict, how the loop ended)."""
     P = rf.pipeline
-    packed, maps, size, shapes = P._kitti_device(c, net, torch.from_numpy(src).cuda(), torch.from_numpy(tgt).cuda(), fineSize, 0.01, th, maxH)
+    packed, maps, size, shapes, _ = P._kitti_device(c, net, torch.from_numpy(src).cuda(), torch.from_numpy(tgt).cuda(), fineSize, 0.01, th, maxH)
     host = P._to_host(packed).copy()
     out = P._unpack_kitti(host.copy(), maps, size, shapes, maxH)
     n = len(out["H"])
