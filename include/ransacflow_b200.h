@@ -320,6 +320,21 @@ int rf_affine_sample_u8(const float* theta, const uint8_t* src, int Hin, int Win
 int rf_val_keypoints(const float* flowDown8, int h8, int w8, const float* theta, int H, int W, int wA, int hA, const int* kpts,
                      const int* count, int capacity, int pair, const double* thresholds_host, int T, unsigned long long* counts,
                      int* err, double* dist_out, float* flow_out, void* stream);
+/* evaluation/evalCorr/getResults.py:78-134 (getFlow, or getFlow_Coarse with onlyCoarse) + :220-227 + alignmentError (:15-38) at
+ * the keypoints only, for one pair: flowDown8 / matchDown8 [nH][2][h8][w8] and H [nH][9] fp32 in DEVICE memory (the flows
+ * and matchabilities may be NULL with onlyCoarse), composed at 8h8 x 8w8; kpts [capacity][4] int32 (xa, ya, xb, yb), *count
+ * (DEVICE) of them used; Ith x Itw the target's size, wA x hA the source's.  th: the merge threshold (float32), multiH: merge
+ * all hypotheses, else hypothesis 0 alone.  thresholds_host [T] pixel thresholds (<=); mth_host [J] the matchability thresholds
+ * th_j in order and slot_host [J] their accumulator rows.  counts [rows][T + 1] uint64 (DEVICE) accumulate, per row, the
+ * keypoints within each pixel threshold and the keypoints scored; an index outside numpy's [-n, n) range sets
+ * *err = min(*err, pair).  Optional (NULL) per-keypoint outputs: flow_out [capacity][2] and match_out [capacity] the merged flow
+ * and matchability at (yb, xb), hyp_out [capacity] the winning hypothesis, dist_out [capacity][J] the fp64 distance per th_j
+ * (NaN where the keypoint is not selected).  For th_j > 0 the map must be square (see DESIGN.md section 12). */
+int rf_corr_keypoints(const float* flowDown8, const float* matchDown8, const float* H, int nH, int h8, int w8, int Ith, int Itw,
+                      int wA, int hA, const int* kpts, const int* count, int capacity, int pair, float th, int multiH, int onlyCoarse,
+                      const double* thresholds_host, int T, const double* mth_host, const int* slot_host, int J,
+                      unsigned long long* counts, int* err, float* flow_out, float* match_out, int* hyp_out, double* dist_out,
+                      void* stream);
 /* F.interpolate(mode='bilinear', align_corners=False): NCHW [NC][h][w] -> [NC][H][W] */
 int rf_upsample_bilinear(const float* in, int NC, int h, int w, int H, int W, float* out, void* stream);
 /* PredFlowMask tail, evaluation/evalHpatch/evaluation.py:37-51 fused:

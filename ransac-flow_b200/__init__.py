@@ -17,9 +17,10 @@ __version__ = "0.1.0"
 
 
 def __getattr__(name):
-    """``validation`` (train/validation.py on the device) is imported on first use, so that ``python -m
-    ransac_flow_b200.validation`` runs the module once, as ``__main__``, instead of after a package-level import of it."""
-    if name == "validation":
+    """``validation`` (train/validation.py on the device) and ``corr_results`` (evalCorr/getResults.py on the device) are
+    imported on first use, so that ``python -m ransac_flow_b200.validation`` (``.corr_results``) runs the module once, as
+    ``__main__``, instead of after a package-level import of it."""
+    if name in ("validation", "corr_results"):
         import importlib
-        return importlib.import_module(".validation", __name__)
+        return importlib.import_module("." + name, __name__)
     raise AttributeError("module %r has no attribute %r" % (__name__, name))

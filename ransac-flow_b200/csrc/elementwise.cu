@@ -630,10 +630,22 @@ __device__ __forceinline__ float lin11(int i, int n) {
     float step = 2.f / (float)(n - 1);
     return (i < n / 2) ? (-1.f + step * (float)i) : (1.f - step * (float)(n - 1 - i));
 }
+// lin11 with both branches written as the single FMA the compiler makes of each in warp_grid_kernel and
+// compose_fine_kernel (their SASS: FFMA step, i, -1 and FFMA -step, n - 1 - i, 1), for code that must reproduce those
+// kernels' values wherever it is compiled
+__device__ __forceinline__ float lin11_fma(int i, int n) {
+    if (n == 1) return -1.f;
+    float step = 2.f / (float)(n - 1);
+    return (i < n / 2) ? __fmaf_rn(step, (float)i, -1.f) : __fmaf_rn(-step, (float)(n - 1 - i), 1.f);
+}
+struct Lin11 { __device__ float operator()(int i, int n) const { return lin11(i, n); } };
+struct Lin11Fma { __device__ float operator()(int i, int n) const { return lin11_fma(i, n); } };
 
-// the grid point of output pixel (r, c) of an h x w homography grid (H: 9 floats), one rounding per operation
-__device__ __forceinline__ float2 homography_grid_point(const float* __restrict__ H, int r, int c, int h, int w) {
-    float x = lin11(c, w), y = lin11(r, h);
+// the grid point of output pixel (r, c) of an h x w homography grid (H: 9 floats), one rounding per operation; lin: the
+// linspace (lin11 in warp_grid_kernel, lin11_fma where another kernel computes the same points in place)
+template <typename Lin = Lin11>
+__device__ __forceinline__ float2 homography_grid_point(const float* __restrict__ H, int r, int c, int h, int w, Lin lin = Lin()) {
+    float x = lin(c, w), y = lin(r, h);
     float px = __fadd_rn(__fadd_rn(__fmul_rn(H[0], x), __fmul_rn(H[1], y)), H[2]);
     float py = __fadd_rn(__fadd_rn(__fmul_rn(H[3], x), __fmul_rn(H[4], y)), H[5]);
     float pz = __fadd_rn(__fadd_rn(__fmul_rn(H[6], x), __fmul_rn(H[7], y)), H[8]);
@@ -781,6 +793,47 @@ __device__ __forceinline__ float up_sample(const float* __restrict__ p, int h, i
     return up_blend(__ldg(p + y0 * w + x0), __ldg(p + y0 * w + x1), __ldg(p + y1 * w + x0), __ldg(p + y1 * w + x1), ly0, ly1, lx0, lx1);
 }
 
+// up_sample with every rounding written out, as compose_fine_kernel's compiled code performs it (its PTX): the source
+// coordinate one FMA, each row of the blend one product and one FMA, the rows' blend fma(ly0, row0, ly1 * row1).  The
+// compiler picks, per call site there, which product of a row it folds into the FMA: A0 / B0 fold lx1 * v01 / lx1 * v11,
+// A1 / B1 fold lx0 * v00 / lx0 * v10.
+template <int A, int B>
+__device__ __forceinline__ float up_sample_rn(const float* __restrict__ p, int h, int w, int H, int W, int Y, int X) {
+    auto coord = [](int dst, int in_size, int out_size, int& i0, int& i1, float& l0, float& l1) {
+        float src = __fmaf_rn(__fdiv_rn((float)in_size, (float)out_size), __fadd_rn((float)dst, 0.5f), -0.5f);
+        if (src < 0.f) src = 0.f;
+        i0 = (int)src;
+        i1 = i0 + ((i0 < in_size - 1) ? 1 : 0);
+        l1 = __fsub_rn(src, (float)i0);
+        l0 = __fsub_rn(1.f, l1);
+    };
+    int y0, y1, x0, x1;
+    float ly0, ly1, lx0, lx1;
+    coord(Y, h, H, y0, y1, ly0, ly1);
+    coord(X, w, W, x0, x1, lx0, lx1);
+    const float v00 = __ldg(p + y0 * w + x0), v01 = __ldg(p + y0 * w + x1), v10 = __ldg(p + y1 * w + x0), v11 = __ldg(p + y1 * w + x1);
+    const float r0 = A == 0 ? __fmaf_rn(lx1, v01, __fmul_rn(lx0, v00)) : __fmaf_rn(lx0, v00, __fmul_rn(lx1, v01));
+    const float r1 = B == 0 ? __fmaf_rn(lx1, v11, __fmul_rn(lx0, v10)) : __fmaf_rn(lx0, v10, __fmul_rn(lx1, v11));
+    return __fmaf_rn(ly0, r0, __fmul_rn(ly1, r1));
+}
+// which upsampling compose_fine_pixel asks for
+enum { UP_FLOW_X = 0, UP_FLOW_Y = 1, UP_M21 = 2, UP_M12 = 3 };
+struct UpSample {
+    __device__ float operator()(int, const float* __restrict__ p, int h, int w, int H, int W, int Y, int X) const {
+        return up_sample(p, h, w, H, W, Y, X);
+    }
+};
+// compose_fine_kernel's roundings per call site: flow x A0 B0, flow y A1 B1, match21 A0 B1, match12 A1 B1
+struct UpSampleRn {
+    __device__ float operator()(int which, const float* __restrict__ p, int h, int w, int H, int W, int Y, int X) const {
+        switch (which) {
+        case UP_FLOW_X: return up_sample_rn<0, 0>(p, h, w, H, W, Y, X);
+        case UP_M21: return up_sample_rn<0, 1>(p, h, w, H, W, Y, X);
+        default: return up_sample_rn<1, 1>(p, h, w, H, W, Y, X);
+        }
+    }
+};
+
 __global__ void upsample_kernel(const float* __restrict__ in, int NC, int h, int w, int H, int W, float* __restrict__ out) {
     long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     long long HW = (long long)H * W;
@@ -860,20 +913,28 @@ __global__ void __launch_bounds__(256) val_keypoints_kernel(const float* __restr
 // evaluation/evalHpatch/evaluation.py:37-51 (and evalCorr :50-55) in one pass over the full-res grid.  The coarse grid
 // may have its own size (Hc, Wc) != (H, W): evaluation/evalKITTI/evaluation.py:296-299 samples the flow of the resized
 // image at the original image's positions, and evalKITTI/getResults.py:104-113 composes two levels that way.
-__global__ void compose_fine_kernel(const float* __restrict__ flow8, const float* __restrict__ m12, const float* __restrict__ m21,
-                                    int h8, int w8, const float* __restrict__ coarse, int Hc, int Wc, int H, int W, int clamp, int align_corners,
-                                    float* __restrict__ flow12, float* __restrict__ match, float* __restrict__ flowUp_out) {
-    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= (long long)H * W) return;
-    int Y = (int)(t / W), X = (int)(t - (long long)Y * W);
-    float fx = up_sample(flow8, h8, w8, H, W, Y, X) + lin11(X, W);
-    float fy = up_sample(flow8 + h8 * w8, h8, w8, H, W, Y, X) + lin11(Y, H);
+// The per-pixel body of compose_fine_kernel at output pixel (Y, X), shared with corr_keypoints_kernel: flowUp = the x8
+// upsampled flow + the grid (clamped when ``clamp``), the composed flow = grid_sample(coarse, flowUp), and with ``want_match``
+// the matchability interp(match12) [* grid_sample(interp(match21), flowUp)] * inside(composed flow).  coarse(y, x) returns
+// point (y, x) of the Hc x Wc coarse grid: a load of the stored grid, or the homography grid point computed in place.
+// emit_up(fx, fy) and emit_flow(ox, oy) receive flowUp and the composed flow as soon as each is known, so that a caller
+// storing them keeps compose_fine_kernel's order of stores.  grid(i, n) is the linspace the flow is added to and
+// up(which, ...) the x8 upsampling (UpSample / Lin11 in compose_fine_kernel; UpSampleRn / Lin11Fma, that kernel's roundings
+// written out, where another kernel must reproduce its values).
+struct FinePixel { float fx, fy, ox, oy, m; };
+template <typename Coarse, typename EmitUp, typename EmitFlow, typename Grid, typename Up>
+__device__ __forceinline__ FinePixel compose_fine_pixel(const float* __restrict__ flow8, const float* __restrict__ m12,
+                                                        const float* __restrict__ m21, int h8, int w8, Coarse coarse, int Hc, int Wc,
+                                                        int H, int W, int Y, int X, int clamp, int align_corners, bool want_match,
+                                                        EmitUp emit_up, EmitFlow emit_flow, Grid grid, Up up) {
+    FinePixel r;
+    float fx = up(UP_FLOW_X, flow8, h8, w8, H, W, Y, X) + grid(X, W);
+    float fy = up(UP_FLOW_Y, flow8 + h8 * w8, h8, w8, H, W, Y, X) + grid(Y, H);
     if (clamp) {
         fx = fminf(fmaxf(fx, -1.f), 1.f);
         fy = fminf(fmaxf(fy, -1.f), 1.f);
     }
-    if (flowUp_out) reinterpret_cast<float2*>(flowUp_out)[t] = make_float2(fx, fy);
-    const float2* cg = reinterpret_cast<const float2*>(coarse);
+    emit_up(fx, fy);
     float ox = 0.f, oy = 0.f, mm = 0.f;
     {   // grid_sample(coarse, flowUp): bilinear, zero padding, in the coarse grid's own pixel coordinates
         float ix = unnormalize(fx, Wc, align_corners), iy = unnormalize(fy, Hc, align_corners);
@@ -882,10 +943,10 @@ __global__ void compose_fine_kernel(const float* __restrict__ flow8, const float
         float nw = (flx + 1.f - ix) * (fly + 1.f - iy), ne = (ix - flx) * (fly + 1.f - iy);
         float sw = (flx + 1.f - ix) * (iy - fly), se = (ix - flx) * (iy - fly);
         bool vx0 = x0 >= 0 && x0 < Wc, vx1 = x1 >= 0 && x1 < Wc, vy0 = y0 >= 0 && y0 < Hc, vy1 = y1 >= 0 && y1 < Hc;
-        if (vy0 && vx0) { float2 v = __ldg(cg + (long long)y0 * Wc + x0); ox += v.x * nw; oy += v.y * nw; }
-        if (vy0 && vx1) { float2 v = __ldg(cg + (long long)y0 * Wc + x1); ox += v.x * ne; oy += v.y * ne; }
-        if (vy1 && vx0) { float2 v = __ldg(cg + (long long)y1 * Wc + x0); ox += v.x * sw; oy += v.y * sw; }
-        if (vy1 && vx1) { float2 v = __ldg(cg + (long long)y1 * Wc + x1); ox += v.x * se; oy += v.y * se; }
+        if (vy0 && vx0) { float2 v = coarse(y0, x0); ox += v.x * nw; oy += v.y * nw; }
+        if (vy0 && vx1) { float2 v = coarse(y0, x1); ox += v.x * ne; oy += v.y * ne; }
+        if (vy1 && vx0) { float2 v = coarse(y1, x0); ox += v.x * sw; oy += v.y * sw; }
+        if (vy1 && vx1) { float2 v = coarse(y1, x1); ox += v.x * se; oy += v.y * se; }
     }
     if (m21) {   // grid_sample(interpolate(match21, (H, W)), flowUp): the sampled map lives on the OUTPUT grid
         float ix = unnormalize(fx, W, align_corners), iy = unnormalize(fy, H, align_corners);
@@ -894,18 +955,168 @@ __global__ void compose_fine_kernel(const float* __restrict__ flow8, const float
         float nw = (flx + 1.f - ix) * (fly + 1.f - iy), ne = (ix - flx) * (fly + 1.f - iy);
         float sw = (flx + 1.f - ix) * (iy - fly), se = (ix - flx) * (iy - fly);
         bool vx0 = x0 >= 0 && x0 < W, vx1 = x1 >= 0 && x1 < W, vy0 = y0 >= 0 && y0 < H, vy1 = y1 >= 0 && y1 < H;
-        if (vy0 && vx0) mm += up_sample(m21, h8, w8, H, W, y0, x0) * nw;
-        if (vy0 && vx1) mm += up_sample(m21, h8, w8, H, W, y0, x1) * ne;
-        if (vy1 && vx0) mm += up_sample(m21, h8, w8, H, W, y1, x0) * sw;
-        if (vy1 && vx1) mm += up_sample(m21, h8, w8, H, W, y1, x1) * se;
+        if (vy0 && vx0) mm += up(UP_M21, m21, h8, w8, H, W, y0, x0) * nw;
+        if (vy0 && vx1) mm += up(UP_M21, m21, h8, w8, H, W, y0, x1) * ne;
+        if (vy1 && vx0) mm += up(UP_M21, m21, h8, w8, H, W, y1, x0) * sw;
+        if (vy1 && vx1) mm += up(UP_M21, m21, h8, w8, H, W, y1, x1) * se;
     }
-    reinterpret_cast<float2*>(flow12)[t] = make_float2(ox, oy);
-    if (match) {
-        float m = up_sample(m12, h8, w8, H, W, Y, X);
+    emit_flow(ox, oy);
+    r.fx = fx; r.fy = fy; r.ox = ox; r.oy = oy; r.m = 0.f;
+    if (want_match) {
+        float m = up(UP_M12, m12, h8, w8, H, W, Y, X);
         if (m21) m *= mm;
         float inside = ((ox >= -1.f && ox <= 1.f) ? 1.f : 0.f) * ((oy >= -1.f && oy <= 1.f) ? 1.f : 0.f);
-        match[t] = m * inside;
+        r.m = m * inside;
     }
+    return r;
+}
+
+__global__ void compose_fine_kernel(const float* __restrict__ flow8, const float* __restrict__ m12, const float* __restrict__ m21,
+                                    int h8, int w8, const float* __restrict__ coarse, int Hc, int Wc, int H, int W, int clamp, int align_corners,
+                                    float* __restrict__ flow12, float* __restrict__ match, float* __restrict__ flowUp_out) {
+    long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)H * W) return;
+    int Y = (int)(t / W), X = (int)(t - (long long)Y * W);
+    const float2* cg = reinterpret_cast<const float2*>(coarse);
+    const FinePixel p = compose_fine_pixel(
+        flow8, m12, m21, h8, w8, [&](int y, int x) { return __ldg(cg + (long long)y * Wc + x); }, Hc, Wc, H, W, Y, X, clamp,
+        align_corners, match != nullptr,
+        [&](float fx, float fy) { if (flowUp_out) reinterpret_cast<float2*>(flowUp_out)[t] = make_float2(fx, fy); },
+        [&](float ox, float oy) { reinterpret_cast<float2*>(flow12)[t] = make_float2(ox, oy); }, Lin11(), UpSample());
+    if (match) match[t] = p.m;
+}
+
+// evaluation/evalCorr/getResults.py:78-134 (getFlow / getFlow_Coarse) and :220-227 + alignmentError (:15-38) at the annotated
+// keypoints only.  A pair's nH hypotheses: flowDown8 / matchDown8 (nH, 2, h8, w8) and H (nH, 9), composed onto the H x W =
+// 8h8 x 8w8 grid.  At one pixel, each hypothesis is compose_fine_pixel with its homography grid taps computed in place
+// (homography_grid_point on lin11_fma: warp_grid_kernel's values) and match21 sampled, the linspace and the upsampling
+// with compose_fine_kernel's roundings written out (Lin11Fma, UpSampleRn): left to the compiler, it contracts them
+// differently here, which moved a few keypoints' values by a few ulps, then torch.clamp (NaN kept); the
+// first-hypothesis-wins merge at th keeps the first hypothesis whose matchability is >= th (only hypothesis 0 without
+// multiH), else hypothesis 0.  onlyCoarse: hypothesis 0's homography grid point, unclamped, with matchability 1.
+#define RF_CORR_MAX_MTH 8
+struct CorrParams {
+    double t[RF_VAL_MAX_THRESHOLDS];   // the pixel thresholds, compared with <=
+    int T;
+    float mth[RF_CORR_MAX_MTH];        // the matchability thresholds th_j, as float32
+    int positive[RF_CORR_MAX_MTH];     // th_j > 0 (as the Python float): the binary map (match >= th_j) * inside, else ones
+    int slot[RF_CORR_MAX_MTH];         // the accumulator row of th_j (equal thresholds share one dict entry)
+    int J, S;                          // matchability thresholds, accumulator rows
+};
+struct MergedPixel { float fx, fy, m; int win; };
+
+// not inlined: the kernel calls it at up to three places (and in a loop), and inlining them all spills
+__device__ __noinline__ MergedPixel corr_merged_pixel(const float* __restrict__ flow8, const float* __restrict__ match8,
+                                                         const float* __restrict__ Hm, int nH, int h8, int w8, int H, int W, int Y,
+                                                         int X, float th, int multiH, int onlyCoarse) {
+    MergedPixel r{0.f, 0.f, 0.f, 0};
+    if (onlyCoarse) {
+        const float2 g = homography_grid_point(Hm, Y, X, H, W, Lin11Fma());
+        r.fx = g.x; r.fy = g.y; r.m = 1.f;
+        return r;
+    }
+    const long long plane = (long long)h8 * w8;
+    for (int i = 0; i < nH; ++i) {
+        const float* Hi = Hm + 9 * i;
+        const float* m8 = match8 + 2 * plane * i;
+        const FinePixel p = compose_fine_pixel(
+            flow8 + 2 * plane * i, m8, m8 + plane, h8, w8, [&](int y, int x) { return homography_grid_point(Hi, y, x, H, W, Lin11Fma()); },
+            H, W, H, W, Y, X, 1, 0, true, [](float, float) {}, [](float, float) {}, Lin11Fma(), UpSampleRn());
+        if (i == 0) { r.fx = clamp11_nan(p.ox); r.fy = clamp11_nan(p.oy); r.m = p.m; }
+        if (p.m >= th) {
+            if (i > 0) { r.fx = clamp11_nan(p.ox); r.fy = clamp11_nan(p.oy); r.m = p.m; r.win = i; }
+            break;
+        }
+        if (!multiH) break;
+    }
+    return r;
+}
+__device__ __forceinline__ bool inside11(float x, float y) { return x >= -1.f && x <= 1.f && y >= -1.f && y <= 1.f; }
+
+// Per keypoint (xa, ya, xb, yb), for each th_j in order: the binary value at [yb, xb] of the map in its own H x W shape
+// (numpy's index rule: a negative index wraps once, anything else records the pair in *err).  For th_j > 0 the reference
+// multiplies the (1, H, W, 1) threshold map by the inside map permuted to (1, 1, H, W); with H == W (the host raises the
+// broadcast's RuntimeError otherwise) that is an (H, H, H) map whose [yb, xb] is a row of H values: the keypoint is selected
+// once per inside pixel of row xb of the merged flow, weight = (match >= th_j) * that count.  A selected keypoint reads the
+// flow viewed as Ith x Itw (the target's size: the flat index yb * Itw + xb of the H x W map), estim = (flow + 1) * 0.5 *
+// (size - 1) in fp32, the distance to (xa, ya) in fp64, and adds its weight to each count whose threshold it is <= and to the
+// keypoints scored.  Block sums in shared memory, then one 64-bit atomic per counter per block.
+__global__ void __launch_bounds__(256) corr_keypoints_kernel(const float* __restrict__ flow8, const float* __restrict__ match8,
+                                                             const float* __restrict__ Hm, int nH, int h8, int w8, int Ith, int Itw,
+                                                             int wA, int hA, const int* __restrict__ kpts, const int* __restrict__ count,
+                                                             int capacity, int pair, float th, int multiH, int onlyCoarse,
+                                                             const __grid_constant__ CorrParams P, unsigned long long* __restrict__ counts,
+                                                             int* __restrict__ err, float* __restrict__ flow_out, float* __restrict__ match_out,
+                                                             int* __restrict__ hyp_out, double* __restrict__ dist_out) {
+    __shared__ unsigned int acc[RF_CORR_MAX_MTH * (RF_VAL_MAX_THRESHOLDS + 1)];
+    const int nacc = P.S * (P.T + 1);
+    for (int i = threadIdx.x; i < nacc; i += blockDim.x) acc[i] = 0u;
+    __syncthreads();
+    const int H = 8 * h8, W = 8 * w8;
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    const int n = min(__ldg(count), capacity);
+    const double qnan = __longlong_as_double(0x7ff8000000000000ll);
+    if (j < n) {
+        const int xa = __ldg(kpts + 4 * j), ya = __ldg(kpts + 4 * j + 1);
+        const int xb = __ldg(kpts + 4 * j + 2), yb = __ldg(kpts + 4 * j + 3);
+        const int my = yb < 0 ? yb + H : yb, mx = xb < 0 ? xb + W : xb;
+        if (my < 0 || my >= H || mx < 0 || mx >= W) {
+            atomicMin(err, pair);
+            if (dist_out) for (int q = 0; q < P.J; ++q) dist_out[(long long)j * P.J + q] = qnan;
+        } else {
+            const MergedPixel g = corr_merged_pixel(flow8, match8, Hm, nH, h8, w8, H, W, my, mx, th, multiH, onlyCoarse);
+            if (flow_out) reinterpret_cast<float2*>(flow_out)[j] = make_float2(g.fx, g.fy);
+            if (match_out) match_out[j] = g.m;
+            if (hyp_out) hyp_out[j] = g.win;
+            const int ey = yb < 0 ? yb + Ith : yb, ex = xb < 0 ? xb + Itw : xb;
+            const bool in_flow = ey >= 0 && ey < Ith && ex >= 0 && ex < Itw;
+            double dist = qnan;
+            bool have = false;
+            int row = -1;
+            for (int q = 0; q < P.J; ++q) {
+                unsigned int w = 1u;
+                if (P.positive[q]) {
+                    w = 0u;
+                    if (g.m >= P.mth[q]) {
+                        if (row < 0) {
+                            row = 0;
+                            for (int k = 0; k < W; ++k) {
+                                const MergedPixel e = corr_merged_pixel(flow8, match8, Hm, nH, h8, w8, H, W, mx, k, th, multiH, onlyCoarse);
+                                row += inside11(e.fx, e.fy) ? 1 : 0;
+                            }
+                        }
+                        w = (unsigned int)row;
+                    }
+                }
+                if (w && !in_flow) {
+                    atomicMin(err, pair);
+                    if (dist_out) for (int r = q; r < P.J; ++r) dist_out[(long long)j * P.J + r] = qnan;
+                    break;
+                }
+                if (w && !have) {
+                    MergedPixel e = g;
+                    const long long flat = (long long)ey * Itw + ex;
+                    const int fy = (int)(flat / W), fx = (int)(flat - (long long)fy * W);
+                    if (fy != my || fx != mx) e = corr_merged_pixel(flow8, match8, Hm, nH, h8, w8, H, W, fy, fx, th, multiH, onlyCoarse);
+                    const float exf = __fmul_rn(__fmul_rn(__fadd_rn(e.fx, 1.f), 0.5f), (float)(wA - 1));
+                    const float eyf = __fmul_rn(__fmul_rn(__fadd_rn(e.fy, 1.f), 0.5f), (float)(hA - 1));
+                    const double ddx = __dsub_rn((double)exf, (double)xa), ddy = __dsub_rn((double)eyf, (double)ya);
+                    dist = __dsqrt_rn(__dadd_rn(__dmul_rn(ddx, ddx), __dmul_rn(ddy, ddy)));
+                    have = true;
+                }
+                if (dist_out) dist_out[(long long)j * P.J + q] = w ? dist : qnan;
+                if (w) {
+                    unsigned int* a = acc + P.slot[q] * (P.T + 1);
+                    for (int t = 0; t < P.T; ++t)
+                        if (dist <= P.t[t]) atomicAdd(a + t, w);
+                    atomicAdd(a + P.T, w);
+                }
+            }
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < nacc; i += blockDim.x)
+        if (acc[i]) atomicAdd(counts + i, (unsigned long long)acc[i]);
 }
 
 // ---------------------------------------------------------------------------
@@ -1693,6 +1904,37 @@ extern "C" int rf_val_keypoints(const float* flowDown8, int h8, int w8, const fl
     th.n = T;
     val_keypoints_kernel<<<blocks_for(capacity, 256), 256, 0, as_stream(stream)>>>(flowDown8, h8, w8, theta, H, W, wA, hA, kpts, count, capacity,
                                                                                    pair, th, counts, err, dist_out, flow_out);
+    RF_LAUNCHED();
+    return 0;
+}
+
+extern "C" int rf_corr_keypoints(const float* flowDown8, const float* matchDown8, const float* H, int nH, int h8, int w8, int Ith,
+                                 int Itw, int wA, int hA, const int* kpts, const int* count, int capacity, int pair, float th, int multiH,
+                                 int onlyCoarse, const double* thresholds_host, int T, const double* mth_host, const int* slot_host,
+                                 int J, unsigned long long* counts, int* err, float* flow_out, float* match_out, int* hyp_out,
+                                 double* dist_out, void* stream) {
+    RF_REQUIRE(h8 > 0 && w8 > 0 && nH >= 1 && Ith > 0 && Itw > 0, "rf_corr_keypoints: empty flow, hypotheses or target");
+    RF_REQUIRE(T >= 1 && T <= RF_VAL_MAX_THRESHOLDS && thresholds_host, "rf_corr_keypoints: 1..16 pixel thresholds");
+    RF_REQUIRE(J >= 1 && J <= RF_CORR_MAX_MTH && mth_host && slot_host, "rf_corr_keypoints: 1..8 matchability thresholds");
+    RF_REQUIRE(counts && err && count && kpts && H, "rf_corr_keypoints: counts, error word, count, keypoints and H are required");
+    RF_REQUIRE(onlyCoarse || (flowDown8 && matchDown8), "rf_corr_keypoints: flowDown8 and matchDown8 are required");
+    RF_REQUIRE((long long)h8 * 8 * w8 * 8 < (1ll << 31) && (long long)Ith * Itw < (1ll << 31), "rf_corr_keypoints: map too large");
+    CorrParams P{};
+    for (int t = 0; t < T; ++t) P.t[t] = thresholds_host[t];
+    P.T = T;
+    P.S = 0;
+    for (int q = 0; q < J; ++q) {
+        RF_REQUIRE(slot_host[q] >= 0 && slot_host[q] < J, "rf_corr_keypoints: accumulator row out of range");
+        P.mth[q] = (float)mth_host[q];
+        P.positive[q] = mth_host[q] > 0.0;
+        P.slot[q] = slot_host[q];
+        P.S = max(P.S, slot_host[q] + 1);
+    }
+    P.J = J;
+    if (capacity <= 0) return 0;
+    corr_keypoints_kernel<<<blocks_for(capacity, 256), 256, 0, as_stream(stream)>>>(flowDown8, matchDown8, H, nH, h8, w8, Ith, Itw, wA, hA,
+                                                                                    kpts, count, capacity, pair, th, multiH, onlyCoarse, P,
+                                                                                    counts, err, flow_out, match_out, hyp_out, dist_out);
     RF_LAUNCHED();
     return 0;
 }

@@ -672,3 +672,53 @@ def imresize_mask(m, h, w, rot=0):
     byte-scaling (``rf_bytescale_mask_u8``), then PIL's BILINEAR passes (``rf_resample_u8``, skipped where a side keeps its
     size), then the comparison.  No host read: it can be captured in a CUDA graph once its resampling tables exist."""
     return imresize_keep(m, h, w, rot).float()
+
+
+# --------------------------------------------------------------------------- pinned staging (validation, corr_results)
+class _Staging:
+    """A ring of pinned host buffers, each uploaded with one asynchronous copy per pair and reused only once the event
+    recorded behind that copy has completed."""
+
+    def __init__(self, slots=3):
+        self.bufs = [None] * slots
+        self.events = [None] * slots
+        self.k = 0
+
+    def upload(self, parts, device):
+        """``parts``: numpy arrays; returns their bytes on ``device`` (one uint8 tensor) and each part's byte offset (16-byte
+        aligned)."""
+        offs, n = [], 0
+        for a in parts:
+            offs.append(n)
+            n += (a.nbytes + 15) // 16 * 16
+        k = self.k
+        self.k = (k + 1) % len(self.bufs)
+        if self.events[k] is not None and not self.events[k].query():
+            self.events[k].synchronize()                 # only when the GPU is this many pairs behind the host
+        if self.bufs[k] is None or self.bufs[k].numel() < n:
+            self.bufs[k] = torch.empty(max(n, 1 << 20), dtype=torch.uint8).pin_memory()
+        host = self.bufs[k].numpy()
+        for a, o in zip(parts, offs):
+            host[o:o + a.nbytes] = np.ascontiguousarray(a).reshape(-1).view(np.uint8)
+        dev = torch.empty(max(n, 16), dtype=torch.uint8, device=device)
+        dev[:n].copy_(self.bufs[k][:n], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(device))
+        self.events[k] = ev
+        return dev, offs
+
+
+_staging = {}
+
+
+def _staging_for(device):
+    d = torch.device(device).index
+    if d not in _staging:
+        _staging[d] = _Staging()
+    return _staging[d]
+
+
+def _view(dev, off, dtype, shape):
+    n = int(np.prod(shape)) * torch.empty(0, dtype=dtype).element_size()
+    return dev[off:off + n].view(dtype).view(shape)
+

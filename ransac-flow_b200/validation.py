@@ -28,7 +28,7 @@ import torch
 
 from . import model, ops
 from ._lib import check, lib, need_cuda, ptr, stream
-from .ops import Ragged
+from .ops import Ragged, _staging_for, _view
 
 MIN_SIZE, STRIDE_NET = 480, 16                                              # validation.py:60-61
 PIXEL_GRID = np.around(np.logspace(0, np.log10(36), 8).reshape(-1, 8))      # validation.py:64: [1, 2, 3, 5, 8, 13, 22, 36]
@@ -180,55 +180,6 @@ def read_counts(host):
     host = np.asarray(host, dtype=np.int64)
     err = int(host[-1:].view(np.int32)[0])
     return host[:-1], (None if err == NO_ERROR else err)
-
-
-# --------------------------------------------------------------------------- pinned staging
-class _Staging:
-    """A ring of pinned host buffers, each uploaded with one asynchronous copy per pair and reused only once the event
-    recorded behind that copy has completed."""
-
-    def __init__(self, slots=3):
-        self.bufs = [None] * slots
-        self.events = [None] * slots
-        self.k = 0
-
-    def upload(self, parts, device):
-        """``parts``: numpy arrays; returns their bytes on ``device`` (one uint8 tensor) and each part's byte offset (16-byte
-        aligned)."""
-        offs, n = [], 0
-        for a in parts:
-            offs.append(n)
-            n += (a.nbytes + 15) // 16 * 16
-        k = self.k
-        self.k = (k + 1) % len(self.bufs)
-        if self.events[k] is not None and not self.events[k].query():
-            self.events[k].synchronize()                 # only when the GPU is this many pairs behind the host
-        if self.bufs[k] is None or self.bufs[k].numel() < n:
-            self.bufs[k] = torch.empty(max(n, 1 << 20), dtype=torch.uint8).pin_memory()
-        host = self.bufs[k].numpy()
-        for a, o in zip(parts, offs):
-            host[o:o + a.nbytes] = np.ascontiguousarray(a).reshape(-1).view(np.uint8)
-        dev = torch.empty(max(n, 16), dtype=torch.uint8, device=device)
-        dev[:n].copy_(self.bufs[k][:n], non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(device))
-        self.events[k] = ev
-        return dev, offs
-
-
-_staging = {}
-
-
-def _staging_for(device):
-    d = torch.device(device).index
-    if d not in _staging:
-        _staging[d] = _Staging()
-    return _staging[d]
-
-
-def _view(dev, off, dtype, shape):
-    n = int(np.prod(shape)) * torch.empty(0, dtype=dtype).element_size()
-    return dev[off:off + n].view(dtype).view(shape)
 
 
 # --------------------------------------------------------------------------- the pair
