@@ -219,10 +219,13 @@ def sigmoid(x):
     return y
 
 
-def preproc_u8(img_u8, normalize):
-    """uint8 [P, 3] CUDA -> fp32 [P, 3] (ToTensor [+ Normalize])."""
-    need_cuda(img_u8)
-    out = torch.empty(img_u8.shape, device=img_u8.device, dtype=torch.float32)
+def preproc_u8(img_u8, normalize, out=None):
+    """uint8 [P, 3] CUDA -> fp32 [P, 3] (ToTensor [+ Normalize]), into ``out`` (contiguous fp32 [P, 3]) when given."""
+    need_cuda(img_u8, out)
+    if out is None:
+        out = torch.empty(img_u8.shape, device=img_u8.device, dtype=torch.float32)
+    elif out.dtype != torch.float32 or tuple(out.shape) != tuple(img_u8.shape) or not out.is_contiguous():
+        raise ValueError("preproc_u8: out must be a contiguous float32 %s tensor" % (tuple(img_u8.shape),))
     check(lib.rf_preproc_u8(ptr(img_u8), img_u8.shape[0], int(normalize), ptr(out), stream()))
     return out
 

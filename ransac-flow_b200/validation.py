@@ -6,7 +6,7 @@
                         float32 arrays, truncated later by ``int()``
   validate_pair       : validation.py:74-110 for one pair with nothing read back: the original uint8 images resized on the
                         device (``ops.resize_lanczos_u8``), ``rf_affine_sample_u8`` (affine_grid + ToTensor + grid_sample of the
-                        source, written into the source's half of the two-image batch) and ``rf_preproc_u8`` (the target's
+                        source, written into the source's half of the two-image batch) and ``ops.preproc_u8`` (the target's
                         half), the two-image fine features + ``l2norm``, the one volume ``CorrNeigh(featt, featsSample)``, the
                         ``NetFlowCoarse`` trunk + ``softmax_flow``, and ``rf_val_keypoints``: the x8 upsampling, the grid, the
                         clamp, the composition with the affine grid and ``alignmentError`` at the keypoints only
@@ -207,7 +207,7 @@ def validate_pair(network, Is_u8, It_u8, theta, kpts, counts, pair=0, dist_out=N
         P = ht * wt
         x = torch.empty((2 * P, 3), device=device, dtype=torch.float32)     # [IsSample ; ItTensor], NHWC rows
         affine_sample_u8(th, Isr, ht, wt, out=x[:P])
-        check(lib.rf_preproc_u8(ptr(Itr), P, 0, ptr(x[P:]), stream()))
+        ops.preproc_u8(Itr.view(P, 3), False, out=x[P:])
         f = network["netFeatCoarse"].forward_ragged(Ragged(x, [(ht, wt)] * 2))
         f = Ragged(ops.l2norm(f.data), f.hw)
         m = f.data.shape[0] // 2

@@ -1,8 +1,9 @@
 """Every kernel call outside the layer programs, checked on the operands the pipeline really gave it.
 
-A spy wraps the kernel entries of ``ransac_flow_b200.ops`` (the functions ``test_kernel_replay_inventory.INVENTORY`` marks
-"replayed here", plus ``imresize_keep``, which composes two of them) while real eager pairs run.  The pipeline modules call
-``ops.<name>`` through the module and ``ops`` calls its own helpers through its globals, so patching the module attributes
+A spy wraps the kernel entries of the package (the callables ``test_kernel_replay_inventory.INVENTORY`` marks "replayed
+here": those of ``ops``, ``validation.affine_sample_u8`` / ``val_keypoints``, ``corr_results.corr_keypoints`` and
+``train_pairs.warp_sample_u8``, plus ``ops.imresize_keep``, which composes two of them) while real eager pairs run.  The
+callers reach each entry through its module (``ops.<name>``, or the module's own globals), so patching the module attributes
 catches every call.  For each call the spy clones every tensor argument before the call and every result, plus the
 arguments the call writes in place, after it (on the current stream), and records the scalars, the strides and the data
 pointer alignment, which decide the kernel variant.  At most two calls are kept per (op, shapes, dtypes, scalars).  The
@@ -11,12 +12,21 @@ graphed paths are compared bit for bit with these eager ones elsewhere, so a cal
 Workloads (engine f16x3, correlation precision 2, unless noted): config 2 (``align_pair_single`` with match21 at 480 x 640,
 also on engines fp32 / precision 0 and tf32 / precision 1), config 3 (``getFlow_all`` at 240 on that pair's outputs), config 4
 (``align_pair_multi``, maxCoarse 3, with the segNet sky mask), config 5 (``align_pair_kitti_graph`` eagerly at 376 x 1241,
-then ``getFlow_all_kitti`` with the hole filling), YFCC (``align_pair_yfcc`` at 480 x 640 with a CUDA background) and
+then ``getFlow_all_kitti`` with the hole filling), YFCC (``align_pair_yfcc`` at 480 x 640 with a CUDA background),
 quick_start's ``align2images`` at 240 x 320 on engines tf32 and f16x3, the one path that runs the single CorrNeigh, the split
-one without its second volume, and the fine flow without clamp (with align_corners = True on tf32).
+one without its second volume, and the fine flow without clamp (with align_corners = True on tf32), and:
+  evalCorr        ``corr_results.score_pair`` on config 4's hypotheses (multiH, and onlyCoarse) and on a 480 x 480 pair
+                  with matchability thresholds (0, 0.5, 0.5): the row count of the broadcast, two thresholds on one row
+  training pair   ``align_train_pair`` (10 000 RANSAC iterations on the Philox stream) on a 480 x 720 source and a 512 x 640
+                  target, on engines f16x3 / precision 2 (presplit matching) and fp32 / precision 0
+  validation      ``validation.validate_pair`` on a 500 x 700 source and a 620 x 470 target with a non-identity theta and
+                  keypoints on the target's last row and column, wrapping and out of range, on engines f16x3 and tf32
 
 Each recorded output is then compared with a reference computed from that call's own recorded inputs, within the bound of
-the op's own unit test (named at each check).  Only the correlation is run again (``test_gpu_wgmma_edges.corr_call``), to read its arg-max keys.
+the op's own unit test (named at each check).  Only the correlation (``test_gpu_wgmma_edges.corr_call``, to read its arg-max
+keys) and the two keypoint kernels (into fresh accumulators, to read their per-keypoint outputs) are run again; the fused
+warp is also compared with the kernel composition it replaces, and the evalCorr keypoints with the dense device maps.  One
+test per check of the last four entries edits a copy of a recorded call and requires the check to fail on it.
 """
 import inspect
 
@@ -30,17 +40,24 @@ import ransac_ref as RR
 import wgmma_ref as R
 from oracle import synth
 from oracle import warp_oracle as WO
+from geometry_ref import bilinear_zeros, coord_delta, gamma, unnormalize64
+from test_gpu_corr_results import _binary, _dense
 from test_gpu_kitti_graph import numpy_step
 from test_gpu_ops import corr_neigh_ref
 from test_gpu_program_replay import _models
 from test_gpu_wgmma_edges import corr_call
 from test_gpu_ransac_exact import check_certified, kernel_provider
+from test_gpu_train_pairs import composition
+from test_gpu_validation import _network, affine_image, tail_ref
 from test_kernel_replay_inventory import INVENTORY, REPLAYED
+from train_pair_ref import decided, warp_u8_ref
 
 pytestmark = pytest.mark.gpu
 
-SPIED = sorted(n for n, w in INVENTORY.items() if w == REPLAYED) + ["imresize_keep"]
-IN_PLACE = {"remove_small_cc": ("match",), "kitti_region_step": ("Mask", "fgMask", "alive", "rec")}
+SPIED = dict(tuple(k.split(".", 1)[::-1]) for k, w in INVENTORY.items() if w == REPLAYED)      # entry name -> its module
+SPIED["imresize_keep"] = "ops"
+IN_PLACE = {"remove_small_cc": ("match",), "kitti_region_step": ("Mask", "fgMask", "alive", "rec"), "val_keypoints": ("counts",),
+            "corr_keypoints": ("counts", "err")}
 KEEP = 2
 
 
@@ -68,12 +85,13 @@ def _key_part(v):
 
 
 class Recorder:
-    def __init__(self, ops):
-        self.ops, self.real, self.calls, self.counts = ops, {}, {}, {}
+    def __init__(self, rf):
+        self.rf, self.real, self.calls, self.counts = rf, {}, {}, {}
         self.where = "?"
 
     def wrap(self, name):
-        fn = getattr(self.ops, name)
+        mod = getattr(self.rf, SPIED[name])
+        fn = getattr(mod, name)
         sig = inspect.signature(fn)
         rec = self
 
@@ -92,8 +110,8 @@ class Recorder:
                 rec.calls.setdefault(name, []).append(dict(args=before, after=after, out=_snap(out), where=rec.where))
             return out
 
-        self.real[name] = fn
-        setattr(self.ops, name, spy)
+        self.real[name] = (mod, fn)
+        setattr(mod, name, spy)
 
     def __enter__(self):
         for n in SPIED:
@@ -101,8 +119,8 @@ class Recorder:
         return self
 
     def __exit__(self, *exc):
-        for n, fn in self.real.items():
-            setattr(self.ops, n, fn)
+        for n, (mod, fn) in self.real.items():
+            setattr(mod, n, fn)
 
 
 def _segnet_class(rf, sds, img):
@@ -114,10 +132,73 @@ def _segnet_class(rf, sds, img):
     return min(ok)[1] if ok else int(ids[0])
 
 
+TH_CANDIDATES = (0.95, 0.9, 0.8, 0.6, 0.4, 0.2, 0.1)
+
+
+def _score(rf, out, seed, mth, later=False, onlyCoarse=False):
+    """``corr_results.score_pair`` on one aligned pair (the target's size is the flow's) with 400 synthetic keypoints: (xb, yb)
+    in [-W, W) x [-H, H), the corners, -1 and -W / -H, one column out of range; (xa, ya) the merged flow's estimate plus
+    noise, so that the distances fall on both sides of the thresholds.  ``later``: th is the first of TH_CANDIDATES at
+    which a later hypothesis wins on 0.1 % of the map, a quarter of the keypoints lie where one does, and the kernel must
+    report such a winner."""
+    flow, Hs, match = out["flowDown8"], np.asarray(out["H"]).reshape(-1, 3, 3), out["matchDown8"]
+    H, W = flow.shape[2] * 8, flow.shape[3] * 8
+    rs = np.random.RandomState(seed)
+    n = 400
+    yb, xb = rs.randint(-H, H, n), rs.randint(-W, W, n)
+    yb[:8] = [H - 1, H - 1, 0, -1, -H, 0, H - 1, 5]
+    xb[:8] = [W - 1, 0, W - 1, -1, -W, -W, -1, W]
+    f, m = rf.pipeline._compose_all(flow, Hs, match, H, W)
+    th = 0.95
+    if later:
+        for th in TH_CANDIDATES:
+            won = (m[0, 0] < th) & (m[1:, 0] >= th).any(0)
+            if float(won.float().mean()) > 1e-3:
+                break
+        else:
+            raise AssertionError("no threshold in %s lets a later hypothesis win" % (TH_CANDIDATES,))
+        py, px = (v.cpu().numpy() for v in torch.nonzero(won, as_tuple=True))
+        pick = rs.choice(len(py), n // 4)
+        yb[8:8 + n // 4], xb[8:8 + n // 4] = py[pick], px[pick]
+    fg = rf.pipeline.merge_first_wins(f, m.permute(0, 2, 3, 1), th)[0][0].cpu().numpy()
+    e = np.nan_to_num(fg[yb % H, xb % W])
+    xa = (e[:, 0] + 1) * 0.5 * (W - 1) + rs.normal(0, 6, n)
+    ya = (e[:, 1] + 1) * 0.5 * (H - 1) + rs.normal(0, 6, n)
+    kpts = tuple(np.asarray(v, dtype=np.float32) for v in (xa, ya, xb, yb))
+    scores = rf.corr_results.CorrScores(mth, th, multiH=True, onlyCoarse=onlyCoarse)
+    ho = torch.full((n,), -1, dtype=torch.int32, device="cuda")
+    rf.corr_results.score_pair(out, kpts, ((W, H), (W, H)), scores, pair=3, hyp_out=ho)
+    if later:
+        assert bool((ho > 0).any()), "th %.2f: no keypoint takes a later hypothesis" % th
+
+
+def _validation_inputs(rf):
+    """A 500 x 700 source and a 620 x 470 target (resized to 480 x 672 and 624 x 480: other sizes, other aspect ratios), a
+    non-identity theta and int32 keypoints in the resized images: on the target's last column and last row, -1 and -W / -H
+    (which wrap), one row out of range; (xa, ya) near the affine estimate, so that the distances spread over the thresholds."""
+    V = rf.validation
+    Is, It = synth.make_pair(31, 500, 700)[0], synth.make_pair(32, 620, 470)[1]
+    theta = np.array([[1.02, 0.03, 0.02], [-0.02, 0.98, -0.03]], np.float32)
+    ws, hs = V.resize_min_resolution_size(700, 500)
+    wt, ht = V.resize_min_resolution_size(470, 620)
+    rs = np.random.RandomState(9)
+    n = 600
+    xb, yb = rs.randint(-wt, wt, n), rs.randint(-ht, ht, n)
+    xb[:40] = wt - 1
+    yb[40:80] = ht - 1
+    xb[80:90], yb[80:90] = -1, -1
+    xb[90], yb[90] = -wt, -ht
+    xb[91], yb[91] = 3, ht
+    gx, gy = (2 * (xb % wt) + 1) / wt - 1.0, (2 * (yb % ht) + 1) / ht - 1.0
+    xa = (theta[0, 0] * gx + theta[0, 1] * gy + theta[0, 2] + 1) * 0.5 * (ws - 1) + rs.normal(0, 8, n)
+    ya = (theta[1, 0] * gx + theta[1, 1] * gy + theta[1, 2] + 1) * 0.5 * (hs - 1) + rs.normal(0, 8, n)
+    return Is, It, theta, np.stack([np.trunc(xa), np.trunc(ya), xb, yb], 1).astype(np.int32)
+
+
 @pytest.fixture(scope="module")
 def recorded(rf):
     from ransac_flow_b200.segnet import SegNet
-    rec = Recorder(rf.ops)
+    rec = Recorder(rf)
     try:
         with rec:
             for engine, prec in (("f16x3", 2), ("fp32", 0), ("tf32", 1)):
@@ -154,7 +235,7 @@ def recorded(rf):
                                  verbose=False, segnet_state_dicts=sds)
             c4.device_preproc = True
             torch.manual_seed(1000)
-            rf.pipeline.align_pair_multi(c4, net, torch.from_numpy(s).cuda(), torch.from_numpy(t).cuda(), maxCoarse=3, segNet=True)
+            out4 = rf.pipeline.align_pair_multi(c4, net, torch.from_numpy(s).cuda(), torch.from_numpy(t).cuda(), maxCoarse=3, segNet=True)
             torch.cuda.synchronize()
             # config 5: the KITTI pair, then its recomposition with the hole filling
             c5, net5 = _models(rf, 5)
@@ -175,6 +256,37 @@ def recorded(rf):
             torch.manual_seed(1000)
             rf.pipeline.align_pair_yfcc(cy, net, Image.fromarray(s), Image.fromarray(t), maxCoarse=3, It_bg=sky)
             torch.cuda.synchronize()
+            # evalCorr: config 4's hypotheses, then a square pair with positive matchability thresholds
+            assert len(out4["H"]) >= 2, "config 4: %d hypotheses, the merge has nothing to choose from" % len(out4["H"])
+            rec.where = "evalCorr config 4"
+            _score(rf, out4, 40, (0,), later=True)
+            rec.where = "evalCorr config 4 onlyCoarse"
+            _score(rf, out4, 41, (0,), onlyCoarse=True)
+            s, t, _ = synth.make_pair(6, 480, 480)
+            rec.where = "evalCorr 480x480"
+            torch.manual_seed(1000)
+            sq = rf.pipeline.align_pair_multi(c4, net, torch.from_numpy(s).cuda(), torch.from_numpy(t).cuda(), maxCoarse=3)
+            assert len(sq["H"]) >= 1, "480 x 480: no hypothesis accepted"
+            _score(rf, sq, 42, (0, 0.5, 0.5))
+            torch.cuda.synchronize()
+            # the training-pair notebook on both matching branches, and MegaDepth validation on both CorrNeigh paths
+            s, t, _ = synth.make_pair(2, 480, 720)
+            t = np.asarray(Image.fromarray(t).resize((640, 512), Image.BILINEAR))
+            vs, vt, theta, vk = _validation_inputs(rf)
+            for engine, prec in (("f16x3", 2), ("fp32", 0)):
+                rf.model.set_engine(engine)
+                rf.outil.corr_precision = prec
+                rec.where = "training pair %s" % engine
+                model = rf.train_pairs.TrainPairModel(rsd, minSize=480)
+                torch.manual_seed(1000)
+                tp = rf.pipeline.align_train_pair(model, s, t)
+                assert tp["kept"] and tp["status"] == rf.outil.RF_RANSAC_OK, ("training pair not kept", engine, tp["status"], tp["nbMatch"])
+                torch.cuda.synchronize()
+            for engine in ("f16x3", "tf32"):
+                rf.model.set_engine(engine)
+                rec.where = "validation %s" % engine
+                rf.validation.validate_pair(_network(rf), vs, vt, theta, vk, rf.validation.new_counts(), pair=5)
+                torch.cuda.synchronize()
     finally:
         rf.model.set_engine("fp32")
         rf.outil.corr_precision = 0
@@ -585,20 +697,177 @@ def check_fill_nearest(rf, call):
     return 0.0, "%.3f matched, %d ties resolved otherwise than scipy" % (mn.mean(), len(other)), "%dx%d" % (H, W)
 
 
+# -- training pairs, validation, evalCorr
+def check_warp_sample(rf, call):
+    """Bit for bit against the composition it fuses (test_gpu_train_pairs.test_warp_sample_equals_its_composition), then
+    floor(255 v) of train_pair_ref.warp_u8_ref (fp64 at the kernel's fp32 grid) on every byte outside the truncation band
+    (test_warp_sample_vs_fp64)."""
+    a = call["args"]
+    H, src, h, w = T(a["H"]), T(a["src"]), int(a["h"]), int(a["w"])
+    assert not a["align_corners"], "the composition samples with align_corners = False"
+    got = T(call["out"])
+    want = composition(rf, H, src, h, w)
+    assert torch.equal(got, want), "%d bytes differ from the composition" % int((got != want).sum())
+    src_np, got = src.cpu().numpy(), got.cpu().numpy().astype(np.int64)
+    g32 = G.warp_grid_f32(H.cpu().numpy().reshape(1, 3, 3), h, w)[0]
+    v, _ = warp_u8_ref(None, src_np, h, w, grid=(g32[..., 0], g32[..., 1]))
+    _, allow, _ = G.grid_sample_ref((src_np.astype(np.float32) / np.float32(255)).transpose(2, 0, 1)[None], g32[None], False)
+    band = 255.0 * allow[0].transpose(1, 2, 0) + 2 * 255.0 * G.U * v
+    ok = decided(v, band)
+    off = got != np.floor(v).astype(np.int64)
+    assert not (off & ok).any(), "%d decided bytes differ from fp64's truncation" % int((off & ok).sum())
+    assert np.abs(got - np.floor(v)).max() <= 1
+    return 0.0, "%d of %d bytes in the truncation band, %d of them off by one" % (int((~ok).sum()), ok.size, int(off.sum())), \
+        "%dx%d -> %dx%d" % (src_np.shape[0], src_np.shape[1], h, w)
+
+
+def affine_ref(call):
+    """The recorded affine_sample_u8 output as (3, h, w) fp64 with test_gpu_validation.affine_image's fp64 sample and the
+    bound of test_affine_sample_fp64_and_torch."""
+    a = call["args"]
+    th, src, h, w = cpu(a["theta"]).reshape(2, 3), cpu(a["src"]), int(a["h"]), int(a["w"])
+    Hin, Win = src.shape[:2]
+    P, S = affine_image(th, h, w)
+    ix, iy = unnormalize64(P[0], Win, False), unnormalize64(P[1], Hin, False)
+    val, absval, Lx, Ly, _ = bilinear_zeros((src.astype(np.float32) / np.float32(255)).transpose(2, 0, 1), ix, iy)
+    allow = gamma(7) * absval + Lx * (coord_delta(ix) + Win / 2.0 * gamma(2) * S[0]) + Ly * (coord_delta(iy) + Hin / 2.0 * gamma(2) * S[1])
+    got = cpu(call["out"]).astype(np.float64).reshape(h, w, 3).transpose(2, 0, 1)
+    return got, val, allow
+
+
+def check_affine_sample(rf, call):
+    got, val, allow = affine_ref(call)
+    worst = G.check(got, val, allow, "affine_sample_u8")
+    a = call["args"]
+    return worst, "theta %s" % np.round(cpu(a["theta"]).astype(np.float64), 3).tolist(), "%s -> %dx%d" % (shape_of(a["src"]), a["h"], a["w"])
+
+
+def _err_word(v):
+    """The low 32 bits of the last int64 of an accumulator (or the int32 word itself), recorded or not."""
+    t = T(v) if isinstance(v, dict) else v
+    return int(np.ascontiguousarray(t.cpu().numpy().reshape(-1)[-1:]).view(np.int32)[0])
+
+
+def check_val_keypoints(rf, call):
+    """Run again into a fresh accumulator with dist_out / flow_out: the same count delta and error word as the recorded call;
+    the fine flow and each distance within test_gpu_validation.tail_ref's fp64 bounds (test_keypoint_tail_fp64); the counts
+    those of the fp64 distances except for keypoints within the bound of a threshold (set aside, at most 2 %, as
+    test_dataset_matches_the_reference's MAX_ASIDE); the error word holds ``pair`` exactly when torch's index rule rejects a
+    keypoint."""
+    V = rf.validation
+    a = call["args"]
+    kp, H, W, hA, wA = T(a["kpts"]), int(a["size_t"][0]), int(a["size_t"][1]), int(a["size_s"][0]), int(a["size_s"][1])
+    thr = np.asarray(a["thresholds"], dtype=np.float64).reshape(-1)
+    cap = kp.shape[0]
+    acc = torch.zeros_like(T(a["counts"]))
+    acc[-1] = V.NO_ERROR
+    d = torch.full((cap,), float("nan"), dtype=torch.float64, device="cuda")
+    fo = torch.full((cap, 4), float("nan"), device="cuda")
+    V.val_keypoints(T(a["flowDown8"]), T(a["theta"]), (H, W), (hA, wA), kp, T(a["count"]), acc, a["pair"], d, fo, a["thresholds"])
+    counts, _ = V.read_counts(acc.cpu().numpy())
+    delta = cpu(call["after"]["counts"])[:-1] - cpu(a["counts"])[:-1]
+    assert np.array_equal(delta, counts), ("count delta", delta.tolist(), counts.tolist())
+    n = min(int(cpu(a["count"])[0]), cap)
+    k = kp[:n].cpu().numpy().astype(np.int64)
+    ok = (k[:, 3] >= -H) & (k[:, 3] < H) & (k[:, 2] >= -W) & (k[:, 2] < W)
+    want_err = a["pair"] if not ok.all() else V.NO_ERROR
+    assert _err_word(acc) == want_err, ("re-run error word", _err_word(acc), want_err)
+    assert _err_word(call["after"]["counts"]) == min(_err_word(a["counts"]), want_err), "recorded error word"
+    dk, fk = d.cpu().numpy()[:n][ok], fo.cpu().numpy()[:n][ok]
+    fl, ef, dref, adist = tail_ref(cpu(a["flowDown8"]), cpu(a["theta"]), H, W, hA, wA, k[ok])
+    G.check(fk[:, :2], fl, ef, "val_keypoints fine flow")
+    worst = G.check(dk, dref, adist, "val_keypoints distance")
+    assert np.array_equal(counts[:-1], (dk[:, None] < thr).sum(0)) and counts[-1] == ok.sum(), "counts differ from dist_out's"
+    near = (np.abs(dref[:, None] - thr) <= adist[:, None]).any(1)
+    assert near.sum() <= 0.02 * len(dk), ("keypoints within the bound of a threshold", int(near.sum()), len(dk))
+    exp = (dref[~near, None] < thr).sum(0) + (dk[near, None] < thr).sum(0)
+    assert np.array_equal(counts[:-1], exp), ("counts differ from fp64's", counts.tolist(), exp.tolist())
+    ys, xs = k[ok, 3] % H, k[ok, 2] % W
+    return worst, "%d keypoints (%d on the last row / column, %d out of range, %d set aside), error word %s" % (
+        n, int(((ys == H - 1) | (xs == W - 1)).sum()), int((~ok).sum()), int(near.sum()),
+        "pair %d" % want_err if want_err != V.NO_ERROR else "untouched"), \
+        "flow %s target %dx%d source %dx%d" % (shape_of(a["flowDown8"]), H, W, hA, wA)
+
+
+def check_corr_keypoints(rf, call):
+    """Run again into fresh accumulators with flow_out / match_out / hyp_out / dist_out: the same count delta and error word
+    as the recorded call; the merged flow and matchability at each keypoint bit for bit against the dense device path
+    (test_gpu_corr_results.test_kernel_against_dense), each winning hypothesis against geometry_ref.compose_fine_ref
+    (test_composition_against_fp64), the counts equal to results.alignment_error on the dense maps, broadcast included."""
+    C = rf.corr_results
+    a = call["args"]
+    f8, kp = T(a["flowDown8"]), T(a["kpts"])
+    nH, _, h8, w8 = f8.shape
+    Hd, Wd = 8 * h8, 8 * w8
+    Ith, Itw, hA, wA = int(a["size_t"][0]), int(a["size_t"][1]), int(a["size_s"][0]), int(a["size_s"][1])
+    mth, slots = [float(t) for t in np.reshape(a["mth"], -1)], [int(q) for q in np.reshape(a["slots"], -1)]
+    th, multiH, onlyCoarse = a["th"], a["multiH"], a["onlyCoarse"]
+    pg = np.asarray(a["thresholds"], dtype=np.float64)
+    nT, J, cap = pg.size, len(mth), kp.shape[0]
+    acc, err = torch.zeros_like(T(a["counts"])), torch.full((1,), C.NO_ERROR, dtype=torch.int32, device="cuda")
+    fo, mo = torch.full((cap, 2), float("nan"), device="cuda"), torch.full((cap,), float("nan"), device="cuda")
+    ho, do = torch.full((cap,), -1, dtype=torch.int32, device="cuda"), torch.full((cap, J), float("nan"), dtype=torch.float64, device="cuda")
+    m8 = T(a["matchDown8"]) if a["matchDown8"] is not None else None
+    C.corr_keypoints(f8, m8, T(a["H"]), (Ith, Itw), (hA, wA), kp, T(a["count"]), acc, err, a["thresholds"], mth, slots, th, multiH,
+                     onlyCoarse, a["pair"], fo, mo, ho, do)
+    rows = (max(slots) + 1) * (nT + 1)
+    counts = acc.cpu().numpy()[:rows]
+    delta = cpu(call["after"]["counts"]).reshape(-1)[:rows] - cpu(a["counts"]).reshape(-1)[:rows]
+    assert np.array_equal(delta, counts), ("count delta", delta.tolist(), counts.tolist())
+    n = min(int(cpu(a["count"])[0]), cap)
+    k = kp[:n].cpu().numpy().astype(np.int64)
+    inside = lambda h, w: (k[:, 3] >= -h) & (k[:, 3] < h) & (k[:, 2] >= -w) & (k[:, 2] < w)
+    ok, okt = inside(Hd, Wd), inside(Ith, Itw)
+    assert not (ok & ~okt).any(), "keypoints on the map but outside the target's view: a case this check does not cover"
+    want_err = a["pair"] if not ok.all() else C.NO_ERROR
+    assert _err_word(err) == want_err, ("re-run error word", _err_word(err), want_err)
+    assert _err_word(call["after"]["err"]) == min(_err_word(a["err"]), want_err), "recorded error word"
+    flow, Hs = f8.cpu().numpy(), T(a["H"]).cpu().numpy().reshape(-1, 3, 3)
+    match = m8.cpu().numpy() if m8 is not None else None
+    fg, mg = _dense(Hs, flow, match, multiH, th, onlyCoarse)
+    ys, xs = k[ok, 3] % Hd, k[ok, 2] % Wd
+    fk, mk, hk = fo.cpu().numpy()[:n][ok], mo.cpu().numpy()[:n][ok], ho.cpu().numpy()[:n][ok]
+    assert np.array_equal(fk.view(np.int32), fg[0].cpu().numpy()[ys, xs].view(np.int32)), "merged flow differs from the dense path"
+    assert np.array_equal(mk.view(np.int32), mg[0, ..., 0].cpu().numpy()[ys, xs].view(np.int32)), "matchability differs from the dense path"
+    worst = 0.0
+    if not onlyCoarse:
+        for i in np.unique(hk):
+            r = G.compose_fine_ref(flow[i], match[i, 0], match[i, 1], G.warp_grid_f32(Hs[i:i + 1], Hd, Wd)[0], Hd, Wd)
+            sel = hk == i
+            y, x = ys[sel], xs[sel]
+            worst = max(worst, G.check(fk[sel], np.clip(r["flow12"][y, x], -1, 1), r["a_flow12"][y, x], "flow12 of hypothesis %d" % i))
+            dd = r["decided"][y, x]
+            worst = max(worst, G.check(mk[sel][dd], (r["match"] * r["inside"])[y, x][dd], (r["a_match"] * r["inside"])[y, x][dd],
+                                       "match of hypothesis %d" % i))
+    kf = [k[ok, c].astype(np.float32) for c in range(4)]
+    cnt = counts.reshape(-1, nT + 1)
+    for s in range(max(slots) + 1):
+        exp_c, exp_n = np.zeros(nT), 0
+        for q in [q for q in range(J) if slots[q] == s]:
+            c, nb = rf.results.alignment_error(Itw, Ith, wA, hA, *kf, fg, _binary(fg, mg, mth[q]), pg)
+            exp_c, exp_n = exp_c + c, exp_n + nb
+        assert np.array_equal(cnt[s, :nT], exp_c) and cnt[s, nT] == exp_n, ("row %d" % s, cnt[s].tolist(), exp_c.tolist(), exp_n)
+    wins = np.bincount(hk, minlength=nH)
+    return worst, "nH %d%s th %.2f mth %s: winners %s, %d keypoints (%d out of range), scored %s, error word %s" % (
+        nH, " onlyCoarse" if onlyCoarse else "", th, mth, wins.tolist(), n, int((~ok).sum()), cnt[:, nT].tolist(),
+        "pair %d" % want_err if want_err != C.NO_ERROR else "untouched"), "map %dx%d target %dx%d" % (Hd, Wd, Ith, Itw)
+
+
 CHECKS = {"_resize_u8": check_resize, "bytescale_mask_u8": check_bytescale, "imresize_keep": check_imresize_keep, "preproc_u8": check_preproc,
           "l2norm": check_l2norm, "l2norm_planes": check_l2norm_planes, "corr_mutual_nn": check_corr_mutual_nn,
           "corr_mutual_nn_presplit": check_corr_mutual_nn_presplit, "build_matches": check_build_matches, "ransac_homography": check_ransac,
           "warp_grid": check_warp_grid, "grid_sample": check_grid_sample, "upsample_bilinear": check_upsample, "compose_fine": check_compose_fine,
           "corr_neigh": check_corr_neigh, "corr_neigh_pair": check_corr_neigh_pair, "corr_neigh_pair_split": check_corr_neigh_pair_split,
           "softmax_flow": check_softmax_flow, "sigmoid": check_sigmoid, "remove_small_cc": check_remove_small_cc,
-          "kitti_region_step": check_kitti_region_step, "fill_nearest_matched": check_fill_nearest}
+          "kitti_region_step": check_kitti_region_step, "fill_nearest_matched": check_fill_nearest, "warp_sample_u8": check_warp_sample,
+          "affine_sample_u8": check_affine_sample, "val_keypoints": check_val_keypoints, "corr_keypoints": check_corr_keypoints}
 
 
 def test_every_spied_op_has_a_check():
     assert set(CHECKS) == set(SPIED)
 
 
-@pytest.mark.parametrize("name", SPIED)
+@pytest.mark.parametrize("name", sorted(SPIED))
 def test_recorded_calls_vs_reference(rf, recorded, name):
     calls = recorded.get(name, [])
     assert calls, "%s: no call recorded; the workloads do not reach it" % name
@@ -611,3 +880,56 @@ def test_recorded_calls_vs_reference(rf, recorded, name):
         worst = max(worst, ratio)
         print("%s [%s] %s: %s, error / allowance %.3g" % (name, call["where"], shapes, variant, ratio))
     print("%s: %d recorded calls, worst error / allowance %.3g" % (name, len(calls), worst))
+
+
+# ------------------------------------------------------------------ each new check rejects a doctored record
+def _copy(v):
+    if isinstance(v, dict):
+        return {k: _copy(x) for k, x in v.items()}
+    if isinstance(v, list):
+        return [_copy(x) for x in v]
+    return v.clone() if isinstance(v, torch.Tensor) else v
+
+
+def _byte_up(rf, call):
+    t = T(call["out"]).view(-1)
+    t[int(torch.nonzero(t < 255)[0, 0])] += 1
+
+
+def _affine_off(rf, call):
+    _, _, allow = affine_ref(call)
+    c, y, x = np.unravel_index(int(np.argmax(allow)), allow.shape)
+    T(call["out"])[y * int(call["args"]["w"]) + x, c] += float(4 * allow[c, y, x])
+
+
+def _count_up(rf, call):
+    T(call["after"]["counts"]).view(-1)[0] += 1
+
+
+def _val_err_cleared(rf, call):
+    T(call["after"]["counts"])[-1] = rf.validation.NO_ERROR
+
+
+def _corr_err_cleared(rf, call):
+    T(call["after"]["err"])[0] = rf.corr_results.NO_ERROR
+
+
+DOCTORED = {"warp_sample_u8 byte": ("warp_sample_u8", _byte_up), "affine_sample_u8 element": ("affine_sample_u8", _affine_off),
+            "val_keypoints count": ("val_keypoints", _count_up), "val_keypoints error word": ("val_keypoints", _val_err_cleared),
+            "corr_keypoints count": ("corr_keypoints", _count_up), "corr_keypoints error word": ("corr_keypoints", _corr_err_cleared)}
+
+
+@pytest.mark.parametrize("case", sorted(DOCTORED))
+def test_check_rejects_a_doctored_record(rf, recorded, case):
+    """One recorded call, copied and edited on the host (an output byte + 1, an element moved by 4x its allowance, a count
+    + 1, the error word cleared), must fail its check; nothing is launched with altered arguments."""
+    name, doctor = DOCTORED[case]
+    calls = recorded[name]
+    if "error word" in case:
+        what = "counts" if name == "val_keypoints" else "err"
+        calls = [c for c in calls if _err_word(c["after"][what]) != getattr(rf, SPIED[name]).NO_ERROR]
+        assert calls, "%s: no recorded call sets the error word" % name
+    bad = _copy(calls[0])
+    doctor(rf, bad)
+    with pytest.raises(AssertionError):
+        CHECKS[name](rf, bad)

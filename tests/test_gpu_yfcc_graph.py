@@ -2,9 +2,7 @@
 select-copy kernels against numpy restatements, the slot chain against the eager draw-and-rewind sequence, whole pairs bit
 for bit against ``align_pair_yfcc`` under ``torch.manual_seed`` (every rotation, a square target, skipped draws, every way the
 loop ends, the TypeError, segNet, the driver's defaults), the oracle's samples, graph replays with eviction and lanes.
-Plus the kernel-entry inventory of ``yfcc_graph`` (no GPU)."""
-import inspect
-
+The kernel entries of ``yfcc_graph`` are assigned to these tests in tests/test_kernel_replay_inventory.py."""
 import numpy as np
 import PIL.Image as Image
 import pytest
@@ -15,22 +13,6 @@ from test_gpu_pair import networks
 from test_gpu_sky import segnet_sds
 
 gpu = pytest.mark.gpu
-
-# every yfcc_graph function that reaches the library, and the test here that checks it
-INVENTORY = {
-    "ransac_homography_drawn": "test_slot_chain_reads_the_eager_tables",
-    "rotation_select": "test_rotation_select_is_the_numpy_restatement",
-    "select_copy": "test_select_copy",
-}
-
-
-def test_inventory_names_every_kernel_entry(rf):
-    Y = rf.yfcc_graph
-    found = {name for name, fn in vars(Y).items()
-             if inspect.isfunction(fn) and fn.__module__ == Y.__name__ and "lib.rf_" in inspect.getsource(fn)}
-    assert found == set(INVENTORY), found
-    for name, test in INVENTORY.items():
-        assert callable(globals()[test]), (name, test)
 
 
 # ------------------------------------------------------------------ kernels
